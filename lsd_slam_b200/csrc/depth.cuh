@@ -498,14 +498,12 @@ __device__ __forceinline__ void observeStereo(const HypField& cur, const DepthCa
 
 __global__ void __launch_bounds__(OBS_THREADS) k_observe(HypField cur, DepthCam cam, DepthGlobals G,
                                                  const float* __restrict__ kfImage, const float4* __restrict__ kfGrad,
-                                                 const float* __restrict__ kfMaxGrad, const __grid_constant__ ObserveParams OPv,
-                                                 const ObserveParams* __restrict__ OPdev, const int* __restrict__ skip)
+                                                 const float* __restrict__ kfMaxGrad, const __grid_constant__ ObserveParams OPv)
 {
     __shared__ int sList[OBS_PIX_PER_CTA];
     __shared__ int sCount;
     pdlWait();                                       // launched early (programmatic dependent launch): wait for the tracking kernel
-    if (skip && *skip) return;                       // this frame's tracking diverged: no mapping (SlamSystem.cpp:948-967)
-    const ObserveParams* OP = OPdev ? OPdev : &OPv;
+    const ObserveParams* OP = &OPv;
     const int iw = cam.w - 6, ih = cam.h - 6;        // x in [3, w-3), y in [3, h-3)  (:118, :150)
     const int nInterior = iw * ih;
     if (threadIdx.x == 0) sCount = 0;
@@ -535,9 +533,8 @@ __global__ void __launch_bounds__(OBS_THREADS) k_observe(HypField cur, DepthCam 
 
 // regularizeDepthMapFillHoles, DepthMap.cpp:656-718.  dst = src + created hypotheses.
 __global__ void __launch_bounds__(256) k_fill_holes(HypField src, HypField dst, DepthCam cam, DepthGlobals G,
-                                                    const float* __restrict__ kfMaxGrad, const int* __restrict__ skip)
+                                                    const float* __restrict__ kfMaxGrad)
 {
-    if (skip && *skip) return;
     const int x = blockIdx.x * 32 + (threadIdx.x & 31);
     const int y = blockIdx.y * 8 + (threadIdx.x >> 5);
     if (x >= cam.w || y >= cam.h) return;
@@ -575,10 +572,8 @@ __global__ void __launch_bounds__(256) k_fill_holes(HypField src, HypField dst, 
 
 // regularizeDepthMapRow<removeOcclusions>, DepthMap.cpp:758-848.  dst = src with smoothed values / removals.
 template <bool removeOcclusions>
-__global__ void __launch_bounds__(256) k_regularize(HypField src, HypField dst, DepthCam cam, DepthGlobals G, int validityTH,
-                                                    const int* __restrict__ skip)
+__global__ void __launch_bounds__(256) k_regularize(HypField src, HypField dst, DepthCam cam, DepthGlobals G, int validityTH)
 {
-    if (skip && *skip) return;
     // 32x8 output pixels per CTA; the 36x12 neighbourhood (idepth, var, validity, valid) is staged once in
     // shared memory, so each hypothesis is fetched from L2 1.7x instead of 25x
     __shared__ float4 tile[12][36];
@@ -728,7 +723,6 @@ __global__ void __launch_bounds__(256) k_set_depth(HypField cur, float* __restri
 template <bool SETDEPTH>
 __global__ void __launch_bounds__(FR_THREADS) k_fill_regularize(HypField src, HypField dst, DepthCam cam, DepthGlobals G,
                                                                 const float* __restrict__ kfMaxGrad, int validityTH,
-                                                                const int* __restrict__ skip,
                                                                 PyrPtrs id, PyrPtrs var, double* __restrict__ partials,
                                                                 unsigned int* counter, double* __restrict__ statsOut)
 {
@@ -736,7 +730,6 @@ __global__ void __launch_bounds__(FR_THREADS) k_fill_regularize(HypField src, Hy
     __shared__ float4 sB[FR_TH + 4][FR_TW + 4];      // after fill:  same fields
     __shared__ unsigned char sCreated[FR_TH + 4][FR_TW + 4];
     pdlWait();                                       // launched early (programmatic dependent launch): wait for k_observe
-    if (skip && *skip) return;
     const int width = cam.w, height = cam.h;
     const int tilesX = (width + FR_TW - 1) / FR_TW;
     const int bx = blockIdx.x % tilesX, by = blockIdx.x / tilesX;
@@ -915,11 +908,9 @@ __global__ void __launch_bounds__(FR_THREADS) k_fill_regularize(HypField src, Hy
 // one 16x16 level-0 tile; the tracker imports the new depth right after every update, so the pyramid is always
 // needed and building it here saves a pass over the level-0 planes and a launch.
 __global__ void __launch_bounds__(256) k_set_depth_pyr(HypField cur, PyrPtrs id, PyrPtrs var, int w, int h,
-                                                       double* __restrict__ partials, unsigned int* counter, double* __restrict__ out,
-                                                       const int* __restrict__ skip)
+                                                       double* __restrict__ partials, unsigned int* counter, double* __restrict__ out)
 {
     __shared__ float2 s0[16][17], s1[8][9], s2[4][5], s3[2][3];
-    if (skip && *skip) return;
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
     const int tilesX = w >> 4;
     const int bx = blockIdx.x % tilesX, by = blockIdx.x / tilesX;

@@ -11,7 +11,6 @@
 //     plus the int32 validity integral image.
 #pragma once
 
-#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -51,7 +50,6 @@ struct FrameSlot {
     float* reactVar = nullptr;
     uint8_t* reactValidity = nullptr;
     bool reactAllocated = false, reactValid = false;
-    CUtensorMap gradMap[LSD_LEVELS];     // TMA descriptors of grad[l] (float4 texels as 4 x f32), box = tracker window
     bool hasDepth = false, idepthPyrValid = false, hasGoodMask = false;
     bool depthHasBeenUpdatedFlag = false;
     float meanIdepth = 1.f;
@@ -95,11 +93,6 @@ struct ObserveParams {
     int kfNumTracked, kfNumMapped;
 };
 
-// per-warp shared-memory window of the new frame's gradient level used by the persistent tracker: WIN_W x WIN_H
-// float4 texels, loaded by one TMA box copy per warp and level (track_persistent.cuh)
-#define TRK_WIN_W 48
-#define TRK_WIN_H 17
-
 // number of reduction channels of one tracker evaluation (see track.cuh)
 #define EV_NCH 40
 
@@ -139,10 +132,8 @@ struct lsdgpu_ctx {
     unsigned int* evCounter = nullptr;
     float* dEvOut = nullptr;             // EV_NCH floats (device)
     float* hEvOut = nullptr;             // pinned host mirror
-    void* dTrackState = nullptr;         // persistent-kernel state block (device)
-    void* hTrackState = nullptr;         // mapped pinned result block (host view)
+    void* hTrackState = nullptr;         // mapped pinned result block of the persistent tracker (host view)
     void* dTrackStateMapped = nullptr;   // device view of the same block
-    int trackUseTma = 0;
     void* dPermaItems = nullptr;         // batched permaRef tracking: candidate descriptors / results (device)
     void* dPermaResults = nullptr;
     void* dSim3Items = nullptr;          // batched Sim3 tracking: problem descriptors / results (device)
@@ -155,24 +146,16 @@ struct lsdgpu_ctx {
     bool undistorterSet = false;
     uint32_t* dPacked = nullptr;         // keyframeMsg.pointcloud staging: w*h InputPointDense records (device)
     int trackGrid = 132;                 // launch shape of the persistent tracker (set by trackPersistentSetup): one CTA per SM
-    int trackG[LSD_LEVELS] = { 1, 1, 1, 1, 1 };          // CTAs taking part in the evaluations of each level
-    unsigned int* trkSync = nullptr;     // per-level barrier counters + level records of the persistent tracker (TP_SYNC_WORDS)
-    unsigned int trkBase[LSD_LEVELS] = { 0, 0, 0, 0, 0 };  // arrivals already counted on each level's counter (never reset)
-    unsigned int tmaTimeoutsSeen = 0;
+    unsigned int* trkSync = nullptr;     // barrier counters + cross-GPU exchange slots of the persistent tracker (TP_SYNC_WORDS)
+    unsigned int trkBase = 0;            // arrivals already counted on the grid barrier's counter (never reset)
     // one stream sharded over several GPUs (lsdgpu_peer_attach): every rank's arena mapped into this process
     int nRanks = 1, rank = 0;
     char* peerBase[8] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };
     unsigned int trkTailBase = 0;
-    // environment switches, read once at lsdgpu_create
-    int optTrackTma = 0, optSingleSync = 0;
-    bool optTrackDebug = false;
-    int optTrackKmax = 3;
-    bool optPdl = true;                  // LSDGPU_PDL=0: plain stream-ordered launches of the dependent kernels
+    bool optTrackDebug = false;          // LSDGPU_TRACK_DEBUG, read once at lsdgpu_create
     int2* seqTable = nullptr;            // seqsum.cuh: per-run maps of the sequential fp32 sum, [SEQ_NBIN][runs]
     unsigned char* seqFlags = nullptr;
     int* seqCounts = nullptr;
-    int* dSkipFlag = nullptr;            // device flag: the frame's tracking diverged -> its mapping kernels do nothing
-    ObserveParams* dObs = nullptr;       // device-resident observe parameters written by k_prepare_observe
     unsigned int trackSeq = 0;           // sequence number of the last tracking launch (TrackState::doneSeq)
     uint8_t* stageRing = nullptr;        // device prefetch ring of raw u8 frames (separate allocation)
     int stageEntries = 0;
@@ -191,7 +174,6 @@ struct lsdgpu_ctx {
     double trackKernelBytes = 0;
     bool profileTrackKernel = false;
     bool trackProfilePending = false;
-    void* encodeTiled = nullptr;         // cuTensorMapEncodeTiled, resolved through cudaGetDriverEntryPoint
 };
 
 struct CtxLock {
@@ -222,13 +204,13 @@ __device__ __forceinline__ void pdlWait()
     asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 template <typename... KArgs, typename... Args>
-static inline cudaError_t launchPDL(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, bool pdl, Args&&... args)
+static inline cudaError_t launchPDL(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args)
 {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
@@ -266,9 +248,8 @@ __device__ __forceinline__ float interpF(const float* __restrict__ mat, float x,
     return dxdy * __ldg(bp + 1 + width) + (dy - dxdy) * __ldg(bp + width) + (dx - dxdy) * __ldg(bp + 1) + (1 - dx - dy + dxdy) * __ldg(bp);
 }
 
-// Frame::prepareForStereoWith, DataStructures/Frame.cpp:295-317 (double -> float like the reference).  Host and
-// device: the same IEEE operations, so k_prepare_observe produces bit-identical constants on the GPU.
-LSD_HD void prepareStereoConsts(const float K[9], const double q[4], const double t[3], const double s, RefConst& rc)
+// Frame::prepareForStereoWith, DataStructures/Frame.cpp:295-317 (host, double -> float like the reference)
+static inline void prepareStereoConsts(const float K[9], const double q[4], const double t[3], const double s, RefConst& rc)
 {
     double qi[4] = { -q[0], -q[1], -q[2], q[3] };
     const double si = 1.0 / s;
@@ -293,37 +274,3 @@ LSD_HD void prepareStereoConsts(const float K[9], const double q[4], const doubl
     for (int i = 0; i < 9; i++) tR[i] = (float)R[i] * (float)s;       // thisToOther_R
     for (int i = 0; i < 3; i++) { rc.row0[i] = tR[i * 3 + 0]; rc.row1[i] = tR[i * 3 + 1]; rc.row2[i] = tR[i * 3 + 2]; }
 }
-
-// Device-side tail of SE3Tracker::trackFrame (SE3Tracker.cpp:473-485) + head of DepthMap::updateKeyframe
-// (DepthMap.cpp:1079-1105) for the frame that was just tracked on the active keyframe: turns the tracker's
-// device-resident result into the observe parameters, so that the mapping kernels can be enqueued behind the
-// tracking kernel without a host round trip.  Runs on the last thread of k_track_persistent.
-struct PrepareConsts {
-    float K[9];
-    int frameId, reactivated, kfNumTracked, kfNumMapped, W1, H1;
-    const float* image;
-    const uint8_t* goodMask;
-};
-__device__ __forceinline__ void devicePrepareObserve(const lsd::SE3<float>& T, int diverged, float lastResidual, float pointUsage,
-                                                     float goodCount, float badCount, const PrepareConsts& c,
-                                                     ObserveParams* __restrict__ OP, int* __restrict__ skip)
-{
-    *skip = diverged;
-    if (diverged) return;
-    const lsd::SE3<double> f2r = lsd::se3Cast<double>(lsd::se3Inverse(T));        // SE3Tracker.cpp:483-485
-    RefConst& rc = OP->refs[0];
-    prepareStereoConsts(c.K, f2r.q, f2r.t, 1.0, rc);
-    rc.initialTrackedResidual = lastResidual / pointUsage;                       // :482
-    rc.id = c.frameId;
-    rc.trackedOnActive = 1;
-    rc.image = c.image;
-    rc.goodMask = c.goodMask;
-    const bool trackingWasGood = goodCount / (c.W1 * c.H1) > 0.04f && goodCount / (goodCount + badCount) > 0.5f;   // :475-477
-    OP->nRefs = 1;
-    OP->byIdOffset = c.frameId; OP->byIdSize = 1; OP->byId[0] = 0;
-    OP->oldestIdx = 0; OP->newestIdx = 0;
-    OP->reactivated = c.reactivated;
-    OP->kfNumTracked = c.kfNumTracked + (trackingWasGood ? 1 : 0);               // :479-480
-    OP->kfNumMapped = c.kfNumMapped;
-}
-

@@ -92,7 +92,7 @@ extern "C" int lsdgpu_create(int device, int width, int height, const float K[9]
     const int maxBlocks = divUp((int)n0, EVAL_THREADS) + 8;
     size_t scratch = alignUp((size_t)maxBlocks * EV_NCH * 4 + 65536, 256) + 4096 + alignUp(sizeof(ObserveParams), 256)
                      + 2 * alignUp(n0, 256) + alignUp(n0 * 32, 256) + alignUp((size_t)maxBlocks * 2 * 8 + 64, 256) + (256 + 2 * alignUp((n0 >> 8) * 16, 256) + 2 * alignUp(n0 * 4, 256) + alignUp(n0, 256)) * (size_t)max_frames + alignUp(n0 * 12, 256) + alignUp(LSD_MAX_PERMA_BATCH * (sizeof(PermaItem) + sizeof(PermaResult)), 256) + 1024 + alignUp(S3_MAX_BATCH * sizeof(Sim3Item), 256) + alignUp(S3_MAX_BATCH * sizeof(Sim3Out), 256)
-                     + alignUp(sizeof(TrackState), 256) + alignUp(sizeof(ObserveParams), 256) + 8192 + TP_SYNC_WORDS * 4;
+                     + 7936 + TP_SYNC_WORDS * 4;
     const int seqRuns = divUp((int)n0, SEQ_RUN);
     scratch += alignUp((size_t)seqRuns * SEQ_NBIN * sizeof(int2), 256) + alignUp((size_t)seqRuns, 256) + alignUp((size_t)seqRuns * 4, 256);
     ctx->arenaBytes = perFrame * max_frames + depthBytes + scratch;
@@ -113,27 +113,6 @@ extern "C" int lsdgpu_create(int device, int width, int height, const float K[9]
         s.goodMask = (uint8_t*)take(n0 / 4);
         memset(s.thisToParent, 0, sizeof(s.thisToParent));
         s.thisToParent[3] = 1; s.thisToParent[7] = 1;
-    }
-    // TMA descriptors for the tracker's shared-memory windows (one per slot and level)
-    {
-        cudaDriverEntryPointQueryResult qres;
-        LSD_CHECK(ctx, cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ctx->encodeTiled, cudaEnableDefault, &qres));
-        if (qres != cudaDriverEntryPointSuccess || !ctx->encodeTiled) return lsd_fail(ctx, "cuTensorMapEncodeTiled not available in this driver");
-        typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-        EncodeFn enc = (EncodeFn)ctx->encodeTiled;
-        for (auto& s : ctx->slots)
-            for (int l = 0; l < LSD_LEVELS; l++) {
-                const cuuint64_t gdim[2] = { (cuuint64_t)4 * (width >> l), (cuuint64_t)(height >> l) };
-                const cuuint64_t gstr[1] = { (cuuint64_t)16 * (width >> l) };
-                const cuuint32_t box[2] = { 4 * TRK_WIN_W, TRK_WIN_H };
-                const cuuint32_t estr[2] = { 1, 1 };
-                CUresult cr = enc(&s.gradMap[l], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)s.grad[l], gdim, gstr, box, estr,
-                                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-                if (cr != CUDA_SUCCESS) return lsd_fail(ctx, "cuTensorMapEncodeTiled failed");
-            }
     }
     ctx->cur.hf = (float4*)take(n0 * 16); ctx->cur.hi = (int4*)take(n0 * 16);
     ctx->oth.hf = (float4*)take(n0 * 16); ctx->oth.hi = (int4*)take(n0 * 16);
@@ -162,9 +141,6 @@ extern "C" int lsdgpu_create(int device, int width, int height, const float K[9]
     ctx->dSim3Outs = take(S3_MAX_BATCH * sizeof(Sim3Out));
     ctx->dStageF = (float*)take(n0 * 32);
     ctx->dScalars = (double*)take((size_t)maxBlocks * 2 * 8 + 64);
-    ctx->dTrackState = take(sizeof(TrackState));
-    ctx->dObs = (ObserveParams*)take(sizeof(ObserveParams));
-    ctx->dSkipFlag = (int*)take(256);
     ctx->seqTable = (int2*)take((size_t)seqRuns * SEQ_NBIN * sizeof(int2));
     ctx->seqFlags = (unsigned char*)take((size_t)seqRuns);
     ctx->seqCounts = (int*)take((size_t)seqRuns * 4);
@@ -181,7 +157,7 @@ extern "C" int lsdgpu_create(int device, int width, int height, const float K[9]
     // the tracker writes its result block straight into mapped pinned memory (no D2H copy on the path)
     LSD_CHECK(ctx, cudaHostAlloc((void**)&ctx->hTrackState, sizeof(TrackState), cudaHostAllocMapped));
     // cudaHostAlloc does not clear: a recycled block may still hold the result of a destroyed context, whose doneSeq would satisfy
-    // the completion spin of this context's first launches (trackPersistentFinish) before the kernel has written anything
+    // the completion spin of this context's first launches (trackPersistent) before the kernel has written anything
     memset(ctx->hTrackState, 0, sizeof(TrackState));
     memset(ctx->hScalars, 0, 64);
     memset(ctx->hEvOut, 0, EV_NCH * 4);
@@ -360,7 +336,7 @@ static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* 
     for (int l = 0; l < LSD_LEVELS; l++) { gp.img[l] = s->image[l]; gp.grad[l] = s->grad[l]; gp.w[l] = w >> l; gp.h[l] = h >> l; }
     gp.maxgrad0 = s->maxgrad;
     // blockIdx.y = level; level 0 runs as 32x8 tiles, levels 1..4 linearly (their block counts are smaller than the tile count)
-    LSD_CHECK(ctx, launchPDL(k_gradients, dim3(divUp(w, GR_TW) * divUp(h, GR_TH), LSD_LEVELS), dim3(256), 0, ctx->stream, ctx->optPdl, gp));      // + maxGradients of level 0
+    LSD_CHECK(ctx, launchPDL(k_gradients, dim3(divUp(w, GR_TW) * divUp(h, GR_TH), LSD_LEVELS), dim3(256), 0, ctx->stream, gp));      // + maxGradients of level 0
     LAUNCH(ctx);
     LSD_CHECK(ctx, cudaGetLastError());
     s->hasDepth = false; s->idepthPyrValid = false; s->hasGoodMask = false;
@@ -763,7 +739,7 @@ extern "C" int lsdgpu_peer_attach(lsdgpu_ctx* ctx, int rank, int n_ranks, const 
     ctx->rank = rank; ctx->nRanks = n_ranks;
     // the exchange rows, done slots and the tail counter start from a known state on every rank (the caller synchronises the ranks
     // between attach and the first tracking)
-    LSD_CHECK(ctx, cudaMemsetAsync(ctx->trkSync + TP_XCHG_OFFSET, 0, (TP_SYNC_WORDS - 4 - TP_XCHG_OFFSET) * sizeof(unsigned int), ctx->stream));
+    LSD_CHECK(ctx, cudaMemsetAsync(ctx->trkSync + TP_XCHG_OFFSET, 0, (TP_SYNC_WORDS - TP_XCHG_OFFSET) * sizeof(unsigned int), ctx->stream));
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
     ctx->trkTailBase = 0;
     return 0;
@@ -840,14 +816,14 @@ extern "C" int lsdgpu_depth_invalidate(lsdgpu_ctx* ctx) { LSD_LOCK(ctx); ctx->ac
 extern "C" int lsdgpu_depth_active_keyframe(lsdgpu_ctx* ctx) { LSD_LOCK(ctx); return ctx->activeKf; }
 
 // Frame::setDepth(currentDepthMap) of the active keyframe
-static int setDepthOnKeyframe(lsdgpu_ctx* ctx, FrameSlot* kf, const int* skip = nullptr)
+static int setDepthOnKeyframe(lsdgpu_ctx* ctx, FrameSlot* kf)
 {
     const int n = ctx->w * ctx->h;
     const int nb = divUp(n, 256);
     PyrPtrs id, var;
     for (int l = 0; l < LSD_LEVELS; l++) { id.l[l] = kf->idepth[l]; var.l[l] = kf->idepthVar[l]; }
     k_set_depth_pyr<<<(ctx->w / 16) * (ctx->h / 16), 256, 0, ctx->stream>>>(ctx->cur, id, var, ctx->w, ctx->h, ctx->dScalars + 8,
-                                                                           ctx->evCounter + 48, kf->dStats, skip);
+                                                                           ctx->evCounter + 48, kf->dStats);
     LAUNCH(ctx);
     LSD_CHECK(ctx, cudaGetLastError());
     kf->statsPending = true;
@@ -870,21 +846,21 @@ extern "C" int lsdgpu_depth_init_from_gt(lsdgpu_ctx* ctx, int kf_id)
     return setDepthOnKeyframe(ctx, kf);
 }
 
-static int runRegularize(lsdgpu_ctx* ctx, bool removeOcclusions, int validityTH, const int* skip = nullptr)
+static int runRegularize(lsdgpu_ctx* ctx, bool removeOcclusions, int validityTH)
 {
     DepthCam cam = depthCam(ctx);
     DepthGlobals G = depthGlobals(ctx);
     dim3 grid(divUp(cam.w, 32), divUp(cam.h, 8));
     std::swap(ctx->cur, ctx->oth);         // oth = previous current (the memcpy of :862), cur = output
-    if (removeOcclusions) k_regularize<true><<<grid, 256, 0, ctx->stream>>>(ctx->oth, ctx->cur, cam, G, validityTH, skip);
-    else k_regularize<false><<<grid, 256, 0, ctx->stream>>>(ctx->oth, ctx->cur, cam, G, validityTH, skip);
+    if (removeOcclusions) k_regularize<true><<<grid, 256, 0, ctx->stream>>>(ctx->oth, ctx->cur, cam, G, validityTH);
+    else k_regularize<false><<<grid, 256, 0, ctx->stream>>>(ctx->oth, ctx->cur, cam, G, validityTH);
     LAUNCH(ctx);
     LSD_CHECK(ctx, cudaGetLastError());
     return 0;
 }
 // regularizeDepthMapFillHoles() + regularizeDepthMap(false, TH) as one kernel (see k_fill_regularize); with
 // setDepthOn != nullptr the kernel also does Frame::setDepth + the idepth pyramid of that keyframe
-static int runFillRegularize(lsdgpu_ctx* ctx, int validityTH, const int* skip = nullptr, FrameSlot* setDepthOn = nullptr)
+static int runFillRegularize(lsdgpu_ctx* ctx, int validityTH, FrameSlot* setDepthOn = nullptr)
 {
     FrameSlot* kf = findSlot(ctx, ctx->activeKf);
     if (!kf) return lsd_fail(ctx, "no active keyframe");
@@ -895,20 +871,20 @@ static int runFillRegularize(lsdgpu_ctx* ctx, int validityTH, const int* skip = 
     PyrPtrs id, var;
     for (int l = 0; l < LSD_LEVELS; l++) { id.l[l] = setDepthOn ? setDepthOn->idepth[l] : nullptr; var.l[l] = setDepthOn ? setDepthOn->idepthVar[l] : nullptr; }
     if (setDepthOn) {
-        LSD_CHECK(ctx, launchPDL(k_fill_regularize<true>, dim3(grid), dim3(FR_THREADS), 0, ctx->stream, ctx->optPdl, ctx->oth, ctx->cur, cam, G,
-                                 (const float*)kf->maxgrad, validityTH, skip, id, var, ctx->dScalars + 8, ctx->evCounter + 48, setDepthOn->dStats));
+        LSD_CHECK(ctx, launchPDL(k_fill_regularize<true>, dim3(grid), dim3(FR_THREADS), 0, ctx->stream, ctx->oth, ctx->cur, cam, G,
+                                 (const float*)kf->maxgrad, validityTH, id, var, ctx->dScalars + 8, ctx->evCounter + 48, setDepthOn->dStats));
         setDepthOn->statsPending = true;
         setDepthOn->hasDepth = true; setDepthOn->idepthPyrValid = true;
         setDepthOn->depthHasBeenUpdatedFlag = true;                    // Frame.cpp:242
     } else
-        LSD_CHECK(ctx, launchPDL(k_fill_regularize<false>, dim3(grid), dim3(FR_THREADS), 0, ctx->stream, ctx->optPdl, ctx->oth, ctx->cur, cam, G,
-                                 (const float*)kf->maxgrad, validityTH, skip, id, var, (double*)nullptr, (unsigned int*)nullptr, (double*)nullptr));
+        LSD_CHECK(ctx, launchPDL(k_fill_regularize<false>, dim3(grid), dim3(FR_THREADS), 0, ctx->stream, ctx->oth, ctx->cur, cam, G,
+                                 (const float*)kf->maxgrad, validityTH, id, var, (double*)nullptr, (unsigned int*)nullptr, (double*)nullptr));
     LAUNCH(ctx);
     LSD_CHECK(ctx, cudaGetLastError());
     return 0;
 }
 
-static int runFillHoles(lsdgpu_ctx* ctx, const int* skip = nullptr)
+static int runFillHoles(lsdgpu_ctx* ctx)
 {
     FrameSlot* kf = findSlot(ctx, ctx->activeKf);
     if (!kf) return lsd_fail(ctx, "no active keyframe");
@@ -916,7 +892,7 @@ static int runFillHoles(lsdgpu_ctx* ctx, const int* skip = nullptr)
     DepthGlobals G = depthGlobals(ctx);
     dim3 grid(divUp(cam.w, 32), divUp(cam.h, 8));
     std::swap(ctx->cur, ctx->oth);
-    k_fill_holes<<<grid, 256, 0, ctx->stream>>>(ctx->oth, ctx->cur, cam, G, kf->maxgrad, skip);
+    k_fill_holes<<<grid, 256, 0, ctx->stream>>>(ctx->oth, ctx->cur, cam, G, kf->maxgrad);
     LAUNCH(ctx);
     LSD_CHECK(ctx, cudaGetLastError());
     return 0;
@@ -1028,19 +1004,19 @@ static int setupObserve(lsdgpu_ctx* ctx, const int* ref_ids, int n_refs, FrameSl
     return setupObserve(ctx, d, n_refs, kf);
 }
 
-static int runObserve(lsdgpu_ctx* ctx, const int* ref_ids, int n_refs, bool devParams = false, const int* skip = nullptr, bool hostParamsReady = false)
+static int runObserve(lsdgpu_ctx* ctx, const int* ref_ids, int n_refs, bool hostParamsReady = false)
 {
     FrameSlot* kf = findSlot(ctx, ctx->activeKf);
     if (!kf) return lsd_fail(ctx, "no active keyframe");
-    if (!devParams && !hostParamsReady) {
+    if (!hostParamsReady) {
         int r = setupObserve(ctx, ref_ids, n_refs, kf);
         if (r) return r;
     }
     DepthCam cam = depthCam(ctx);
     DepthGlobals G = depthGlobals(ctx);
     const int grid = divUp((cam.w - 6) * (cam.h - 6), OBS_PIX_PER_CTA);
-    LSD_CHECK(ctx, launchPDL(k_observe, dim3(grid), dim3(OBS_THREADS), 0, ctx->stream, ctx->optPdl, ctx->cur, cam, G, (const float*)kf->image[0],
-                             (const float4*)kf->grad[0], (const float*)kf->maxgrad, ctx->hObs, (const ObserveParams*)(devParams ? ctx->dObs : nullptr), skip));
+    LSD_CHECK(ctx, launchPDL(k_observe, dim3(grid), dim3(OBS_THREADS), 0, ctx->stream, ctx->cur, cam, G, (const float*)kf->image[0],
+                             (const float4*)kf->grad[0], (const float*)kf->maxgrad, ctx->hObs));
     LAUNCH(ctx);
     LSD_CHECK(ctx, cudaGetLastError());
     return 0;
@@ -1069,7 +1045,7 @@ extern "C" int lsdgpu_depth_update_keyframe(lsdgpu_ctx* ctx, const int* ref_ids,
     if (!kf) return lsd_fail(ctx, "updateKeyframe: depth map is not valid (no active keyframe)");
     int r = runObserve(ctx, ref_ids, n_refs);                      // :1127
     if (r) return r;
-    r = runFillRegularize(ctx, VAL_SUM_MIN_FOR_KEEP, nullptr,      // :1135 + :1143 (+ setDepth :1150-1157 in the same kernel)
+    r = runFillRegularize(ctx, VAL_SUM_MIN_FOR_KEEP,               // :1135 + :1143 (+ setDepth :1150-1157 in the same kernel)
                           kf->depthHasBeenUpdatedFlag ? nullptr : kf);
     if (r) return r;
     kf->numMappedOnThis++;                                         // :1165
@@ -1084,9 +1060,9 @@ extern "C" int lsdgpu_depth_update_keyframe_refs(lsdgpu_ctx* ctx, const lsdgpu_r
     if (!kf) return lsd_fail(ctx, "updateKeyframe: depth map is not valid (no active keyframe)");
     int r = setupObserve(ctx, refs, n_refs, kf);
     if (r) return r;
-    r = runObserve(ctx, nullptr, n_refs, false, nullptr, true);    // :1127 (parameters already in ctx->hObs)
+    r = runObserve(ctx, nullptr, n_refs, true);                    // :1127 (parameters already in ctx->hObs)
     if (r) return r;
-    r = runFillRegularize(ctx, VAL_SUM_MIN_FOR_KEEP, nullptr, kf->depthHasBeenUpdatedFlag ? nullptr : kf);
+    r = runFillRegularize(ctx, VAL_SUM_MIN_FOR_KEEP, kf->depthHasBeenUpdatedFlag ? nullptr : kf);
     if (r) return r;
     kf->numMappedOnThis++;                                         // :1165
     return 0;
@@ -1243,7 +1219,7 @@ extern "C" int lsdgpu_depth_finalize_keyframe(lsdgpu_ctx* ctx)
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* kf = findSlot(ctx, ctx->activeKf);
     if (!kf) return lsd_fail(ctx, "finalizeKeyFrame: depth map is not valid");
-    int r = runFillRegularize(ctx, VAL_SUM_MIN_FOR_KEEP, nullptr, kf);   // :1373 + :1379 + setDepth :1385
+    int r = runFillRegularize(ctx, VAL_SUM_MIN_FOR_KEEP, kf);            // :1373 + :1379 + setDepth :1385
     if (r) return r;
     return takeReactivationData(ctx, kf);                                // :1387 (calculateMeanInformation :1386 returns at once, Frame.cpp:178)
 }
@@ -1257,49 +1233,6 @@ extern "C" int lsdgpu_track_and_map(lsdgpu_ctx* ctx, int kf_id, int frame_id, co
     FrameSlot* kf = findSlot(ctx, kf_id);
     if (!kf) return lsd_fail(ctx, "unknown keyframe id");
     if (kf->depthHasBeenUpdatedFlag) { r = lsdgpu_ref_import(ctx, kf_id); if (r) return r; }     // SlamSystem.cpp:907-912
-    FrameSlot* fr = findSlot(ctx, frame_id);
-    // LSDGPU_SINGLE_SYNC=1 (opt-in): the whole frame is enqueued back to back and the host synchronises once; the stereo
-    // constants of prepareForStereoWith are then computed by the tracking kernel's last thread, whose one-thread double-precision
-    // work at the kernel's tail costs about what the round trip of the default (poll the tracking result, constants on the
-    // host) saves.
-    const bool singleSync = ctx->optSingleSync == 1;
-    if (singleSync && mode == 1 && !keyframe_change && ctx->activeKf == kf_id && fr) {
-        // Whole frame enqueued back to back: tracking kernel, device-side prepareForStereoWith, observe, fill holes,
-        // regularise, setDepth -- ONE host synchronisation at the end (the mapping kernels read the pose from the
-        // tracker's device-resident result and do nothing if tracking diverged).
-        lsdgpu_track_settings ds;
-        if (!s) { lsdgpu_default_track_settings(&ds); ds.maxItsPerLvl[4] = 0; s = &ds; }
-        r = ensureIdepthPyramid(ctx, kf);
-        if (r) return r;
-        PrepareConsts pc;
-        memcpy(pc.K, ctx->cam[0].K, 36);
-        pc.frameId = frame_id; pc.reactivated = ctx->activeKfReactivated ? 1 : 0;
-        pc.kfNumTracked = kf->numFramesTrackedOnThis; pc.kfNumMapped = kf->numMappedOnThis;
-        pc.W1 = ctx->w >> SE3TRACKING_MIN_LEVEL; pc.H1 = ctx->h >> SE3TRACKING_MIN_LEVEL;
-        pc.image = fr->image[0]; pc.goodMask = fr->goodMask;
-        r = trackPersistentEnqueue(ctx, kf, fr, init_qt, s, &pc);         // the kernel's last thread also writes ctx->dObs / dSkipFlag
-        if (r) return r;
-        r = runObserve(ctx, &frame_id, 1, true, ctx->dSkipFlag);          // DepthMap.cpp:1127
-        if (r) return r;
-        const bool didSetDepth = !kf->depthHasBeenUpdatedFlag;            // :1150-1157
-        const bool prevPending = kf->statsPending, prevPyr = kf->idepthPyrValid;
-        r = runFillRegularize(ctx, VAL_SUM_MIN_FOR_KEEP, ctx->dSkipFlag, didSetDepth ? kf : nullptr);    // :1135 + :1143 (+ setDepth)
-        if (r) return r;
-        r = trackPersistentFinish(ctx, fr, out);                          // the one synchronisation of the frame
-        if (r) return r;
-        if (out->diverged) {                 // nothing ran on the device: undo the host-side bookkeeping
-            std::swap(ctx->cur, ctx->oth);   // the (skipped) fill+regularise kernel had swapped the ping-pong buffers once
-            if (didSetDepth) { kf->depthHasBeenUpdatedFlag = false; kf->statsPending = prevPending; kf->idepthPyrValid = prevPyr; }
-            return 0;
-        }
-        if (out->trackingWasGood) kf->numFramesTrackedOnThis++;           // SE3Tracker.cpp:479-480
-        fr->initialTrackedResidual = out->initialTrackedResidual;
-        for (int i = 0; i < 7; i++) fr->thisToParent[i] = out->frameToRef_qt[i];
-        fr->thisToParent[7] = 1.0;
-        fr->parentId = kf->id;
-        kf->numMappedOnThis++;                                            // DepthMap.cpp:1165
-        return lsdgpu_frame_clear_good_mask(ctx, frame_id);               // SlamSystem.cpp:573
-    }
     r = lsdgpu_se3_track(ctx, kf_id, frame_id, init_qt, s, mode, out);
     if (r) return r;
     if (out->diverged) return 0;                 // the caller decides (relocalisation is out of scope)

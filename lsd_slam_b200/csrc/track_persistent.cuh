@@ -32,9 +32,7 @@
 #define TP_THREADS 512
 #define TP_WARPS (TP_THREADS / 32)
 #define TP_MAXGRID 160               // combine code is unrolled for <= 160 CTAs (H100 SXM: 132 SMs)
-#define TP_MAXGRID_DBG 160
-#define TP_WIN_SMEM (TP_WARPS * TRK_WIN_W * TRK_WIN_H * 16)    // 16 warps x 13056 B = 208896 B of dynamic smem
-#define TP_SYNC_WORDS 4096           // ctx->trkSync: word 0 = arrival counter of the grid barrier; last 4 words: debug counters
+#define TP_SYNC_WORDS 4096           // ctx->trkSync: word 0 = arrival counter of the grid barrier
 #define TP_MAX_RANKS 8               // GPUs one stream's tracking can be sharded over (peer exchange, see gridExchangeRanks)
 #define TP_XCHG_OFFSET 1024          // word offset of the cross-GPU exchange rows: [TP_MAX_RANKS][64] slots of {value, tag} (8 B each)
 #define TP_DONE_OFFSET 3072          // word offset of the per-peer "my writes into your memory are complete" slots (8 B each)
@@ -53,11 +51,9 @@ struct TrackLevelParams {
     // j = (x-1) + (y-1)*iw, and cut into chunks of 32 consecutive j (chunk c -> CTA c % gridDim, warp slot c / gridDim).
     // At 640x480 level 1 has 318*238 = 75 684 interior pixels = 2 366 chunks over 132 CTAs x 16 warps: one or two chunks per warp.
     int iw, nInt, nChunks;
-    int G;                           // unused by trackFrame (all CTAs take part in every level); kept for the batch trackers
 };
 
-struct alignas(64) TrackParams {
-    CUtensorMap gradMap[LSD_LEVELS]; // TMA descriptors of the tracked frame's gradient levels (64-byte aligned)
+struct TrackParams {
     TrackLevelParams lvl[LSD_LEVELS];
     uint8_t* goodMask;               // level-1 mask of the tracked frame
     int maskFresh;                   // 1: initialise the mask to true first (Frame.h:433)
@@ -69,22 +65,17 @@ struct alignas(64) TrackParams {
     int useAffine;
     float* partials;                 // [2][gridDim][TP_ROW]
     unsigned int* sync;              // word 0: arrival counter of the grid barrier (monotonic, never reset)
-    unsigned int barrierBase[LSD_LEVELS];   // [0]: arrivals counted by earlier launches
+    unsigned int barrierBase;        // arrivals counted by earlier launches
     int debug;                       // 1: also write the per-CTA cycle table
     unsigned int launchSeq;          // value the kernel stores in TrackState::doneSeq when the result block is complete
     int minLevel;                    // last level of the coarse-to-fine loop (1 for trackFrame, 4 for permaRef tracking)
-    int useTma;                      // 1: per-warp shared-memory windows loaded by TMA; 0: all taps through L1/L2
-    int kmax;                        // candidate poses per pass (1 = no speculation; <= TP_KMAX)
+    int kmax;                        // candidate poses per pass (TP_KMAX for trackFrame, 1 = no speculation for permaRef tracking)
     // one stream sharded over nRanks GPUs (BASELINE config 5): this GPU evaluates every nRanks-th chunk; the per-pass sums and the
     // level-1 mask are exchanged through peer-mapped memory inside the kernel (no host, no NCCL call on the path)
     int nRanks, rank;
     unsigned int* peerSync[TP_MAX_RANKS];     // each rank's `sync` block as mapped into THIS process (own entry = sync)
     uint8_t* peerMask[TP_MAX_RANKS];          // the tracked frame's level-1 mask on each rank
     unsigned int tailBase;                    // arrivals already counted on the tail barrier
-    int doPrepare;                   // 1: the last thread also turns the result into the observe parameters of the same frame
-    PrepareConsts prep;              //    (Frame::prepareForStereoWith + head of DepthMap::updateKeyframe), no host round trip
-    ObserveParams* obsOut;
-    int* skipOut;
 };
 
 // what the kernel hands back (block 0 writes it)
@@ -101,41 +92,8 @@ struct TrackState {
     int totalEvals;                  // passes (= grid barriers) of this launch
     volatile unsigned int doneSeq;   // written last (after a system-wide fence): the host polls it instead of a stream sync
     long long cyc[6];                // block-0 cycle breakdown: points, CTA reduce, barrier, combine, serial LM, total
-    long long cycBlk[TP_MAXGRID_DBG][6];   // the same per CTA (debug)
+    long long cycBlk[TP_MAXGRID][6];   // the same per CTA (debug); the last row holds warp 0's cycles
 };
-
-// ---- TMA / mbarrier PTX (sm_90+; SASS: UTMALDG / SYNCS) ---------------------------------------------------
-__device__ __forceinline__ uint32_t smemU32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbarInit(uint64_t* bar, unsigned int count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smemU32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbarExpectTx(uint64_t* bar, unsigned int bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smemU32(bar)), "r"(bytes) : "memory");
-}
-// bounded wait: returns false if the phase did not complete within ~maxPolls probes (never observed; keeps a
-// mis-programmed copy from hanging the whole cooperative grid)
-__device__ __forceinline__ bool mbarWait(uint64_t* bar, unsigned int parity, int maxPolls = 1 << 16)
-{
-    for (int it = 0; it < maxPolls; it++) {
-        unsigned int done;
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-            "selp.u32 %0, 1, 0, p;\n"
-            "}\n" : "=r"(done) : "r"(smemU32(bar)), "r"(parity) : "memory");
-        if (done) return true;
-    }
-    return false;
-}
-__device__ __forceinline__ void tmaLoad2D(void* dst, const CUtensorMap* map, int x, int y, uint64_t* bar)
-{
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                 ::"r"(smemU32(dst)), "l"(map), "r"(x), "r"(y), "r"(smemU32(bar)) : "memory");
-}
-
 
 // Grid-wide barrier.  Arrivals are counted on one word (monotonic: epoch e completes at base + e * gridDim arrivals, the
 // counter is never reset): release-add, then polling of the counter itself; thread 0 carries the release / acquire for its
@@ -245,14 +203,8 @@ __device__ __forceinline__ int tpChunkOf(int b, int k, int G)
     return k * G + (b + k * 37) % G;
 }
 
-struct WarpWindow {
-    const float4* win;               // this warp's TRK_WIN_H x TRK_WIN_W window in shared memory
-    uint64_t* bar;
-    unsigned int parity;             // phase of the next completion to wait for
-    int lvl;                         // level the window currently holds (-1: none)
-    int ox, oy;                      // window origin in level pixels
-    bool valid;
-    unsigned int hits;               // low 16 bits: taps served from the window, high 16: taps through L1/L2
+// per-thread state carried in registers from one pass to the next
+struct ThreadCarry {
     // the thread's first pixel of the current level, reconstructed once (see gridEvaluate)
     int pcLvl;
     bool pcIsPoint;
@@ -325,7 +277,7 @@ __device__ __forceinline__ void gridTailRanks(const TrackParams& p)
 }
 
 __device__ __forceinline__ void gridEvaluate(const TrackParams& p, int lvl, LMShared& sh, float (*sm)[EV_NCHX], float (*comb)[TP_ROW],
-                                             unsigned int& epoch, long long* cyc, WarpWindow& W)
+                                             unsigned int& epoch, long long* cyc, ThreadCarry& tc)
 {
     long long t0 = clock64();
     const TrackLevelParams& L = p.lvl[lvl];
@@ -345,7 +297,7 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, int lvl, LMSh
     // sharded over nRanks GPUs: the CTAs of all ranks form one virtual grid (this CTA is number b * nRanks + rank of it)
     const int Gv = G * p.nRanks, vb = (int)blockIdx.x * p.nRanks + p.rank;
     const int nSlots = (L.nChunks + Gv - 1) / Gv;
-    if (mask) { W.lastBits = 0u; W.pointBits = 0u; }
+    if (mask) { tc.lastBits = 0u; tc.pointBits = 0u; }
     int slot = 0;
     for (int k = warp; k < nSlots; k += TP_WARPS, slot++) {
         const int chunk = tpChunkOf(vb, k, Gv);
@@ -359,11 +311,11 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, int lvl, LMSh
             const int yy = j / iw;
             i = (j - yy * iw + 1) + (yy + 1) * w;                      // x = 1 + j % iw, y = 1 + j / iw
         }
-        if (firstChunk && W.pcLvl == lvl) {
+        if (firstChunk && tc.pcLvl == lvl) {
             // the thread's first pixel of a level never changes between the passes of that level: keep the
             // reconstructed point in registers instead of re-reading the keyframe planes (an L2 round trip at the head
             // of every pass's dependency chain)
-            isPoint = W.pcIsPoint; px = W.pcx; py = W.pcy; pz = W.pcz; var = W.pcVar; color = W.pcColor;
+            isPoint = tc.pcIsPoint; px = tc.pcx; py = tc.pcy; pz = tc.pcz; var = tc.pcVar; color = tc.pcColor;
         } else {
             if (j < nInt) {
                 const float idepth = __ldg(L.kfIdepth + i);
@@ -377,75 +329,20 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, int lvl, LMSh
                 }
             }
             if (firstChunk) {
-                W.pcLvl = lvl; W.pcIsPoint = isPoint;
-                W.pcx = px; W.pcy = py; W.pcz = pz; W.pcVar = var; W.pcColor = color;
-            }
-        }
-        // First chunk of this warp on a new level: stage the part of the frame's gradient level that the chunk
-        // warps into (centred on the chunk under the level's initial pose) in shared memory with ONE TMA box copy.
-        // All later passes of the level tap the window; taps that leave it fall back to L1/L2.
-        if (p.useTma && firstChunk && W.lvl != lvl) {                  // warp-uniform condition
-            float u = 0.f, v = 0.f;
-            bool ok = false;
-            if (isPoint) {
-                const float Wx = ((P.R[0] * px + P.R[1] * py) + P.R[2] * pz) + P.t[0];
-                const float Wy = ((P.R[3] * px + P.R[4] * py) + P.R[5] * pz) + P.t[1];
-                const float Wz = ((P.R[6] * px + P.R[7] * py) + P.R[8] * pz) + P.t[2];
-                u = (Wx / Wz) * L.fx + L.cx; v = (Wy / Wz) * L.fy + L.cy;
-                ok = (u > -1e4f && u < 1e4f && v > -1e4f && v < 1e4f);
-            }
-            const unsigned int bal = __ballot_sync(0xffffffffu, ok);
-            W.lvl = lvl;
-            W.valid = bal != 0u;
-            if (W.valid) {
-                // reference lane: the valid lane closest to the chunk centre
-                int src = 16;
-                if (!((bal >> 16) & 1u)) src = (bal >> 16) ? (__ffs(bal >> 16) - 1 + 16) : (31 - __clz(bal));
-                const float uc = __shfl_sync(0xffffffffu, u, src), vc = __shfl_sync(0xffffffffu, v, src);
-                W.ox = (int)floorf(uc) - (src - 16) - (TRK_WIN_W - 32) / 2 - 16;
-                W.oy = (int)floorf(vc) - TRK_WIN_H / 2;
-                __syncwarp();
-                if (lane == 0) {
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of the old window are done
-                    mbarExpectTx(W.bar, TRK_WIN_W * TRK_WIN_H * 16);
-                    tmaLoad2D((void*)W.win, &p.gradMap[lvl], 4 * W.ox, W.oy, W.bar);
-                }
-                if (mbarWait(W.bar, W.parity)) W.parity ^= 1u;
-                else { W.valid = false; W.lvl = -2; if (lane == 0) atomicAdd(p.sync + TP_SYNC_WORDS - 4, 1u); }   // counted, reported by the host
+                tc.pcLvl = lvl; tc.pcIsPoint = isPoint;
+                tc.pcx = px; tc.pcy = py; tc.pcz = pz; tc.pcVar = var; tc.pcColor = color;
             }
         }
         if (isPoint) {
-            const bool useWin = p.useTma && firstChunk && W.valid && W.lvl == lvl;
-            const float4* win = W.win;
-            const int ox = W.ox, oy = W.oy;
-            unsigned int* hitCtr = &W.hits;
-            auto tap = [fg, w, win, ox, oy, useWin, hitCtr](float u, float v, float& o0, float& o1, float& o2) {
-                const int ix = (int)u, iy = (int)v;
-                const int lx = ix - ox, ly = iy - oy;
-                if (useWin && lx >= 0 && lx < TRK_WIN_W - 1 && ly >= 0 && ly < TRK_WIN_H - 1) {
-                    (*hitCtr)++;
-                    // same weights and summation order as interp43 (globalFuncs.h:63-77), texels from shared memory
-                    const float dx = u - ix, dy = v - iy;
-                    const float dxdy = dx * dy;
-                    const float4* bp = win + ly * TRK_WIN_W + lx;
-                    const float4 br = bp[1 + TRK_WIN_W], bl = bp[TRK_WIN_W], tr = bp[1], tl = bp[0];
-                    const float w0 = dxdy, w1 = (dy - dxdy), w2 = (dx - dxdy), w3 = (1 - dx - dy + dxdy);
-                    o0 = w0 * br.x + w1 * bl.x + w2 * tr.x + w3 * tl.x;
-                    o1 = w0 * br.y + w1 * bl.y + w2 * tr.y + w3 * tl.y;
-                    o2 = w0 * br.z + w1 * bl.z + w2 * tr.z + w3 * tl.z;
-                } else {
-                    (*hitCtr) += 0x10000u;
-                    interp43(fg, u, v, w, o0, o1, o2);
-                }
-            };
+            auto tap = [fg, w](float u, float v, float& o0, float& o1, float& o2) { interp43(fg, u, v, w, o0, o1, o2); };
             const int good = evalPoint(px, py, pz, color, var, P, p.C, L.fx, L.fy, L.cx, L.cy, w, h, tap, acc);
             if (K > 1) {                                               // block-uniform
                 if (K > 2) evalPointLight<false>(px, py, pz, color, var, sh.pose[1], p.C, L.fx, L.fy, L.cx, L.cy, w, h, tap, ext);
                 const int goodL = evalPointLight<true>(px, py, pz, color, var, sh.pose[K - 1], p.C, L.fx, L.fy, L.cx, L.cy, w, h, tap, ext);
-                if (mask) W.lastBits |= (unsigned int)goodL << slot;
+                if (mask) tc.lastBits |= (unsigned int)goodL << slot;
             }
             if (mask) {
-                mask[i] = (uint8_t)good; W.pointBits |= 1u << slot;
+                mask[i] = (uint8_t)good; tc.pointBits |= 1u << slot;
                 if (p.nRanks > 1)                                      // the other ranks own other chunks: give them this one's flag
                     for (int d = 0; d < p.nRanks; d++) if (d != p.rank) p.peerMask[d][i] = (uint8_t)good;
             }
@@ -471,7 +368,7 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, int lvl, LMSh
     if (threadIdx.x < nch) __stcg(part + (size_t)blockIdx.x * TP_ROW + threadIdx.x, ctaSum);
     epoch++;
     long long t2 = clock64();
-    gridBarrier(p.sync, p.barrierBase[0] + epoch * gridDim.x);
+    gridBarrier(p.sync, p.barrierBase + epoch * gridDim.x);
     long long t3 = clock64();
     // warp wi adds rows wi, wi+16, ... (<= 10): the lower half-warp takes the even ones of those, the upper half the odd ones, each
     // lane one float4 (4 channels) of a 256-byte row -- 5 vector loads per thread, all in flight before the first add.  fp32 adds
@@ -612,7 +509,7 @@ struct LMState {
     int lvl, iteration, phase, incTry, diverged;
     int chainBase;                   // lm.incTry when the chain of the pass in flight was built
     int statsFrom;                   // where the statistics of the last evaluated pose are: 0 = main block, 1 = extension block
-    int commitLast;                  // 1: the good-mask of the last evaluated pose is in WarpWindow::lastBits, not yet in the mask
+    int commitLast;                  // 1: the good-mask of the last evaluated pose is in ThreadCarry::lastBits, not yet in the mask
     int posesEvaluated;
     long long dbg[4];                // warp-0 cycles: decisions, chain building
 };
@@ -830,7 +727,7 @@ __device__ __forceinline__ void lmAdvance(const TrackParams& p, LMState& lm, LMS
     }
 }
 
-__global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid_constant__ TrackParams p, TrackState* __restrict__ out, TrackState* __restrict__ outDev)
+__global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid_constant__ TrackParams p, TrackState* __restrict__ out)
 {
     __shared__ alignas(LMShared) unsigned char shStorage[sizeof(LMShared)];   // raw storage: Cand holds a type with a constructor
     LMShared& sh = *reinterpret_cast<LMShared*>(shStorage);
@@ -839,21 +736,13 @@ __global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid
     __shared__ float sm[TP_WARPS][EV_NCHX];
     __shared__ __align__(16) float comb[TP_WARPS][TP_ROW];         // per-warp partial sums of the combine
     static_assert(EV_NCH == 40 && EV_NX == 16, "warpReduceAcc / warpReduceExt are written for 32 + 8 (+ 16) channels");
-    extern __shared__ __align__(128) unsigned char winSmem[];      // TP_WARPS windows of TRK_WIN_H x TRK_WIN_W float4
-    __shared__ __align__(8) uint64_t winBar[TP_WARPS];
     unsigned int epoch = 0;
     long long cyc[6] = { 0, 0, 0, 0, 0, 0 };
     const long long tStart = clock64();
-    WarpWindow W;
-    W.win = reinterpret_cast<const float4*>(winSmem) + (size_t)(threadIdx.x >> 5) * (TRK_WIN_W * TRK_WIN_H);
-    W.bar = &winBar[threadIdx.x >> 5];
-    W.parity = 0u; W.lvl = -1; W.ox = 0; W.oy = 0; W.valid = false; W.hits = 0u; W.pcLvl = -1; W.pcIsPoint = false;
-    W.pcx = W.pcy = W.pcz = W.pcVar = W.pcColor = 0.f;
-    W.lastBits = 0u; W.pointBits = 0u;
-    if (p.useTma && (threadIdx.x & 31) == 0) {
-        mbarInit(W.bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    ThreadCarry tc;
+    tc.pcLvl = -1; tc.pcIsPoint = false;
+    tc.pcx = tc.pcy = tc.pcz = tc.pcVar = tc.pcColor = 0.f;
+    tc.lastBits = 0u; tc.pointBits = 0u;
 
     // fresh refPixelWasGood mask: all true (Frame.h:433); ordered before the level-1 passes by the barriers
     if (p.maskFresh) {
@@ -876,7 +765,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid
 
     while (true) {
         const int lvl = sh.lvl;
-        gridEvaluate(p, lvl, sh, sm, comb, epoch, cyc, W);
+        gridEvaluate(p, lvl, sh, sm, comb, epoch, cyc, tc);
         if (threadIdx.x < 32) {
             if (threadIdx.x == 0) { lm.nEval[lvl]++; lm.nPts[lvl] = sh.sums[CH_REFNUM]; }
             lmAdvance(p, lm, sh, threadIdx.x);
@@ -894,11 +783,11 @@ __global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid
         const int nSlots = (L.nChunks + Gv - 1) / Gv;
         int slot = 0;
         for (int k = warp; k < nSlots; k += TP_WARPS, slot++) {
-            if (!((W.pointBits >> slot) & 1u)) continue;
+            if (!((tc.pointBits >> slot) & 1u)) continue;
             const int j = (tpChunkOf(vb, k, Gv) << 5) + lane;
             const int yy = j / L.iw;
             const int i = (j - yy * L.iw + 1) + (yy + 1) * L.w;
-            const uint8_t g = (uint8_t)((W.lastBits >> slot) & 1u);
+            const uint8_t g = (uint8_t)((tc.lastBits >> slot) & 1u);
             p.goodMask[i] = g;
             if (p.nRanks > 1)
                 for (int d = 0; d < p.nRanks; d++) if (d != p.rank) p.peerMask[d][i] = g;
@@ -906,11 +795,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid
     }
     if (p.nRanks > 1) gridTailRanks(p);
 
-    if (p.debug) {
-        atomicAdd(p.sync + TP_SYNC_WORDS - 3, W.hits & 0xffffu);
-        atomicAdd(p.sync + TP_SYNC_WORDS - 2, W.hits >> 16);
-    }
-    if (p.debug && threadIdx.x == 0 && blockIdx.x < TP_MAXGRID_DBG - 1) {
+    if (p.debug && threadIdx.x == 0 && blockIdx.x < TP_MAXGRID - 1) {
         long long tot = clock64() - tStart;
         for (int i = 0; i < 4; i++) out->cycBlk[blockIdx.x][i] = cyc[i];
         out->cycBlk[blockIdx.x][5] = tot;
@@ -940,36 +825,13 @@ __global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid
         }
         out->posesEvaluated = lm.posesEvaluated;
         out->totalEvals = (int)epoch;
-        // device-resident copy of what the mapping kernels of the same frame need (no host round trip in between)
-        for (int i = 0; i < 7; i++) outDev->refToFrame[i] = out->refToFrame[i];
-        outDev->pointUsage = ev.pointUsage; outDev->goodCount = ev.goodCount; outDev->badCount = ev.badCount;
-        outDev->lastResidual = lm.last_residual; outDev->diverged = lm.diverged;
-        if (p.doPrepare)
-            devicePrepareObserve(lm.refToFrame, lm.diverged, lm.last_residual, ev.pointUsage, ev.goodCount, ev.badCount, p.prep, p.obsOut, p.skipOut);
         cyc[5] = clock64() - tStart;
         cyc[4] = cyc[5] - cyc[0] - cyc[1] - cyc[2] - cyc[3];
         for (int i = 0; i < 6; i++) out->cyc[i] = cyc[i];
-        if (p.debug) for (int i = 0; i < 4; i++) out->cycBlk[TP_MAXGRID_DBG - 1][i] = lm.dbg[i];
+        if (p.debug) for (int i = 0; i < 4; i++) out->cycBlk[TP_MAXGRID - 1][i] = lm.dbg[i];
         __threadfence_system();
         out->doneSeq = p.launchSeq;
     }
-}
-
-// Environment switches are read ONCE, when the context is created (they used to cost several getenv() per frame).
-static void trackReadOptions(lsdgpu_ctx* ctx)
-{
-    const char* e;
-    // TMA windows off by default: on H100 (L1 and shared memory share 256 KB per SM) the 204 KB of windows leave L1 small, and
-    // with 132 CTAs x 16 warps for the 2 366 level-1 chunks of a 640x480 frame 254 warps have a second chunk without a window;
-    // all taps through L1/L2 with the full L1 track a 640x480 frame faster.  Results are identical either way.
-    ctx->optTrackTma = (e = getenv("LSDGPU_TRACK_TMA")) ? atoi(e) : 0;
-    ctx->optTrackDebug = getenv("LSDGPU_TRACK_DEBUG") != nullptr;
-    ctx->optSingleSync = (e = getenv("LSDGPU_SINGLE_SYNC")) ? atoi(e) : 0;
-    // candidate poses per pass (1 = one pose per pass, the round-1 behaviour; default TP_KMAX)
-    ctx->optTrackKmax = (e = getenv("LSDGPU_TRACK_KMAX")) ? atoi(e) : TP_KMAX;
-    ctx->optPdl = (e = getenv("LSDGPU_PDL")) ? atoi(e) != 0 : true;
-    if (ctx->optTrackKmax < 1) ctx->optTrackKmax = 1;
-    if (ctx->optTrackKmax > TP_KMAX) ctx->optTrackKmax = TP_KMAX;
 }
 
 static cudaError_t trackPersistentSetup(lsdgpu_ctx* ctx)
@@ -978,15 +840,11 @@ static cudaError_t trackPersistentSetup(lsdgpu_ctx* ctx)
     cudaError_t e = cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, ctx->device);
     if (e != cudaSuccess) return e;
     if (!coop) return cudaErrorNotSupported;
-    e = cudaFuncSetAttribute((const void*)k_track_persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, TP_WIN_SMEM);
-    if (e != cudaSuccess) return e;
-    trackReadOptions(ctx);
+    ctx->optTrackDebug = getenv("LSDGPU_TRACK_DEBUG") != nullptr;              // read once, not per frame
     ctx->trackGrid = ctx->smCount < TP_MAXGRID ? ctx->smCount : TP_MAXGRID;      // one CTA per SM, co-resident (cooperative launch)
-    if (ctx->optTrackDebug) fprintf(stderr, "[track] grid %d, candidate poses per pass <= %d\n", ctx->trackGrid, ctx->optTrackKmax);
+    if (ctx->optTrackDebug) fprintf(stderr, "[track] grid %d, candidate poses per pass <= %d\n", ctx->trackGrid, TP_KMAX);
     return cudaSuccess;
 }
-
-static int trackPersistentFinish(lsdgpu_ctx* ctx, FrameSlot* fr, lsdgpu_track_result* out);
 
 // device time of the last profiled tracking launch (CUDA events on the context's stream), accumulated lazily
 static void flushTrackProfile(lsdgpu_ctx* ctx)
@@ -998,9 +856,9 @@ static void flushTrackProfile(lsdgpu_ctx* ctx)
     ctx->trackProfilePending = false;
 }
 
-// enqueue the tracking kernel of one frame on the context's stream (no host synchronisation)
-static int trackPersistentEnqueue(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const double init_qt[7],
-                                  const lsdgpu_track_settings* st, const PrepareConsts* prep = nullptr)
+// track one frame: launch the kernel on the context's stream, wait for its result block and translate it (SE3Tracker.cpp:453-485)
+static int trackPersistent(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const double init_qt[7],
+                           const lsdgpu_track_settings* st, lsdgpu_track_result* out)
 {
     flushTrackProfile(ctx);
     TrackParams P;
@@ -1012,10 +870,7 @@ static int trackPersistentEnqueue(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr,
         L.w = c.w; L.h = c.h; L.fx = c.fx; L.fy = c.fy; L.cx = c.cx; L.cy = c.cy;
         L.fxi = c.fxi; L.fyi = c.fyi; L.cxi = c.cxi; L.cyi = c.cyi;
         L.iw = c.w - 2; L.nInt = (c.w - 2) * (c.h - 2); L.nChunks = (L.nInt + 31) / 32;
-        L.G = ctx->trackGrid;
     }
-    for (int l = 0; l < LSD_LEVELS; l++) P.gradMap[l] = fr->gradMap[l];
-    P.useTma = ctx->optTrackTma;
     P.minLevel = SE3TRACKING_MIN_LEVEL;
     P.goodMask = fr->goodMask;
     P.maskFresh = fr->hasGoodMask ? 0 : 1;
@@ -1032,8 +887,8 @@ static int trackPersistentEnqueue(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr,
     P.useAffine = ctx->g.useAffineLightningEstimation;
     P.partials = ctx->evPartials;
     P.sync = ctx->trkSync;
-    P.barrierBase[0] = ctx->trkBase[0];
-    P.kmax = ctx->optTrackKmax;
+    P.barrierBase = ctx->trkBase;
+    P.kmax = TP_KMAX;
     P.nRanks = ctx->nRanks; P.rank = ctx->rank;
     P.tailBase = ctx->trkTailBase;
     for (int d = 0; d < ctx->nRanks; d++) {
@@ -1042,21 +897,16 @@ static int trackPersistentEnqueue(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr,
         P.peerMask[d] = reinterpret_cast<uint8_t*>(base + ((char*)fr->goodMask - ctx->arena));
     }
     if (ctx->nRanks > 1) ctx->trkTailBase += (unsigned int)ctx->trackGrid;
-    if (prep) { P.doPrepare = 1; P.prep = *prep; P.obsOut = ctx->dObs; P.skipOut = ctx->dSkipFlag; }
     TrackState* dOut = (TrackState*)ctx->dTrackStateMapped;
-    TrackState* dOutDev = (TrackState*)ctx->dTrackState;
 
     const int grid = ctx->trackGrid;                                               // one CTA per SM
-    void* args[] = { (void*)&P, (void*)&dOut, (void*)&dOutDev };
-    const bool dbg = ctx->optTrackDebug;
-    P.debug = dbg ? 1 : 0;
+    void* args[] = { (void*)&P, (void*)&dOut };
+    P.debug = ctx->optTrackDebug ? 1 : 0;
     P.launchSeq = ++ctx->trackSeq;
-    if (dbg) LSD_CHECK(ctx, cudaMemsetAsync(ctx->trkSync + TP_SYNC_WORDS - 4, 0, 4 * sizeof(unsigned int), ctx->stream));
     if (ctx->profileTrackKernel) cudaEventRecord(ctx->kBegin, ctx->stream);
     {
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(grid); cfg.blockDim = dim3(TP_THREADS); cfg.stream = ctx->stream;
-        cfg.dynamicSmemBytes = P.useTma ? TP_WIN_SMEM : 0;           // without windows the shared-memory carve-out goes to L1
         cudaLaunchAttribute at[1];
         at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
@@ -1065,21 +915,7 @@ static int trackPersistentEnqueue(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr,
     ctx->launches++;
     if (ctx->profileTrackKernel) cudaEventRecord(ctx->kEnd, ctx->stream);
     fr->hasGoodMask = true;
-    ctx->trackUseTma = P.useTma;
-    return 0;
-}
 
-static int trackPersistent(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const double init_qt[7],
-                           const lsdgpu_track_settings* st, lsdgpu_track_result* out)
-{
-    int r = trackPersistentEnqueue(ctx, kf, fr, init_qt, st);
-    if (r) return r;
-    return trackPersistentFinish(ctx, fr, out);
-}
-
-// wait for the frame's work and translate the mapped result block (SE3Tracker.cpp:453-485)
-static int trackPersistentFinish(lsdgpu_ctx* ctx, FrameSlot* fr, lsdgpu_track_result* out)
-{
     memset(out, 0, sizeof(*out));
     TrackState* hOut = (TrackState*)ctx->hTrackState;
     // The result block lives in mapped pinned memory and its last word is a sequence number: spin on it (a few
@@ -1096,7 +932,7 @@ static int trackPersistentFinish(lsdgpu_ctx* ctx, FrameSlot* fr, lsdgpu_track_re
     // the other fields of the mapped result block are read with plain loads below: keep them behind the doneSeq read.  Block 0
     // publishes doneSeq while other CTAs may still be exiting, so only STREAM-ORDERED consumers may assume the kernel has retired.
     std::atomic_thread_fence(std::memory_order_acquire);
-    ctx->trkBase[0] += (unsigned int)hOut->totalEvals * (unsigned int)ctx->trackGrid;    // the arrival counter is never reset
+    ctx->trkBase += (unsigned int)hOut->totalEvals * (unsigned int)ctx->trackGrid;    // the arrival counter is never reset
 
     if (ctx->profileTrackKernel) {           // the event pair is read lazily (flushTrackProfile): no extra sync on the path
         // SURVEY 8d, fused single-pass kernel: B_fused(l) = 20 B per valid point + 16 B per texel of the frame's gradient
@@ -1113,19 +949,16 @@ static int trackPersistentFinish(lsdgpu_ctx* ctx, FrameSlot* fr, lsdgpu_track_re
     }
 
     if (ctx->optTrackDebug) {
-        unsigned int dbgc[4] = { 0, 0, 0, 0 };
-        cudaMemcpy(dbgc, ctx->trkSync + TP_SYNC_WORDS - 4, 16, cudaMemcpyDeviceToHost);
-        fprintf(stderr, "[track] useTma=%d tmaTimeouts=%u taps: %u from the smem window, %u through L1/L2\n", ctx->trackUseTma, dbgc[0], dbgc[1], dbgc[2]);
         fprintf(stderr, "[track] passes=%d (L4..L1: %d %d %d %d) poses=%d reference evaluations=%d cycles: points=%lld ctaReduce=%lld barrier=%lld combine=%lld serialLM=%lld total=%lld\n",
                 hOut->totalEvals, hOut->evalsAtLevel[4], hOut->evalsAtLevel[3], hOut->evalsAtLevel[2], hOut->evalsAtLevel[1], hOut->posesEvaluated,
                 hOut->numCalcResidualCalls[4] + hOut->numCalcResidualCalls[3] + hOut->numCalcResidualCalls[2] + hOut->numCalcResidualCalls[1],
                 hOut->cyc[0], hOut->cyc[1], hOut->cyc[2], hOut->cyc[3], hOut->cyc[4], hOut->cyc[5]);
-        fprintf(stderr, "   warp 0: decisions=%lld chain building=%lld\n", hOut->cycBlk[TP_MAXGRID_DBG - 1][0], hOut->cycBlk[TP_MAXGRID_DBG - 1][1]);
+        fprintf(stderr, "   warp 0: decisions=%lld chain building=%lld\n", hOut->cycBlk[TP_MAXGRID - 1][0], hOut->cycBlk[TP_MAXGRID - 1][1]);
         const char* nm[6] = { "points", "ctaReduce", "barrier", "combine", "serial", "total" };
         const int gAll = ctx->trackGrid;
         for (int k = 0; k < 6; k++) {
             long long mn = 1LL << 60, mx = 0, sum = 0; int imx = 0, imn = 0;
-            for (int b = 0; b < gAll && b < TP_MAXGRID_DBG - 1; b++) {
+            for (int b = 0; b < gAll && b < TP_MAXGRID - 1; b++) {
                 long long v = hOut->cycBlk[b][k];
                 if (v < mn) { mn = v; imn = b; }
                 if (v > mx) { mx = v; imx = b; }
@@ -1136,18 +969,9 @@ static int trackPersistentFinish(lsdgpu_ctx* ctx, FrameSlot* fr, lsdgpu_track_re
         if (getenv("LSDGPU_TRACK_DEBUG_CTAS")) {
             for (int k = 0; k < 3; k++) {
                 fprintf(stderr, "   %s per cta:", nm[k]);
-                for (int b = 0; b < gAll && b < TP_MAXGRID_DBG - 1; b++) fprintf(stderr, " %lld", hOut->cycBlk[b][k] / 100);
+                for (int b = 0; b < gAll && b < TP_MAXGRID - 1; b++) fprintf(stderr, " %lld", hOut->cycBlk[b][k] / 100);
                 fprintf(stderr, "\n");
             }
-        }
-    }
-    // a TMA copy that never completed downgrades that warp to the L1/L2 path (same results): never silent
-    if (!ctx->optTrackDebug && (ctx->trackSeq & 0xff) == 0) {
-        unsigned int tmo = 0;
-        cudaMemcpy(&tmo, ctx->trkSync + TP_SYNC_WORDS - 4, 4, cudaMemcpyDeviceToHost);
-        if (tmo != ctx->tmaTimeoutsSeen) {
-            fprintf(stderr, "[lsdgpu] warning: %u TMA window copies timed out so far (tracking falls back to L1/L2 taps for those warps)\n", tmo);
-            ctx->tmaTimeoutsSeen = tmo;
         }
     }
     out->pointUsage = hOut->pointUsage; out->lastGoodCount = hOut->goodCount; out->lastBadCount = hOut->badCount;

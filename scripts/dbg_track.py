@@ -1,4 +1,4 @@
-"""per-phase cycle counters and shared-memory-window tap rates of k_track_persistent (LSDGPU_TRACK_DEBUG=1)
+"""per-phase cycle counters of k_track_persistent (LSDGPU_TRACK_DEBUG=1)
    python scripts/dbg_track.py [width height [frames]]"""
 import os, sys, numpy as np
 sys.path.insert(0, os.getcwd())

@@ -344,11 +344,8 @@ def test_fused_call_equals_individual_calls(seq_small, frames_small):
     assert np.array_equal(outs[0][2], outs[1][2])
 
 
-@pytest.mark.parametrize("single_sync", ["0", "1"])
-def test_fused_call_divergence_leaves_map_untouched(seq_small, frames_small, single_sync, monkeypatch):
-    """frame path (also the opt-in single-sync variant, where the mapping kernels are already enqueued behind the
-    tracking kernel): when tracking diverges nothing of the map may change"""
-    monkeypatch.setenv("LSDGPU_SINGLE_SYNC", single_sync)
+def test_fused_call_divergence_leaves_map_untouched(seq_small, frames_small):
+    """frame path: when tracking diverges nothing of the map may change"""
     ctx = abi.Context(seq_small.w, seq_small.h, seq_small.K, max_frames=8)
     from lsd_slam_b200.stream import GpuStream
     gs = GpuStream(ctx, mode=1, kf_every=0, fused_call=True)
@@ -369,23 +366,6 @@ def test_fused_call_divergence_leaves_map_untouched(seq_small, frames_small, sin
     p = gs.step(3, frames_small[3][0])
     assert not gs.tracker.diverged and np.isfinite(p).all()
     ctx.close()
-
-
-def test_single_sync_variant_is_bit_identical(seq_small, frames_small, monkeypatch):
-    """LSDGPU_SINGLE_SYNC=1 (device-side prepareForStereoWith) == default path, bit for bit"""
-    from lsd_slam_b200.stream import GpuStream
-    outs = []
-    for v in ("0", "1"):
-        monkeypatch.setenv("LSDGPU_SINGLE_SYNC", v)
-        ctx = abi.Context(seq_small.w, seq_small.h, seq_small.K, max_frames=8)
-        gs = GpuStream(ctx, mode=1, kf_every=0, fused_call=True)
-        gs.init_gt(0, frames_small[0][0], frames_small[0][1])
-        for k in range(1, 6):
-            gs.step(k, frames_small[k][0])
-        outs.append((np.array(gs.poses), gs.map.current().copy()))
-        ctx.close()
-    assert np.array_equal(outs[0][0], outs[1][0])
-    assert outs[0][1].tobytes() == outs[1][1].tobytes()
 
 
 def test_reactivated_keyframe_and_multiple_reference_frames(gpu_ctx_small, oracle, seq_small, frames_small):

@@ -158,28 +158,3 @@ def test_new_context_never_sees_the_result_block_of_a_destroyed_one(seq_small, f
         first, host, _ = one(k)
         assert pose_err(first, host)[0] <= 1e-4, k
     alive.close()
-
-
-def test_tma_windows_on_and_off_track_and_map_bit_identically(monkeypatch):
-    """LSDGPU_TRACK_TMA=1 serves the tracker's taps from TMA-loaded shared-memory windows, 0 (the default) from L1/L2 with
-    no dynamic shared memory: same weights, same summation order, so the same poses and depth maps bit for bit.  640x480,
-    where 132 CTAs x 16 warps leave some warps a second level-1 chunk without a window."""
-    from lsd_slam_b200 import synth
-    from lsd_slam_b200.stream import GpuStream
-    seq = synth.Sequence(640, 480, seed=1234)
-    frames = [seq.render(k) for k in range(7)]
-    out = {}
-    for tma in ("0", "1"):
-        monkeypatch.setenv("LSDGPU_TRACK_TMA", tma)            # read when the context is created
-        ctx = abi.Context(seq.w, seq.h, seq.K, device=0, max_frames=8)
-        gs = GpuStream(ctx, mode=1, kf_every=0)
-        gs.init_gt(0, *frames[0])
-        for k in range(1, 7):
-            gs.step(k, frames[k][0])
-        out[tma] = (np.array(gs.poses), gs.map.current().copy())
-        ctx.close()
-    assert np.array_equal(out["0"][0], out["1"][0])
-    for f in abi.HYP_DTYPE.names:
-        if f != "_pad":
-            a, b = (np.ascontiguousarray(out[t][1][f]).view(np.uint8) for t in ("0", "1"))
-            assert np.array_equal(a, b), f          # as bit patterns
