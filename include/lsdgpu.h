@@ -30,7 +30,9 @@ extern "C" {
 
 #define LSDGPU_LEVELS 5                 /* PYRAMID_LEVELS, util/settings.h:106 */
 /* 2: additive over 1 -- lsdgpu_get_globals, lsdgpu_depth_update_keyframe_refs (lsdgpu_ref_desc), lsdgpu_seq_sum_f32,
- *    lsdgpu_peer_export / _attach / _detach; contexts are thread-safe (per-context mutex).  No existing signature changed. */
+ *    lsdgpu_peer_export / _attach / _detach; contexts are thread-safe (per-context mutex).  No existing signature changed.
+ *    lsdgpu_track_and_map_group (lsdgpu_group_step) was added later without a version change, also additively: find it by
+ *    symbol lookup (dlsym) rather than by the version number. */
 #define LSDGPU_ABI_VERSION 2
 
 typedef struct lsdgpu_ctx lsdgpu_ctx;
@@ -176,6 +178,30 @@ int lsdgpu_se3_track(lsdgpu_ctx* ctx, int kf_id, int frame_id, const double fram
 int lsdgpu_track_and_map(lsdgpu_ctx* ctx, int kf_id, int frame_id, const uint8_t* gray, int stage_index,
                          const double frameToRef_init_qt[7], const lsdgpu_track_settings* s, int mode,
                          int keyframe_change, lsdgpu_track_result* out, double new_kf_thisToParent_qts[8]);
+
+/* Several independent streams on one GPU: K SlamSystems (one camera each, one context each) advanced by one frame each in one
+ * call, in the order of SlamSystem::trackFrame (SlamSystem.cpp:890-1040) followed by SlamSystem::doMappingIteration (SlamSystem.cpp:739-828)
+ * per stream.  The call equals lsdgpu_track_and_map(steps[i]..., mode = 1, ...) for i = 0..n-1 issued one after the other, bit
+ * for bit (tracking results, new keyframes' thisToParent, refPixelWasGood masks, frame poses and counters, depth maps), but the
+ * trackings of all n frames share ONE cooperative launch in which each stream gets floor(SMs / n) SMs and its own grid barrier.
+ * Each step's Frame construction and mapping run on its own context's stream, so the mapping of different streams can overlap.
+ * A step whose tracking diverges skips its own mapping (as the single call does); the others still map.
+ * Requirements: 1 <= n <= 8; distinct contexts, all on the same device and of the same width x height; none peer-attached
+ * (lsdgpu_peer_attach).  Otherwise, or for an unknown keyframe id, nothing is done, the call returns an error and every context
+ * of the group carries a message naming the step.  The call locks all n contexts (in ascending address order).
+ * new_kf_thisToParent_qts: 8 doubles per step (written for the steps with keyframe_change != 0), or NULL. */
+typedef struct {
+    lsdgpu_ctx* ctx;                      /* the stream's context */
+    int kf_id, frame_id;
+    const uint8_t* gray;                  /* HOST image, or NULL: prefetch-ring entry stage_index */
+    int stage_index;
+    double frameToRef_init_qt[7];
+    const lsdgpu_track_settings* settings;  /* NULL: the main tracker's defaults, as lsdgpu_se3_track */
+    int keyframe_change;
+} lsdgpu_group_step;
+/* SlamSystem.cpp:890-1040 + SlamSystem.cpp:739-828 for n streams, one tracking launch (see above) */
+int lsdgpu_track_and_map_group(int n, const lsdgpu_group_step* steps, lsdgpu_track_result* results,
+                               double* new_kf_thisToParent_qts);
 
 /* ---- input staging: UndistorterPTAM fused into the Frame construction (SURVEY 8f row 3) ----------------------------
  * UndistorterPTAM::UndistorterPTAM, util/Undistorter.cpp:171-317, with the four lines of the calibration file already parsed:

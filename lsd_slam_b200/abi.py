@@ -74,6 +74,16 @@ class EvalResult(C.Structure):
                 ("sxx", C.c_float), ("syy", C.c_float), ("sx", C.c_float), ("sy", C.c_float), ("sw", C.c_float)]
 
 
+class GroupStep(C.Structure):
+    """lsdgpu_group_step (include/lsdgpu.h): one stream's frame in lsdgpu_track_and_map_group"""
+    _fields_ = [("ctx", C.c_void_p), ("kf_id", C.c_int), ("frame_id", C.c_int), ("gray", C.POINTER(C.c_uint8)),
+                ("stage_index", C.c_int), ("frameToRef_init_qt", C.c_double * 7), ("settings", C.POINTER(TrackSettings)),
+                ("keyframe_change", C.c_int)]
+
+
+GROUP_MAX_STEPS = 8
+
+
 # every symbol include/lsdgpu.h declares: (name, restype, argtypes)
 _vp, _fp, _dp, _ip, _u8p = C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_double), C.POINTER(C.c_int), C.POINTER(C.c_uint8)
 class Sim3Result(C.Structure):
@@ -124,6 +134,7 @@ SYMBOLS = [
     ("lsdgpu_se3_eval", C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _fp, C.c_float, C.c_float, C.POINTER(TrackSettings), C.c_int, C.POINTER(EvalResult)]),
     ("lsdgpu_se3_track", C.c_int, [_vp, C.c_int, C.c_int, _dp, C.POINTER(TrackSettings), C.c_int, C.POINTER(TrackResult)]),
     ("lsdgpu_track_and_map", C.c_int, [_vp, C.c_int, C.c_int, _u8p, C.c_int, _dp, C.POINTER(TrackSettings), C.c_int, C.c_int, C.POINTER(TrackResult), _dp]),
+    ("lsdgpu_track_and_map_group", C.c_int, [C.c_int, C.POINTER(GroupStep), C.POINTER(TrackResult), _dp]),
     ("lsdgpu_undistorter_ptam_prepare", C.c_int, [_fp, C.c_int, C.c_int, _fp, C.c_int, C.c_int, _fp, _fp, _fp]),
     ("lsdgpu_undistorter_validate_tables", C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, _fp, _fp]),
     ("lsdgpu_set_undistorter", C.c_int, [_vp, C.c_int, C.c_int, _fp, _fp]),

@@ -152,6 +152,11 @@ struct lsdgpu_ctx {
     int nRanks = 1, rank = 0;
     char* peerBase[8] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };
     unsigned int trkTailBase = 0;
+    // several contexts tracked in one launch (lsdgpu_track_and_map_group)
+    uint8_t* dLastMask = nullptr;        // level-1 flags of the last candidate of a pass (w*h/4 bytes)
+    void* dGroupSegs = nullptr;          // TP_MAX_GROUP segment descriptors of a group launched on this context's stream (device)
+    void* hGroupSegs = nullptr;          // their pinned staging
+    cudaEvent_t groupEvent = nullptr;    // orders the group launch after the other streams' work and their later work after it
     bool optTrackDebug = false;          // LSDGPU_TRACK_DEBUG, read once at lsdgpu_create
     int2* seqTable = nullptr;            // seqsum.cuh: per-run maps of the sequential fp32 sum, [SEQ_NBIN][runs]
     unsigned char* seqFlags = nullptr;

@@ -12,6 +12,7 @@
 #include "output.cuh"
 
 #include <algorithm>
+#include <functional>
 #include <stdlib.h>
 #include <new>
 
@@ -92,7 +93,7 @@ extern "C" int lsdgpu_create(int device, int width, int height, const float K[9]
     const int maxBlocks = divUp((int)n0, EVAL_THREADS) + 8;
     size_t scratch = alignUp((size_t)maxBlocks * EV_NCH * 4 + 65536, 256) + 4096 + alignUp(sizeof(ObserveParams), 256)
                      + 2 * alignUp(n0, 256) + alignUp(n0 * 32, 256) + alignUp((size_t)maxBlocks * 2 * 8 + 64, 256) + (256 + 2 * alignUp((n0 >> 8) * 16, 256) + 2 * alignUp(n0 * 4, 256) + alignUp(n0, 256)) * (size_t)max_frames + alignUp(n0 * 12, 256) + alignUp(LSD_MAX_PERMA_BATCH * (sizeof(PermaItem) + sizeof(PermaResult)), 256) + 1024 + alignUp(S3_MAX_BATCH * sizeof(Sim3Item), 256) + alignUp(S3_MAX_BATCH * sizeof(Sim3Out), 256)
-                     + 7936 + TP_SYNC_WORDS * 4;
+                     + 7936 + TP_SYNC_WORDS * 4 + alignUp(n0 / 4, 256) + alignUp(TP_MAX_GROUP * sizeof(TrackGroupSeg), 256);
     const int seqRuns = divUp((int)n0, SEQ_RUN);
     scratch += alignUp((size_t)seqRuns * SEQ_NBIN * sizeof(int2), 256) + alignUp((size_t)seqRuns, 256) + alignUp((size_t)seqRuns * 4, 256);
     ctx->arenaBytes = perFrame * max_frames + depthBytes + scratch;
@@ -144,6 +145,8 @@ extern "C" int lsdgpu_create(int device, int width, int height, const float K[9]
     ctx->seqTable = (int2*)take((size_t)seqRuns * SEQ_NBIN * sizeof(int2));
     ctx->seqFlags = (unsigned char*)take((size_t)seqRuns);
     ctx->seqCounts = (int*)take((size_t)seqRuns * 4);
+    ctx->dLastMask = (uint8_t*)take(n0 / 4);
+    ctx->dGroupSegs = take(TP_MAX_GROUP * sizeof(TrackGroupSeg));
     if ((size_t)(p - ctx->arena) > ctx->arenaBytes) return lsd_fail(ctx, "arena overflow");
 
     LSD_CHECK(ctx, cudaHostAlloc((void**)&ctx->hEvOut, EV_NCH * 4, cudaHostAllocDefault));
@@ -154,6 +157,8 @@ extern "C" int lsdgpu_create(int device, int width, int height, const float K[9]
     }
     LSD_CHECK(ctx, cudaHostAlloc((void**)&ctx->hStageF, n0 * 32, cudaHostAllocDefault));
     LSD_CHECK(ctx, cudaHostAlloc((void**)&ctx->hScalars, 64, cudaHostAllocDefault));
+    LSD_CHECK(ctx, cudaHostAlloc(&ctx->hGroupSegs, TP_MAX_GROUP * sizeof(TrackGroupSeg), cudaHostAllocDefault));
+    LSD_CHECK(ctx, cudaEventCreateWithFlags(&ctx->groupEvent, cudaEventDisableTiming));
     // the tracker writes its result block straight into mapped pinned memory (no D2H copy on the path)
     LSD_CHECK(ctx, cudaHostAlloc((void**)&ctx->hTrackState, sizeof(TrackState), cudaHostAllocMapped));
     // cudaHostAlloc does not clear: a recycled block may still hold the result of a destroyed context, whose doneSeq would satisfy
@@ -190,6 +195,8 @@ extern "C" void lsdgpu_destroy(lsdgpu_ctx* ctx)
     cudaFreeHost(ctx->hEvOut); cudaFreeHost(ctx->hStage[0]); cudaFreeHost(ctx->hStage[1]); cudaFreeHost(ctx->hStageF);
     cudaEventDestroy(ctx->stageDone[0]); cudaEventDestroy(ctx->stageDone[1]);
     cudaFreeHost(ctx->hScalars); cudaFreeHost(ctx->hTrackState);
+    if (ctx->hGroupSegs) cudaFreeHost(ctx->hGroupSegs);
+    if (ctx->groupEvent) cudaEventDestroy(ctx->groupEvent);
     for (int i = 0; i < 8; i++) { if (ctx->tBegin[i]) cudaEventDestroy(ctx->tBegin[i]); if (ctx->tEnd[i]) cudaEventDestroy(ctx->tEnd[i]); }
     if (ctx->kBegin) cudaEventDestroy(ctx->kBegin);
     if (ctx->kEnd) cudaEventDestroy(ctx->kEnd);
@@ -1244,6 +1251,111 @@ extern "C" int lsdgpu_track_and_map(lsdgpu_ctx* ctx, int kf_id, int frame_id, co
     r = lsdgpu_depth_update_keyframe(ctx, &frame_id, 1);
     if (r) return r;
     return lsdgpu_frame_clear_good_mask(ctx, frame_id);
+}
+
+// ------------------------------------------------------------------------------------------------------
+// several streams per GPU: one tracking launch for the frames of n contexts
+// ------------------------------------------------------------------------------------------------------
+// the message goes to every context of the group (each one's own lock is taken again: recursive)
+static int groupFail(int n, const lsdgpu_group_step* steps, int step, const char* msg, int rc = -2)
+{
+    char b[600];
+    if (step >= 0) snprintf(b, sizeof(b), "track_and_map_group: step %d: %s", step, msg);
+    else snprintf(b, sizeof(b), "track_and_map_group: %s", msg);
+    for (int i = 0; i < n; i++)
+        if (steps[i].ctx) { CtxLock l(steps[i].ctx); steps[i].ctx->err = b; }
+    return rc;
+}
+// an entry point called for step `step` failed and set its context's message: hand it to the whole group
+static int groupPropagate(int n, const lsdgpu_group_step* steps, int step, int rc)
+{
+    const std::string m = steps[step].ctx->err;
+    return groupFail(n, steps, step, m.c_str(), rc);
+}
+
+extern "C" int lsdgpu_track_and_map_group(int n, const lsdgpu_group_step* steps, lsdgpu_track_result* results, double* new_qts)
+{
+    if (!steps || n < 1) return -2;
+    if (n > TP_MAX_GROUP) return groupFail(n, steps, -1, "the number of steps must be 1..8");
+    for (int i = 0; i < n; i++)
+        if (!steps[i].ctx) return groupFail(n, steps, i, "null context");
+    if (!results) return groupFail(n, steps, -1, "null result array");
+    for (int i = 1; i < n; i++)
+        for (int j = 0; j < i; j++)
+            if (steps[i].ctx == steps[j].ctx) return groupFail(n, steps, i, "the same context as an earlier step");
+    // every context's lock for the whole call, taken in ascending address order: two threads issuing overlapping groups cannot deadlock
+    lsdgpu_ctx* order[TP_MAX_GROUP];
+    for (int i = 0; i < n; i++) order[i] = steps[i].ctx;
+    std::sort(order, order + n, std::less<lsdgpu_ctx*>());
+    std::unique_lock<std::recursive_mutex> locks[TP_MAX_GROUP];
+    for (int i = 0; i < n; i++) locks[i] = std::unique_lock<std::recursive_mutex>(order[i]->mu);
+
+    lsdgpu_ctx* c0 = steps[0].ctx;
+    for (int i = 0; i < n; i++) {
+        const lsdgpu_ctx* c = steps[i].ctx;
+        if (c->device != c0->device) return groupFail(n, steps, i, "context is on another device than step 0's");
+        if (c->w != c0->w || c->h != c0->h) return groupFail(n, steps, i, "context size differs from step 0's");
+        if (c->nRanks > 1) return groupFail(n, steps, i, "context is peer-attached (a sharded stream cannot be grouped)");
+        if (!findSlot(steps[i].ctx, steps[i].kf_id)) return groupFail(n, steps, i, "unknown frame id (keyframe)");
+    }
+    if (cudaSetDevice(c0->device) != cudaSuccess) return groupFail(n, steps, -1, "cudaSetDevice failed", -1);
+
+    // 1. per step, on its own stream: Frame construction, importFrame if the keyframe's depth changed (SlamSystem.cpp:907-912)
+    lsdgpu_ctx* ctxs[TP_MAX_GROUP];
+    FrameSlot* kfs[TP_MAX_GROUP];
+    FrameSlot* frs[TP_MAX_GROUP];
+    const double* inits[TP_MAX_GROUP];
+    const lsdgpu_track_settings* sts[TP_MAX_GROUP];
+    lsdgpu_track_settings ds[TP_MAX_GROUP];
+    for (int i = 0; i < n; i++) {
+        const lsdgpu_group_step& st = steps[i];
+        lsdgpu_ctx* ctx = st.ctx;
+        ctxs[i] = ctx;
+        int r = st.gray ? lsdgpu_frame_upload_u8(ctx, st.frame_id, st.gray) : lsdgpu_frame_from_stage(ctx, st.frame_id, st.stage_index);
+        if (r) return groupPropagate(n, steps, i, r);
+        kfs[i] = findSlot(ctx, st.kf_id);
+        frs[i] = findSlot(ctx, st.frame_id);
+        if (!kfs[i] || !frs[i]) return groupFail(n, steps, i, "unknown frame id");
+        if (kfs[i]->depthHasBeenUpdatedFlag) {
+            r = lsdgpu_ref_import(ctx, st.kf_id);
+            if (r) return groupPropagate(n, steps, i, r);
+        }
+        r = ensureIdepthPyramid(ctx, kfs[i]);                // as lsdgpu_se3_track
+        if (r) return groupPropagate(n, steps, i, r);
+        inits[i] = st.frameToRef_init_qt;
+        sts[i] = st.settings;
+        if (!sts[i]) { lsdgpu_default_track_settings(&ds[i]); ds[i].maxItsPerLvl[4] = 0; sts[i] = &ds[i]; }
+    }
+    // 2-5. one launch on steps[0]'s stream for all the frames
+    int failed = 0;
+    int r = trackPersistentGroup(n, ctxs, kfs, frs, inits, sts, results, &failed);
+    if (r) return groupPropagate(n, steps, failed, r);
+    for (int i = 0; i < n; i++) {                            // the Frame side effects of lsdgpu_se3_track
+        const lsdgpu_track_result* out = &results[i];
+        if (out->diverged) continue;
+        if (out->trackingWasGood) kfs[i]->numFramesTrackedOnThis++;                       // SE3Tracker.cpp:479-480
+        frs[i]->initialTrackedResidual = out->initialTrackedResidual;                     // :482
+        for (int k = 0; k < 7; k++) frs[i]->thisToParent[k] = out->frameToRef_qt[k];      // :483
+        frs[i]->thisToParent[7] = 1.0;
+        frs[i]->parentId = kfs[i]->id;                                                    // :484
+    }
+    // 6. mapping, each step on its own stream; a diverged step maps nothing.  The contexts are independent, so the order across
+    // steps is free: the keyframe changes, whose createKeyFrame waits for its stream, go last so that the updates of the other
+    // streams are already in flight.
+    for (int pass = 0; pass < 2; pass++)
+        for (int i = 0; i < n; i++) {
+            const lsdgpu_group_step& st = steps[i];
+            if (results[i].diverged || (st.keyframe_change != 0) != (pass == 1)) continue;
+            if (st.keyframe_change) {
+                r = lsdgpu_depth_finalize_keyframe(st.ctx);
+                if (!r) r = lsdgpu_depth_create_keyframe(st.ctx, st.frame_id, new_qts ? new_qts + 8 * i : nullptr);
+            } else {
+                r = lsdgpu_depth_update_keyframe(st.ctx, &st.frame_id, 1);
+                if (!r) r = lsdgpu_frame_clear_good_mask(st.ctx, st.frame_id);
+            }
+            if (r) return groupPropagate(n, steps, i, r);
+        }
+    return 0;
 }
 
 // ------------------------------------------------------------------------------------------------------

@@ -39,6 +39,7 @@
 #define TP_TAIL_OFFSET 3200          // word: arrival counter of the end-of-kernel barrier of a sharded launch
 #define TP_KMAX 3                    // poses per pass: the try + up to two speculative successors
 #define TP_ROW 64                    // floats per exchange row (256 B, one row per CTA; EV_NCHX = 56 used)
+#define TP_MAX_GROUP 8               // streams one group launch can track (lsdgpu_track_and_map_group)
 
 struct TrackLevelParams {
     const float* kfIdepth;
@@ -93,6 +94,28 @@ struct TrackState {
     volatile unsigned int doneSeq;   // written last (after a system-wide fence): the host polls it instead of a stream sync
     long long cyc[6];                // block-0 cycle breakdown: points, CTA reduce, barrier, combine, serial LM, total
     long long cycBlk[TP_MAXGRID][6];   // the same per CTA (debug); the last row holds warp 0's cycles
+};
+
+// ---- several streams in one launch (k_track_persistent_group) ------------------------------------------------------------------
+// The launch is cut into n segments of Gs = floor(trackGrid / n) CTAs; segment s tracks stream s with its own parameters, partial
+// rows, barrier counter and result block.  A segment keeps the single-stream launch's VIRTUAL grid of Gv = trackGrid CTAs: its
+// physical CTA b stands in for the virtual CTAs b, b + Gs, ... < Gv one after the other, evaluating exactly the chunks, with the
+// same warp / lane mapping, and writing exactly the row that virtual CTA writes in a single-stream launch.  The combine then adds
+// the same Gv rows in the same order, so every sum, every LM decision and every result is bit-identical to k_track_persistent's.
+// A native grid of Gs CTAs would deal the chunks out differently and change the fp32 summation order.
+struct TrackGroupSeg {
+    TrackParams p;                   // the stream's parameters (nRanks == 1, debug == 0)
+    TrackState* out;                 // its context's mapped result block
+    uint8_t* lastMask;               // level-1 scratch of its context: the last candidate's good flags (ThreadCarry::lastBits
+                                     // would need up to ceil(Gv / Gs) times as many bits)
+};
+
+// where a CTA sits in a group launch (unused by the single-stream instantiation)
+struct SegGrid {
+    int b;                           // physical CTA within the segment
+    int Gs;                          // physical CTAs of the segment (the barrier counts these)
+    int Gv;                          // virtual grid (rows of the combine) = the single-stream launch's grid
+    uint8_t* lastMask;
 };
 
 // Grid-wide barrier.  Arrivals are counted on one word (monotonic: epoch e completes at base + e * gridDim arrivals, the
@@ -276,99 +299,111 @@ __device__ __forceinline__ void gridTailRanks(const TrackParams& p)
     __syncthreads();
 }
 
-__device__ __forceinline__ void gridEvaluate(const TrackParams& p, int lvl, LMShared& sh, float (*sm)[EV_NCHX], float (*comb)[TP_ROW],
-                                             unsigned int& epoch, long long* cyc, ThreadCarry& tc)
+template <bool GROUP>
+__device__ __forceinline__ void gridEvaluate(const TrackParams& p, const SegGrid& sg, int lvl, LMShared& sh, float (*sm)[EV_NCHX],
+                                             float (*comb)[TP_ROW], unsigned int& epoch, long long* cyc, ThreadCarry& tc)
 {
-    long long t0 = clock64();
+    long long t0 = clock64(), t1;
     const TrackLevelParams& L = p.lvl[lvl];
     const int K = sh.nPose;
     const EvalPose P = sh.pose[0];
-    PointAcc acc;
-    float ext[EV_NX];
-#pragma unroll
-    for (int c = 0; c < EV_NCH; c++) acc.v[c] = 0.f;
-#pragma unroll
-    for (int c = 0; c < EV_NX; c++) ext[c] = 0.f;
-    const int w = L.w, h = L.h, iw = L.iw, nInt = L.nInt, G = (int)gridDim.x;
+    const int w = L.w, h = L.h, iw = L.iw, nInt = L.nInt, G = GROUP ? sg.Gs : (int)gridDim.x;
     const float4* fg = L.frameGrad;
     uint8_t* mask = (lvl == SE3TRACKING_MIN_LEVEL) ? p.goodMask : nullptr;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     // chunks of this CTA: tpChunkOf(b, k, G), k = 0 .. nSlots-1 where it exists; warp `warp` takes k = warp, warp + 16, ...
-    // sharded over nRanks GPUs: the CTAs of all ranks form one virtual grid (this CTA is number b * nRanks + rank of it)
-    const int Gv = G * p.nRanks, vb = (int)blockIdx.x * p.nRanks + p.rank;
+    // sharded over nRanks GPUs: the CTAs of all ranks form one virtual grid (this CTA is number b * nRanks + rank of it).
+    // In a group launch the CTA runs the virtual CTAs sg.b, sg.b + Gs, ... of the segment's virtual grid in turn.
+    const int Gv = GROUP ? sg.Gv : G * p.nRanks;
+    int vb = GROUP ? sg.b : (int)blockIdx.x * p.nRanks + p.rank;
     const int nSlots = (L.nChunks + Gv - 1) / Gv;
-    if (mask) { tc.lastBits = 0u; tc.pointBits = 0u; }
-    int slot = 0;
-    for (int k = warp; k < nSlots; k += TP_WARPS, slot++) {
-        const int chunk = tpChunkOf(vb, k, Gv);
-        if (chunk >= L.nChunks) continue;                              // warp-uniform
-        const int j = (chunk << 5) + lane;                             // interior pixel number
-        const bool firstChunk = (k == warp);
-        bool isPoint = false;
-        float px = 0.f, py = 0.f, pz = 0.f, var = 0.f, color = 0.f;
-        int i = 0;
-        if (j < nInt) {
-            const int yy = j / iw;
-            i = (j - yy * iw + 1) + (yy + 1) * w;                      // x = 1 + j % iw, y = 1 + j / iw
-        }
-        if (firstChunk && tc.pcLvl == lvl) {
-            // the thread's first pixel of a level never changes between the passes of that level: keep the
-            // reconstructed point in registers instead of re-reading the keyframe planes (an L2 round trip at the head
-            // of every pass's dependency chain)
-            isPoint = tc.pcIsPoint; px = tc.pcx; py = tc.pcy; pz = tc.pcz; var = tc.pcVar; color = tc.pcColor;
-        } else {
+    if (!GROUP && mask) { tc.lastBits = 0u; tc.pointBits = 0u; }
+    const int nch = K > 1 ? EV_NCHX : EV_NCH;
+    const unsigned int parity = epoch & 1u;
+    float* part = p.partials + (size_t)parity * TP_ROW * (GROUP ? (unsigned int)Gv : gridDim.x);
+    do {
+        PointAcc acc;
+        float ext[EV_NX];
+#pragma unroll
+        for (int c = 0; c < EV_NCH; c++) acc.v[c] = 0.f;
+#pragma unroll
+        for (int c = 0; c < EV_NX; c++) ext[c] = 0.f;
+        int slot = 0;
+        for (int k = warp; k < nSlots; k += TP_WARPS, slot++) {
+            const int chunk = tpChunkOf(vb, k, Gv);
+            if (chunk >= L.nChunks) continue;                              // warp-uniform
+            const int j = (chunk << 5) + lane;                             // interior pixel number
+            const bool firstChunk = (k == warp) && (!GROUP || vb == sg.b);  // the point cache holds the first virtual CTA's pixel
+            bool isPoint = false;
+            float px = 0.f, py = 0.f, pz = 0.f, var = 0.f, color = 0.f;
+            int i = 0;
             if (j < nInt) {
-                const float idepth = __ldg(L.kfIdepth + i);
-                var = __ldg(L.kfVar + i);
-                if (!(var <= 0 || idepth == 0)) {                      // TrackingReference.cpp:133
-                    const int yy = j / iw, x = j - yy * iw + 1, y = yy + 1;
-                    const float sc = 1.0f / idepth;
-                    px = sc * (L.fxi * x + L.cxi); py = sc * (L.fyi * y + L.cyi); pz = sc * 1;
-                    color = __ldg(L.kfColor + i);
-                    isPoint = true;
+                const int yy = j / iw;
+                i = (j - yy * iw + 1) + (yy + 1) * w;                      // x = 1 + j % iw, y = 1 + j / iw
+            }
+            if (firstChunk && tc.pcLvl == lvl) {
+                // the thread's first pixel of a level never changes between the passes of that level: keep the
+                // reconstructed point in registers instead of re-reading the keyframe planes (an L2 round trip at the head
+                // of every pass's dependency chain)
+                isPoint = tc.pcIsPoint; px = tc.pcx; py = tc.pcy; pz = tc.pcz; var = tc.pcVar; color = tc.pcColor;
+            } else {
+                if (j < nInt) {
+                    const float idepth = __ldg(L.kfIdepth + i);
+                    var = __ldg(L.kfVar + i);
+                    if (!(var <= 0 || idepth == 0)) {                      // TrackingReference.cpp:133
+                        const int yy = j / iw, x = j - yy * iw + 1, y = yy + 1;
+                        const float sc = 1.0f / idepth;
+                        px = sc * (L.fxi * x + L.cxi); py = sc * (L.fyi * y + L.cyi); pz = sc * 1;
+                        color = __ldg(L.kfColor + i);
+                        isPoint = true;
+                    }
+                }
+                if (firstChunk) {
+                    tc.pcLvl = lvl; tc.pcIsPoint = isPoint;
+                    tc.pcx = px; tc.pcy = py; tc.pcz = pz; tc.pcVar = var; tc.pcColor = color;
                 }
             }
-            if (firstChunk) {
-                tc.pcLvl = lvl; tc.pcIsPoint = isPoint;
-                tc.pcx = px; tc.pcy = py; tc.pcz = pz; tc.pcVar = var; tc.pcColor = color;
+            if (isPoint) {
+                auto tap = [fg, w](float u, float v, float& o0, float& o1, float& o2) { interp43(fg, u, v, w, o0, o1, o2); };
+                const int good = evalPoint(px, py, pz, color, var, P, p.C, L.fx, L.fy, L.cx, L.cy, w, h, tap, acc);
+                if (K > 1) {                                               // block-uniform
+                    if (K > 2) evalPointLight<false>(px, py, pz, color, var, sh.pose[1], p.C, L.fx, L.fy, L.cx, L.cy, w, h, tap, ext);
+                    const int goodL = evalPointLight<true>(px, py, pz, color, var, sh.pose[K - 1], p.C, L.fx, L.fy, L.cx, L.cy, w, h, tap, ext);
+                    if (mask) {
+                        if (GROUP) sg.lastMask[i] = (uint8_t)goodL;
+                        else tc.lastBits |= (unsigned int)goodL << slot;
+                    }
+                }
+                if (mask) {
+                    mask[i] = (uint8_t)good;
+                    if (!GROUP) tc.pointBits |= 1u << slot;
+                    if (!GROUP && p.nRanks > 1)                            // the other ranks own other chunks: give them this one's flag
+                        for (int d = 0; d < p.nRanks; d++) if (d != p.rank) p.peerMask[d][i] = (uint8_t)good;
+                }
             }
         }
-        if (isPoint) {
-            auto tap = [fg, w](float u, float v, float& o0, float& o1, float& o2) { interp43(fg, u, v, w, o0, o1, o2); };
-            const int good = evalPoint(px, py, pz, color, var, P, p.C, L.fx, L.fy, L.cx, L.cy, w, h, tap, acc);
-            if (K > 1) {                                               // block-uniform
-                if (K > 2) evalPointLight<false>(px, py, pz, color, var, sh.pose[1], p.C, L.fx, L.fy, L.cx, L.cy, w, h, tap, ext);
-                const int goodL = evalPointLight<true>(px, py, pz, color, var, sh.pose[K - 1], p.C, L.fx, L.fy, L.cx, L.cy, w, h, tap, ext);
-                if (mask) tc.lastBits |= (unsigned int)goodL << slot;
-            }
-            if (mask) {
-                mask[i] = (uint8_t)good; tc.pointBits |= 1u << slot;
-                if (p.nRanks > 1)                                      // the other ranks own other chunks: give them this one's flag
-                    for (int d = 0; d < p.nRanks; d++) if (d != p.rank) p.peerMask[d][i] = (uint8_t)good;
-            }
-        }
-    }
-    __syncthreads();
-    long long t1 = clock64();
-    warpReduceAcc(acc, lane, sm[warp]);
-    if (K > 1) warpReduceExt(ext, lane, sm[warp]);
-    __syncthreads();
-    const int nch = K > 1 ? EV_NCHX : EV_NCH;
-    float ctaSum = 0.f;
-    if (threadIdx.x < nch) {
+        __syncthreads();
+        t1 = clock64();
+        warpReduceAcc(acc, lane, sm[warp]);
+        if (K > 1) warpReduceExt(ext, lane, sm[warp]);
+        __syncthreads();
+        float ctaSum = 0.f;
+        if (threadIdx.x < nch) {
 #pragma unroll
-        for (int wi = 0; wi < TP_WARPS; wi++) ctaSum += sm[wi][threadIdx.x];
-    }
-    // ---- exchange: ONE 256-byte row per CTA ([parity][cta][64 floats], written through to L2 as one coalesced store),
-    // ONE grid barrier, then every CTA combines all rows in a fixed order.  (Round 1 laid the buffer out [channel][cta]:
-    // 40 four-byte writes per CTA into lines shared with 31 other CTAs -- 5 920 partial-sector writes per pass behind the
-    // release of the barrier, and the combine's loads then waited ~5 000 cycles on those lines: 25 % of the kernel, ncu.)
-    const unsigned int parity = epoch & 1u;
-    float* part = p.partials + (size_t)parity * TP_ROW * gridDim.x;
-    if (threadIdx.x < nch) __stcg(part + (size_t)blockIdx.x * TP_ROW + threadIdx.x, ctaSum);
+            for (int wi = 0; wi < TP_WARPS; wi++) ctaSum += sm[wi][threadIdx.x];
+        }
+        // ---- exchange: ONE 256-byte row per CTA ([parity][cta][64 floats], written through to L2 as one coalesced store),
+        // ONE grid barrier, then every CTA combines all rows in a fixed order.  (Round 1 laid the buffer out [channel][cta]:
+        // 40 four-byte writes per CTA into lines shared with 31 other CTAs -- 5 920 partial-sector writes per pass behind the
+        // release of the barrier, and the combine's loads then waited ~5 000 cycles on those lines: 25 % of the kernel, ncu.)
+        // A group launch writes the row of every virtual CTA it stands in for; the next one reuses sm only after the
+        // __syncthreads that ends its chunk loop.
+        if (threadIdx.x < nch) __stcg(part + (size_t)(GROUP ? (unsigned int)vb : blockIdx.x) * TP_ROW + threadIdx.x, ctaSum);
+        vb += G;
+    } while (GROUP && vb < Gv);
     epoch++;
     long long t2 = clock64();
-    gridBarrier(p.sync, p.barrierBase + epoch * gridDim.x);
+    gridBarrier(p.sync, p.barrierBase + epoch * (GROUP ? (unsigned int)G : gridDim.x));
     long long t3 = clock64();
     // warp wi adds rows wi, wi+16, ... (<= 10): the lower half-warp takes the even ones of those, the upper half the odd ones, each
     // lane one float4 (4 channels) of a 256-byte row -- 5 vector loads per thread, all in flight before the first add.  fp32 adds
@@ -376,7 +411,7 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, int lvl, LMSh
     // the same additions in the same order on the same data, so the totals are bit-identical everywhere, and the sums stay in
     // the precision the per-point accumulators and the reference's own (sequential fp32) sums have.
     {
-        const int nb = (int)gridDim.x;
+        const int nb = GROUP ? Gv : (int)gridDim.x;
         const int half = lane >> 4, q = lane & 15;
         constexpr int NR = (TP_MAXGRID / TP_WARPS + 1) / 2;
         float4 v[NR];
@@ -402,7 +437,7 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, int lvl, LMSh
         sh.sums[threadIdx.x] = t;
     }
     __syncthreads();
-    if (p.nRanks > 1) gridExchangeRanks(p, sh, nch, (p.launchSeq << 16) | (epoch & 0xffffu), epoch & 1u);
+    if (!GROUP && p.nRanks > 1) gridExchangeRanks(p, sh, nch, (p.launchSeq << 16) | (epoch & 0xffffu), epoch & 1u);
     long long t4 = clock64();
     cyc[0] += t1 - t0; cyc[1] += t2 - t1; cyc[2] += t3 - t2; cyc[3] += t4 - t3;
 }
@@ -727,7 +762,10 @@ __device__ __forceinline__ void lmAdvance(const TrackParams& p, LMState& lm, LMS
     }
 }
 
-__global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid_constant__ TrackParams p, TrackState* __restrict__ out)
+// The tracker of one stream.  GROUP = false: the whole grid (k_track_persistent); GROUP = true: one segment of a group launch
+// (k_track_persistent_group), whose position `sg` gives.  Both instantiations run the same passes, decisions and combine.
+template <bool GROUP>
+__device__ __forceinline__ void trackStream(const TrackParams& p, TrackState* __restrict__ out, const SegGrid& sg)
 {
     __shared__ alignas(LMShared) unsigned char shStorage[sizeof(LMShared)];   // raw storage: Cand holds a type with a constructor
     LMShared& sh = *reinterpret_cast<LMShared*>(shStorage);
@@ -747,7 +785,8 @@ __global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid
     // fresh refPixelWasGood mask: all true (Frame.h:433); ordered before the level-1 passes by the barriers
     if (p.maskFresh) {
         uint32_t* m32 = reinterpret_cast<uint32_t*>(p.goodMask);
-        for (int i = blockIdx.x * TP_THREADS + threadIdx.x; i < p.maskBytes / 4; i += gridDim.x * TP_THREADS) m32[i] = 0x01010101u;
+        if (GROUP) for (int i = sg.b * TP_THREADS + threadIdx.x; i < p.maskBytes / 4; i += sg.Gs * TP_THREADS) m32[i] = 0x01010101u;
+        else for (int i = blockIdx.x * TP_THREADS + threadIdx.x; i < p.maskBytes / 4; i += gridDim.x * TP_THREADS) m32[i] = 0x01010101u;
     }
 
     if (threadIdx.x == 0) {
@@ -765,7 +804,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid
 
     while (true) {
         const int lvl = sh.lvl;
-        gridEvaluate(p, lvl, sh, sm, comb, epoch, cyc, tc);
+        gridEvaluate<GROUP>(p, sg, lvl, sh, sm, comb, epoch, cyc, tc);
         if (threadIdx.x < 32) {
             if (threadIdx.x == 0) { lm.nEval[lvl]++; lm.nPts[lvl] = sh.sums[CH_REFNUM]; }
             lmAdvance(p, lm, sh, threadIdx.x);
@@ -776,7 +815,23 @@ __global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid
 
     // The mask holds the flags of candidate 0 of the last level-1 pass; if the last pose the reference evaluates was the chain's
     // last candidate instead, its flags (kept per thread) replace them now.  Same threads, same pixels: no synchronisation.
-    if (lm.commitLast && p.minLevel == SE3TRACKING_MIN_LEVEL) {
+    if (GROUP && lm.commitLast && p.minLevel == SE3TRACKING_MIN_LEVEL) {
+        // group launch: the flags are in sg.lastMask, written by this thread in the last pass for every point it evaluated; the
+        // points are found again from the keyframe planes (the test of gridEvaluate)
+        const TrackLevelParams& L = p.lvl[SE3TRACKING_MIN_LEVEL];
+        const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+        const int nSlots = (L.nChunks + sg.Gv - 1) / sg.Gv;
+        for (int v = sg.b; v < sg.Gv; v += sg.Gs)
+            for (int k = warp; k < nSlots; k += TP_WARPS) {
+                const int j = (tpChunkOf(v, k, sg.Gv) << 5) + lane;
+                if (j >= L.nInt) continue;
+                const int yy = j / L.iw;
+                const int i = (j - yy * L.iw + 1) + (yy + 1) * L.w;
+                const float idepth = L.kfIdepth[i], var = L.kfVar[i];
+                if (!(var <= 0 || idepth == 0)) p.goodMask[i] = sg.lastMask[i];
+            }
+    }
+    if (!GROUP && lm.commitLast && p.minLevel == SE3TRACKING_MIN_LEVEL) {
         const TrackLevelParams& L = p.lvl[SE3TRACKING_MIN_LEVEL];
         const int G = (int)gridDim.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
         const int Gv = G * p.nRanks, vb = (int)blockIdx.x * p.nRanks + p.rank;
@@ -793,15 +848,16 @@ __global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid
                 for (int d = 0; d < p.nRanks; d++) if (d != p.rank) p.peerMask[d][i] = g;
         }
     }
-    if (p.nRanks > 1) gridTailRanks(p);
+    if (!GROUP && p.nRanks > 1) gridTailRanks(p);
 
-    if (p.debug && threadIdx.x == 0 && blockIdx.x < TP_MAXGRID - 1) {
+    // the per-CTA cycle table (LSDGPU_TRACK_DEBUG) is written by single-stream launches only
+    if (!GROUP && p.debug && threadIdx.x == 0 && blockIdx.x < TP_MAXGRID - 1) {
         long long tot = clock64() - tStart;
         for (int i = 0; i < 4; i++) out->cycBlk[blockIdx.x][i] = cyc[i];
         out->cycBlk[blockIdx.x][5] = tot;
         out->cycBlk[blockIdx.x][4] = tot - cyc[0] - cyc[1] - cyc[2] - cyc[3];
     }
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
+    if ((GROUP ? sg.b : (int)blockIdx.x) == 0 && threadIdx.x == 0) {
         // statistics of the LAST EVALUATED pose (SURVEY App. A-1): main block, or the extension block's last candidate
         float fin[EV_NCH];
         for (int c = 0; c < EV_NCH; c++) fin[c] = sh.sums[c];
@@ -828,10 +884,25 @@ __global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid
         cyc[5] = clock64() - tStart;
         cyc[4] = cyc[5] - cyc[0] - cyc[1] - cyc[2] - cyc[3];
         for (int i = 0; i < 6; i++) out->cyc[i] = cyc[i];
-        if (p.debug) for (int i = 0; i < 4; i++) out->cycBlk[TP_MAXGRID - 1][i] = lm.dbg[i];
+        if (!GROUP && p.debug) for (int i = 0; i < 4; i++) out->cycBlk[TP_MAXGRID - 1][i] = lm.dbg[i];
         __threadfence_system();
         out->doneSeq = p.launchSeq;
     }
+}
+
+__global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid_constant__ TrackParams p, TrackState* __restrict__ out)
+{
+    trackStream<false>(p, out, SegGrid{});
+}
+
+// n streams in one cooperative launch of n * Gs CTAs: CTAs [s * Gs, (s + 1) * Gs) track segs[s] on a virtual grid of Gv CTAs
+__global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent_group(const TrackGroupSeg* __restrict__ segs, int Gs, int Gv)
+{
+    const int s = (int)blockIdx.x / Gs;
+    const TrackGroupSeg& g = segs[s];
+    SegGrid sg;
+    sg.b = (int)blockIdx.x - s * Gs; sg.Gs = Gs; sg.Gv = Gv; sg.lastMask = g.lastMask;
+    trackStream<true>(g.p, g.out, sg);
 }
 
 static cudaError_t trackPersistentSetup(lsdgpu_ctx* ctx)
@@ -856,12 +927,10 @@ static void flushTrackProfile(lsdgpu_ctx* ctx)
     ctx->trackProfilePending = false;
 }
 
-// track one frame: launch the kernel on the context's stream, wait for its result block and translate it (SE3Tracker.cpp:453-485)
-static int trackPersistent(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const double init_qt[7],
-                           const lsdgpu_track_settings* st, lsdgpu_track_result* out)
+// the parameters of one frame's tracking on this context (single-GPU part; trackPersistent adds the peers of a sharded stream)
+static void fillTrackParams(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const double init_qt[7], const lsdgpu_track_settings* st,
+                            TrackParams& P)
 {
-    flushTrackProfile(ctx);
-    TrackParams P;
     memset(&P, 0, sizeof(P));
     for (int l = SE3TRACKING_MIN_LEVEL; l < SE3TRACKING_MAX_LEVEL; l++) {
         const LevelCam& c = ctx->cam[l];
@@ -889,6 +958,75 @@ static int trackPersistent(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const 
     P.sync = ctx->trkSync;
     P.barrierBase = ctx->trkBase;
     P.kmax = TP_KMAX;
+    P.nRanks = 1; P.rank = 0;
+}
+
+// Wait for the result block of launch `ctx->trackSeq`, spinning on its sequence word (a few hundred ns of latency) instead of a stream
+// synchronisation; `launchStream` is the stream the kernel was launched on.
+static int waitTrackState(lsdgpu_ctx* ctx, cudaStream_t launchStream)
+{
+    TrackState* hOut = (TrackState*)ctx->hTrackState;
+    bool done = false;
+    for (long long spin = 0; spin < 200000000LL; spin++) {
+        if (hOut->doneSeq == ctx->trackSeq) { done = true; break; }
+        if ((spin & 0xffff) == 0xffff && cudaStreamQuery(launchStream) != cudaErrorNotReady) { done = hOut->doneSeq == ctx->trackSeq; break; }
+    }
+    if (!done) LSD_CHECK(ctx, cudaStreamSynchronize(launchStream));
+    // the other fields of the mapped result block are read with plain loads afterwards: keep them behind the doneSeq read.  Block 0
+    // publishes doneSeq while other CTAs may still be exiting, so only STREAM-ORDERED consumers may assume the kernel has retired.
+    std::atomic_thread_fence(std::memory_order_acquire);
+    return 0;
+}
+
+// SURVEY 8d, fused single-pass kernel: B_fused(l) = 20 B per valid point + 16 B per texel of the frame's gradient
+// level (+5 B per point on L1: mask byte + index) + 160 B of partial sums, per evaluation OF THE REFERENCE
+// (numCalcResidualCalls; speculative candidates the reference would not evaluate are not counted).  The kernel reads the
+// three keyframe planes densely (12 B per pixel); the ALGORITHMIC figure charges only the valid points, as the survey defines it.
+static double trackAlgorithmicBytes(const lsdgpu_ctx* ctx, const TrackState* hOut)
+{
+    double bytes = 0;
+    for (int l = SE3TRACKING_MIN_LEVEL; l < SE3TRACKING_MAX_LEVEL; l++) {
+        const double np_ = (double)hOut->pointsAtLevel[l];   // numData[level]: valid points of the level (CH_REFNUM)
+        bytes += (double)hOut->numCalcResidualCalls[l] * (20.0 * np_ + 16.0 * (double)ctx->cam[l].w * ctx->cam[l].h + (l == 1 ? 5.0 * np_ : 0.0) + EV_NCH * 4.0);
+    }
+    return bytes;
+}
+
+// the result block -> SE3Tracker's public fields (SE3Tracker.cpp:453-485)
+static void translateTrackState(const lsdgpu_ctx* ctx, const TrackState* hOut, lsdgpu_track_result* out)
+{
+    out->pointUsage = hOut->pointUsage; out->lastGoodCount = hOut->goodCount; out->lastBadCount = hOut->badCount;
+    out->lastMeanRes = hOut->meanRes;
+    out->affineEstimation_a = hOut->affine_a; out->affineEstimation_b = hOut->affine_b;
+    for (int l = 0; l < LSD_LEVELS; l++) {
+        out->numCalcResidualCalls[l] = hOut->numCalcResidualCalls[l];
+        out->numCalcWarpUpdateCalls[l] = hOut->numCalcWarpUpdateCalls[l];
+    }
+    if (hOut->diverged) {
+        out->frameToRef_qt[3] = 1;
+        out->diverged = 1; out->trackingWasGood = 0;
+        return;
+    }
+    const int W = ctx->w, H = ctx->h;
+    out->lastResidual = hOut->lastResidual;
+    out->trackingWasGood = hOut->goodCount / ((W >> SE3TRACKING_MIN_LEVEL) * (H >> SE3TRACKING_MIN_LEVEL)) > 0.04f
+                           && hOut->goodCount / (hOut->goodCount + hOut->badCount) > 0.5f;
+    out->initialTrackedResidual = out->lastResidual / out->pointUsage;
+    lsd::SE3<float> T;
+    for (int i = 0; i < 4; i++) T.q[i] = hOut->refToFrame[i];
+    for (int i = 0; i < 3; i++) T.t[i] = hOut->refToFrame[4 + i];
+    lsd::SE3<double> f2r = lsd::se3Cast<double>(lsd::se3Inverse(T));
+    for (int i = 0; i < 4; i++) out->frameToRef_qt[i] = f2r.q[i];
+    for (int i = 0; i < 3; i++) out->frameToRef_qt[4 + i] = f2r.t[i];
+}
+
+// track one frame: launch the kernel on the context's stream, wait for its result block and translate it (SE3Tracker.cpp:453-485)
+static int trackPersistent(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const double init_qt[7],
+                           const lsdgpu_track_settings* st, lsdgpu_track_result* out)
+{
+    flushTrackProfile(ctx);
+    TrackParams P;
+    fillTrackParams(ctx, kf, fr, init_qt, st, P);
     P.nRanks = ctx->nRanks; P.rank = ctx->rank;
     P.tailBase = ctx->trkTailBase;
     for (int d = 0; d < ctx->nRanks; d++) {
@@ -920,31 +1058,17 @@ static int trackPersistent(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const 
     TrackState* hOut = (TrackState*)ctx->hTrackState;
     // The result block lives in mapped pinned memory and its last word is a sequence number: spin on it (a few
     // hundred ns of latency) instead of a stream synchronisation.  Later launches are stream-ordered anyway.
-    if (ctx->optTrackDebug) LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-    else {
-        bool done = false;
-        for (long long spin = 0; spin < 200000000LL; spin++) {
-            if (hOut->doneSeq == ctx->trackSeq) { done = true; break; }
-            if ((spin & 0xffff) == 0xffff && cudaStreamQuery(ctx->stream) != cudaErrorNotReady) { done = hOut->doneSeq == ctx->trackSeq; break; }
-        }
-        if (!done) LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+    if (ctx->optTrackDebug) {
+        LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+        std::atomic_thread_fence(std::memory_order_acquire);
+    } else {
+        const int r = waitTrackState(ctx, ctx->stream);
+        if (r) return r;
     }
-    // the other fields of the mapped result block are read with plain loads below: keep them behind the doneSeq read.  Block 0
-    // publishes doneSeq while other CTAs may still be exiting, so only STREAM-ORDERED consumers may assume the kernel has retired.
-    std::atomic_thread_fence(std::memory_order_acquire);
     ctx->trkBase += (unsigned int)hOut->totalEvals * (unsigned int)ctx->trackGrid;    // the arrival counter is never reset
 
     if (ctx->profileTrackKernel) {           // the event pair is read lazily (flushTrackProfile): no extra sync on the path
-        // SURVEY 8d, fused single-pass kernel: B_fused(l) = 20 B per valid point + 16 B per texel of the frame's gradient
-        // level (+5 B per point on L1: mask byte + index) + 160 B of partial sums, per evaluation OF THE REFERENCE
-        // (numCalcResidualCalls; speculative candidates the reference would not evaluate are not counted).  The kernel reads the
-        // three keyframe planes densely (12 B per pixel); the ALGORITHMIC figure charges only the valid points, as the survey defines it.
-        double bytes = 0;
-        for (int l = SE3TRACKING_MIN_LEVEL; l < SE3TRACKING_MAX_LEVEL; l++) {
-            const double np_ = (double)hOut->pointsAtLevel[l];   // numData[level]: valid points of the level (CH_REFNUM)
-            bytes += (double)hOut->numCalcResidualCalls[l] * (20.0 * np_ + 16.0 * (double)ctx->cam[l].w * ctx->cam[l].h + (l == 1 ? 5.0 * np_ : 0.0) + EV_NCH * 4.0);
-        }
-        ctx->trackKernelBytes += bytes;
+        ctx->trackKernelBytes += trackAlgorithmicBytes(ctx, hOut);
         ctx->trackProfilePending = true;
     }
 
@@ -974,28 +1098,72 @@ static int trackPersistent(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const 
             }
         }
     }
-    out->pointUsage = hOut->pointUsage; out->lastGoodCount = hOut->goodCount; out->lastBadCount = hOut->badCount;
-    out->lastMeanRes = hOut->meanRes;
-    out->affineEstimation_a = hOut->affine_a; out->affineEstimation_b = hOut->affine_b;
-    for (int l = 0; l < LSD_LEVELS; l++) {
-        out->numCalcResidualCalls[l] = hOut->numCalcResidualCalls[l];
-        out->numCalcWarpUpdateCalls[l] = hOut->numCalcWarpUpdateCalls[l];
+    translateTrackState(ctx, hOut, out);
+    return 0;
+}
+
+// Track the frames of n contexts on one device in ONE cooperative launch of k_track_persistent_group on ctxs[0]'s stream.  The
+// caller has enqueued every frame's construction on its own context's stream: the launching stream waits for all of them, and every
+// other stream waits for the launch, so that each context's later work stays ordered after its tracking.
+// On an error, *failed is the index of the context whose message is set.
+static int trackPersistentGroup(int n, lsdgpu_ctx* const* ctxs, FrameSlot* const* kfs, FrameSlot* const* frs, const double* const* initQts,
+                                const lsdgpu_track_settings* const* sts, lsdgpu_track_result* outs, int* failed)
+{
+    lsdgpu_ctx* c0 = ctxs[0];
+    int Gs = c0->trackGrid / n, Gv = c0->trackGrid;
+    TrackGroupSeg* h = (TrackGroupSeg*)c0->hGroupSegs;
+    for (int i = 0; i < n; i++) {
+        lsdgpu_ctx* ctx = ctxs[i];
+        *failed = i;
+        flushTrackProfile(ctx);
+        fillTrackParams(ctx, kfs[i], frs[i], initQts[i], sts[i], h[i].p);
+        h[i].p.launchSeq = ++ctx->trackSeq;
+        h[i].out = (TrackState*)ctx->dTrackStateMapped;
+        h[i].lastMask = ctx->dLastMask;
+        if (i > 0) {
+            LSD_CHECK(ctx, cudaEventRecord(ctx->groupEvent, ctx->stream));
+            LSD_CHECK(c0, cudaStreamWaitEvent(c0->stream, ctx->groupEvent, 0));
+        }
     }
-    if (hOut->diverged) {
-        out->frameToRef_qt[3] = 1;
-        out->diverged = 1; out->trackingWasGood = 0;
-        return 0;
+    *failed = 0;
+    // the descriptors go through the launching context's pinned staging: the previous group launch that read it has completed
+    // (its results were waited for), and the copy is ordered before this launch on the same stream
+    LSD_CHECK(c0, cudaMemcpyAsync(c0->dGroupSegs, h, n * sizeof(TrackGroupSeg), cudaMemcpyHostToDevice, c0->stream));
+    const TrackGroupSeg* dSegs = (const TrackGroupSeg*)c0->dGroupSegs;
+    void* args[] = { (void*)&dSegs, (void*)&Gs, (void*)&Gv };
+    if (c0->profileTrackKernel) cudaEventRecord(c0->kBegin, c0->stream);
+    {
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(n * Gs); cfg.blockDim = dim3(TP_THREADS); cfg.stream = c0->stream;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
+        cfg.attrs = at; cfg.numAttrs = 1;
+        LSD_CHECK(c0, cudaLaunchKernelExC(&cfg, (const void*)k_track_persistent_group, args));
     }
-    const int W = ctx->w, H = ctx->h;
-    out->lastResidual = hOut->lastResidual;
-    out->trackingWasGood = hOut->goodCount / ((W >> SE3TRACKING_MIN_LEVEL) * (H >> SE3TRACKING_MIN_LEVEL)) > 0.04f
-                           && hOut->goodCount / (hOut->goodCount + hOut->badCount) > 0.5f;
-    out->initialTrackedResidual = out->lastResidual / out->pointUsage;
-    lsd::SE3<float> T;
-    for (int i = 0; i < 4; i++) T.q[i] = hOut->refToFrame[i];
-    for (int i = 0; i < 3; i++) T.t[i] = hOut->refToFrame[4 + i];
-    lsd::SE3<double> f2r = lsd::se3Cast<double>(lsd::se3Inverse(T));
-    for (int i = 0; i < 4; i++) out->frameToRef_qt[i] = f2r.q[i];
-    for (int i = 0; i < 3; i++) out->frameToRef_qt[4 + i] = f2r.t[i];
+    c0->launches++;
+    if (c0->profileTrackKernel) cudaEventRecord(c0->kEnd, c0->stream);
+    LSD_CHECK(c0, cudaEventRecord(c0->groupEvent, c0->stream));
+    for (int i = 1; i < n; i++) {
+        *failed = i;
+        LSD_CHECK(ctxs[i], cudaStreamWaitEvent(ctxs[i]->stream, c0->groupEvent, 0));
+    }
+
+    double bytes = 0;
+    for (int i = 0; i < n; i++) {
+        lsdgpu_ctx* ctx = ctxs[i];
+        frs[i]->hasGoodMask = true;
+        memset(&outs[i], 0, sizeof(outs[i]));
+        *failed = i;
+        const int r = waitTrackState(ctx, c0->stream);
+        if (r) return r;
+        const TrackState* hOut = (const TrackState*)ctx->hTrackState;
+        ctx->trkBase += (unsigned int)hOut->totalEvals * (unsigned int)Gs;     // this segment's barrier counts Gs CTAs per pass
+        bytes += trackAlgorithmicBytes(ctx, hOut);
+        translateTrackState(ctx, hOut, &outs[i]);
+    }
+    if (c0->profileTrackKernel) {            // one launch for the whole group, accounted on the launching context
+        c0->trackKernelBytes += bytes;
+        c0->trackProfilePending = true;
+    }
     return 0;
 }
