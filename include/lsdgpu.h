@@ -233,6 +233,41 @@ typedef struct { float idepth; float idepth_var; unsigned char color[4]; } lsdgp
 /* the packing loop of ROSOutput3DWrapper::publishKeyframe (ROSOutput3DWrapper.cpp:91-110) for level `publish_level`:
  * out receives (w >> level) * (h >> level) records, one device-to-host copy in wire layout */
 int lsdgpu_keyframe_pack_pointcloud(lsdgpu_ctx* ctx, int kf_id, int publish_level, lsdgpu_input_point_dense* out);
+/* ---- the resident map as one world-frame point cloud (lsd_slam_viewer) -------------------------------------------------
+ * The viewer's filtered point cloud of many keyframes in one call: KeyFrameDisplay::refreshPC (KeyFrameDisplay.cpp:106-222,
+ * the drawn vertex buffer) followed by KeyFrameDisplay::flushPC (:269-339, the points of pc.ply, KeyFrameGraphDisplay.cpp:60-92)
+ * with the same camToWorld.  Found by symbol lookup (dlsym), like lsdgpu_track_and_map_group; LSDGPU_ABI_VERSION is unchanged.
+ * The filter is the viewer's run-time settings, lsd_slam_viewer/src/settings.cpp:36-40. */
+typedef struct { float scaledDepthVarTH, absDepthVarTH; int minNearSupport, sparsifyFactor; } lsdgpu_cloud_filter;
+/* the viewer's defaults, settings.cpp:36-40: 1, 1, 5, 1 */
+void lsdgpu_default_cloud_filter(lsdgpu_cloud_filter* f);
+enum {
+    LSDGPU_CLOUD_PLY = 0,               /* flushPC, KeyFrameDisplay.cpp:328-333: float x,y,z (world), float intensity -- 16 B */
+    LSDGPU_CLOUD_VERTEX = 1             /* refreshPC, KeyFrameDisplay.cpp:188-195: MyVertex {float point[3] (camera frame);
+                                           uchar color[4]} -- 16 B (KeyFrameDisplay.h:33-37) */
+};
+/* the return value of lsdgpu_map_export_pointcloud when out cannot hold the points */
+#define LSDGPU_CLOUD_ERR_CAPACITY (-4)
+/* Device buffers of lsdgpu_map_export_pointcloud for up to max_keyframes_per_launch keyframes per launch (two output buffers of
+ * max_keyframes_per_launch * (w-2) * (h-2) points each, for the context's level-0 size), as lsdgpu_stage_reserve does for the prefetch
+ * ring: a separate allocation, the arena is unchanged.  Calling it again replaces the reservation. */
+int lsdgpu_cloud_reserve(lsdgpu_ctx* ctx, int max_keyframes_per_launch);
+/* Point cloud of the n keyframes kf_ids at pyramid level `level` (the publish level of ROSOutput3DWrapper.cpp:85-110).
+ * camToWorld: 7 floats per keyframe = keyframeMsg.camToWorld (keyframeMsg.msg:8), the data() of Sophus::Sim3f: the quaternion
+ * scaled by the scale (x,y,z,w), then the translation.  Points come in keyframe order, each keyframe in the viewer's loop order
+ * (y over [1, h-1) outer, x over [1, w-1) inner) -- the concatenation of flushPC's points (PLY) or of refreshPC's vertex buffer
+ * (VERTEX) of each keyframe in turn.  counts (2 per keyframe, may be NULL) = refreshPC's totalPoints and displayedPoints (:200-201).
+ * out = HOST buffer of capacity_points records, or NULL to only count.  *n_points_out = the number of points.  If
+ * capacity_points is too small the call returns LSDGPU_CLOUD_ERR_CAPACITY, sets *n_points_out and counts and writes nothing to out.
+ * Rejected with an error naming the keyframe: an unknown id, a frame without depth; also a bad level or layout, no reservation and
+ * sparsifyFactor != 1 (the viewer draws rand(), KeyFrameDisplay.cpp:157, :279).  n larger than the reservation runs in batches;
+ * the device-to-host copy of one batch overlaps the kernel of the next.  Allocates nothing and reads no tracking or mapping state. */
+int lsdgpu_map_export_pointcloud(lsdgpu_ctx* ctx, int n, const int* kf_ids, const float* camToWorld, int level,
+                                 const lsdgpu_cloud_filter* f, int layout, void* out, int64_t capacity_points,
+                                 int64_t* n_points_out, int32_t* counts);
+/* device time (CUDA events, ms) from the start of the first kernel of the last lsdgpu_map_export_pointcloud call to the end of its
+ * last kernel (the copies of a batched call run between them); for benchmarks, KeyFrameDisplay.cpp:106-222 */
+int lsdgpu_cloud_last_kernel_ms(lsdgpu_ctx* ctx, float* ms);
 /* Frame::takeReActivationData(currentDepthMap), DataStructures/Frame.cpp:107-145: snapshot of the ACTIVE depth map into the
  * keyframe's idepth_reAct / idepthVar_reAct / validity_reAct -- kept on the device.  lsdgpu_depth_finalize_keyframe calls it
  * (DepthMap.cpp:1387); exposed for re-activation bookkeeping outside finalize. */

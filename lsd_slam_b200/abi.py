@@ -101,6 +101,38 @@ class Sim3EvalResult(C.Structure):
                 ("pointUsage", C.c_float), ("affine_a_lastIt", C.c_float), ("affine_b_lastIt", C.c_float)]
 
 
+class CloudFilter(C.Structure):
+    """lsdgpu_cloud_filter: the viewer's filter settings, lsd_slam_viewer/src/settings.cpp:36-40"""
+    _fields_ = [("scaledDepthVarTH", C.c_float), ("absDepthVarTH", C.c_float), ("minNearSupport", C.c_int), ("sparsifyFactor", C.c_int)]
+
+
+CLOUD_PLY, CLOUD_VERTEX = 0, 1
+CLOUD_ERR_CAPACITY = -4
+# LSDGPU_CLOUD_PLY: flushPC's record (KeyFrameDisplay.cpp:328-333); LSDGPU_CLOUD_VERTEX: MyVertex (KeyFrameDisplay.h:33-37)
+CLOUD_PLY_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("intensity", "<f4")])
+CLOUD_VERTEX_DTYPE = np.dtype([("point", "<f4", (3,)), ("color", "u1", (4,))])
+
+
+def default_cloud_filter(**kw) -> CloudFilter:
+    f = CloudFilter()
+    load().lsdgpu_default_cloud_filter(C.byref(f))
+    for k, v in kw.items():
+        setattr(f, k, v)
+    return f
+
+
+def write_ply(path, points: np.ndarray) -> None:
+    """Writes points (CLOUD_PLY_DTYPE, e.g. from Context.export_pointcloud) as the viewer's pc.ply: the header of
+    KeyFrameGraphDisplay.cpp:74-82, then the 16-byte records.  The viewer's copy loop `while(!f3.eof()) f2.put(f3.get())`
+    (:84-85) appends one stray 0xFF byte after the last record; this writer does not, so its file is the viewer's minus that byte."""
+    pts = np.ascontiguousarray(points, CLOUD_PLY_DTYPE)
+    with open(path, "wb") as f:
+        f.write(b"ply\nformat binary_little_endian 1.0\n")
+        f.write(b"element vertex %d\n" % len(pts))
+        f.write(b"property float x\nproperty float y\nproperty float z\nproperty float intensity\nend_header\n")
+        f.write(pts.tobytes())
+
+
 SYMBOLS = [
     ("lsdgpu_create", C.c_int, [C.c_int, C.c_int, C.c_int, _fp, C.c_int, C.POINTER(_vp)]),
     ("lsdgpu_destroy", None, [_vp]),
@@ -141,6 +173,11 @@ SYMBOLS = [
     ("lsdgpu_undistort_u8", C.c_int, [_vp, C.POINTER(C.c_uint8), C.POINTER(C.c_uint8)]),
     ("lsdgpu_frame_upload_distorted_u8", C.c_int, [_vp, C.c_int, C.POINTER(C.c_uint8)]),
     ("lsdgpu_keyframe_pack_pointcloud", C.c_int, [_vp, C.c_int, C.c_int, _vp]),
+    ("lsdgpu_default_cloud_filter", None, [C.c_void_p]),
+    ("lsdgpu_cloud_reserve", C.c_int, [_vp, C.c_int]),
+    ("lsdgpu_map_export_pointcloud", C.c_int, [_vp, C.c_int, _ip, _fp, C.c_int, C.c_void_p, C.c_int, _vp, C.c_int64,
+                                               C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
+    ("lsdgpu_cloud_last_kernel_ms", C.c_int, [_vp, _fp]),
     ("lsdgpu_frame_take_reactivation_data", C.c_int, [_vp, C.c_int]),
     ("lsdgpu_frame_download_reactivation_data", C.c_int, [_vp, C.c_int, _fp, _fp, C.POINTER(C.c_uint8)]),
     ("lsdgpu_depth_set_from_existing_kf", C.c_int, [_vp, C.c_int]),
@@ -414,6 +451,57 @@ class Context:
         out = np.zeros(n, POINT_DENSE)
         self._ck(self.L.lsdgpu_keyframe_pack_pointcloud(self.ptr, kf_id, level, out.ctypes.data_as(_vp)))
         return out
+
+    def cloud_reserve(self, max_keyframes_per_launch: int):
+        """device buffers of export_pointcloud (lsdgpu_cloud_reserve): larger exports run in batches of this many keyframes"""
+        self._ck(self.L.lsdgpu_cloud_reserve(self.ptr, int(max_keyframes_per_launch)))
+
+    def export_pointcloud(self, kf_ids, camToWorld, level: int = 0, filter=None, layout: int = CLOUD_PLY, capacity=None, out=None):
+        """the viewer's point cloud of keyframes kf_ids (KeyFrameDisplay::refreshPC + flushPC, KeyFrameDisplay.cpp:106-222,
+        :269-339), filtered and transformed on the device: camToWorld = (n, 7) float32 Sim3f data (keyframeMsg.camToWorld).
+        filter: CloudFilter, dict of its fields, or None (the viewer's defaults).  Returns (points, counts): points in keyframe
+        order (CLOUD_PLY_DTYPE world points + intensity, or CLOUD_VERTEX_DTYPE camera points + colour), counts = (n, 2) int32
+        totalPoints, displayedPoints.  Needs cloud_reserve first.  capacity=None sizes the output for every interior pixel;
+        out = a caller's array of the layout's dtype to fill instead (its length is the capacity; the points are a view of it)."""
+        ids = np.ascontiguousarray(kf_ids, np.int32).reshape(-1)
+        n = len(ids)
+        c2w = np.ascontiguousarray(camToWorld, np.float32).reshape(n, 7)
+        if filter is None or isinstance(filter, dict):
+            filter = default_cloud_filter(**(filter or {}))
+        wl, hl = self.w >> level, self.h >> level
+        if out is None:
+            if capacity is None:
+                capacity = n * max(wl - 2, 0) * max(hl - 2, 0)
+            out = np.empty(max(int(capacity), 1), CLOUD_VERTEX_DTYPE if layout == CLOUD_VERTEX else CLOUD_PLY_DTYPE)
+        else:
+            assert out.flags.c_contiguous and out.dtype.itemsize == 16
+            capacity = len(out)
+        counts = np.zeros((n, 2), np.int32)
+        npts = C.c_int64(0)
+        rc = self.L.lsdgpu_map_export_pointcloud(self.ptr, n, ids.ctypes.data_as(_ip), c2w.ctypes.data_as(_fp), level, C.byref(filter),
+                                                 layout, out.ctypes.data_as(_vp), int(capacity), C.byref(npts),
+                                                 counts.ctypes.data_as(C.POINTER(C.c_int32)))
+        self._ck(rc)
+        return out[:npts.value], counts
+
+    def count_pointcloud(self, kf_ids, camToWorld, level: int = 0, filter=None):
+        """(number of points, counts) of export_pointcloud without the points (out = NULL)"""
+        ids = np.ascontiguousarray(kf_ids, np.int32).reshape(-1)
+        c2w = np.ascontiguousarray(camToWorld, np.float32).reshape(len(ids), 7)
+        if filter is None or isinstance(filter, dict):
+            filter = default_cloud_filter(**(filter or {}))
+        counts = np.zeros((len(ids), 2), np.int32)
+        npts = C.c_int64(0)
+        self._ck(self.L.lsdgpu_map_export_pointcloud(self.ptr, len(ids), ids.ctypes.data_as(_ip), c2w.ctypes.data_as(_fp), level,
+                                                     C.byref(filter), CLOUD_PLY, None, 0, C.byref(npts),
+                                                     counts.ctypes.data_as(C.POINTER(C.c_int32))))
+        return npts.value, counts
+
+    def cloud_kernel_ms(self) -> float:
+        """device time of the last export's kernels (lsdgpu_cloud_last_kernel_ms)"""
+        ms = C.c_float(0)
+        self._ck(self.L.lsdgpu_cloud_last_kernel_ms(self.ptr, C.byref(ms)))
+        return ms.value
 
     def take_reactivation_data(self, kf_id: int):
         self._ck(self.L.lsdgpu_frame_take_reactivation_data(self.ptr, kf_id))

@@ -170,6 +170,21 @@ struct lsdgpu_ctx {
     int stageIdx = 0;
     float* hStageF = nullptr;            // pinned float staging (depth / idepth uploads)
     float* dStageF = nullptr;
+    // lsdgpu_map_export_pointcloud (cloud.cuh): separate allocations made by lsdgpu_cloud_reserve, two of each (batch b uses set b & 1)
+    int cloudMaxKf = 0;
+    char* cloudMem = nullptr;            // device: descriptors, tile states + ticket + counts, output points, intensity table
+    char* hCloudMem = nullptr;           // pinned: descriptors and counts of both sets
+    void* dCloudKfs[2] = { nullptr, nullptr };
+    void* hCloudKfs[2] = { nullptr, nullptr };
+    unsigned long long* dCloudState[2] = { nullptr, nullptr };   // tile states, then the ticket, then 2 counts per keyframe
+    size_t cloudStateBytes = 0;
+    int* hCloudCounts[2] = { nullptr, nullptr };
+    float4* dCloudOut[2] = { nullptr, nullptr };
+    float* dCloudIntensity = nullptr;
+    cudaStream_t cloudCopyStream = nullptr;
+    cudaEvent_t cloudKernDone[2], cloudCopyDone[2];
+    cudaEvent_t cloudT0 = nullptr, cloudT1 = nullptr;
+    bool cloudTimed = false;
 
     // timers
     cudaEvent_t tBegin[8], tEnd[8];

@@ -11,6 +11,10 @@ is forced every ``kf_every`` frames (SURVEY 8d).  This driver only issues C-ABI 
 times and what the full-loop parity tests run.  ``fused_call=True`` issues the whole frame as ONE ABI call
 (``lsdgpu_track_and_map``, same call sequence inside the library); ``False`` issues the individual calls.
 
+The stream keeps the ids of its keyframes and their camToWorld, chained from the thisToParent Sim3 that createKeyFrame returns
+(odometry: no pose graph), so that ``ctx.export_pointcloud(stream.keyframe_ids, stream.keyframe_cam_to_world_f7())`` is the
+viewer's map of the run.  With ``keep_keyframes=True`` finished keyframes stay resident (the context needs a frame slot for each).
+
 ``GpuStreamGroup`` steps K such streams (one context each, same GPU) with ONE call per frame
 (``lsdgpu_track_and_map_group``): the trackings of the K frames share one launch, each stream on its own slice of the SMs.
 """
@@ -23,11 +27,46 @@ import numpy as np
 from . import abi
 
 IDENT = np.array([0, 0, 0, 1, 0, 0, 0], np.float64)
+IDENT_QTS = np.array([0, 0, 0, 1, 0, 0, 0, 1], np.float64)
+
+
+def _quat_mul(a, b):
+    """Hamilton product of (x, y, z, w) quaternions"""
+    ax, ay, az, aw = a
+    bx, by, bz, bw = b
+    return np.array([aw * bx + ax * bw + ay * bz - az * by, aw * by + ay * bw + az * bx - ax * bz,
+                     aw * bz + az * bw + ax * by - ay * bx, aw * bw - ax * bx - ay * by - az * bz])
+
+
+def _quat_rot(q, v):
+    u = np.cross(q[:3], v)
+    u = u + u
+    return v + q[3] * u + np.cross(q[:3], u)
+
+
+def sim3_mul_qts(a, b) -> np.ndarray:
+    """a * b for Sim3 as qts[8] (unit quaternion x,y,z,w, translation, scale), in double"""
+    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
+    q = _quat_mul(a[:4], b[:4])
+    q /= np.sqrt(q @ q)
+    t = a[7] * _quat_rot(a[:4], b[4:7]) + a[4:7]
+    return np.concatenate([q, t, [a[7] * b[7]]])
+
+
+def qts_to_sim3f(qts) -> np.ndarray:
+    """the ABI's Sim3 qts[8] as the 7 floats of keyframeMsg.camToWorld: Sophus::Sim3f::data() of getScaledCamToWorld().cast<float>()
+    (the quaternion scaled by the scale, then the translation; ROSOutput3DWrapper.cpp:85-88)"""
+    qts = np.asarray(qts, np.float64)
+    return np.concatenate([qts[:4] * qts[7], qts[4:7]]).astype(np.float32)
 
 
 class GpuStream:
-    def __init__(self, ctx: abi.Context, mode: int = 1, kf_every: int = 20, fused_call: bool = True, kf_phase: int = 0):
+    def __init__(self, ctx: abi.Context, mode: int = 1, kf_every: int = 20, fused_call: bool = True, kf_phase: int = 0,
+                 keep_keyframes: bool = False):
         self.ctx = ctx
+        self.keep_keyframes = keep_keyframes
+        self.keyframe_ids: list[int] = []          # every keyframe of the run, oldest first
+        self.keyframe_cam_to_world: list[np.ndarray] = []   # their camToWorld as qts[8], the first keyframe at the origin
         self.kf_phase = kf_phase          # shifts the forced keyframe changes: frame n changes keyframe when (n + kf_phase) % kf_every == 0
         self.tracker = abi.SE3Tracker(ctx, mode=mode)
         self.map = abi.DepthMap(ctx)
@@ -48,6 +87,11 @@ class GpuStream:
         self.map.initializeFromGTDepth(fid)
         self.kf_id = fid
         self.last_pose = IDENT.copy()
+        self.keyframe_ids, self.keyframe_cam_to_world = [fid], [IDENT_QTS.copy()]
+
+    def keyframe_cam_to_world_f7(self) -> np.ndarray:
+        """(n, 7) float32 camToWorld of keyframe_ids, as keyframeMsg carries them"""
+        return np.stack([qts_to_sim3f(q) for q in self.keyframe_cam_to_world])
 
     def _track_and_map_fused(self, fid, image_u8, stage_index, kf_change):
         ctx, trk = self.ctx, self.tracker
@@ -94,20 +138,23 @@ class GpuStream:
         if not self.fused_call:
             if kf_change:
                 self.map.finalizeKeyFrame()
-                self.map.createKeyFrame(fid)
+                self._qts[:] = self.map.createKeyFrame(fid)
             else:
                 self.map.updateKeyframe([fid])
                 ctx.clear_good_mask(fid)             # SlamSystem.cpp:573
-        self._advance(fid, pose, kf_change)
+        self._advance(fid, pose, kf_change, self._qts)
         return pose
 
-    def _advance(self, fid: int, pose: np.ndarray, kf_change: bool):
+    def _advance(self, fid: int, pose: np.ndarray, kf_change: bool, new_kf_qts=None):
         """bookkeeping after a mapped frame: the keyframe, the next initial pose and the frames that can be released"""
         ctx = self.ctx
         if kf_change:
             old_kf, self.kf_id = self.kf_id, fid
             self.last_pose = IDENT.copy()
-            for i in self.prev_ids + [old_kf]:
+            if self.keyframe_ids:               # the new keyframe's thisToParent (createKeyFrame) chained onto its parent
+                self.keyframe_ids.append(fid)
+                self.keyframe_cam_to_world.append(sim3_mul_qts(self.keyframe_cam_to_world[-1], new_kf_qts))
+            for i in self.prev_ids + ([] if self.keep_keyframes else [old_kf]):
                 ctx.release(i)
             self.prev_ids = []
         else:
@@ -162,7 +209,7 @@ class GpuStreamGroup:
             if gs.tracker.diverged:
                 diverged.append(fids[i])
                 continue
-            gs._advance(fids[i], pose, kf_changes[i])
+            gs._advance(fids[i], pose, kf_changes[i], self._qts[i])
             poses.append(pose)
         if diverged:
             raise RuntimeError(f"tracking diverged on frame(s) {diverged}")
