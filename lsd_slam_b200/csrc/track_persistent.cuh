@@ -40,6 +40,7 @@
 #define TP_KMAX 3                    // poses per pass: the try + up to two speculative successors
 #define TP_ROW 64                    // floats per exchange row (256 B, one row per CTA; EV_NCHX = 56 used)
 #define TP_MAX_GROUP 8               // streams one group launch can track (lsdgpu_track_and_map_group)
+#define TP_CARRY_BITS 32             // level-1 chunk slots one thread can carry the last candidate's flags for in registers
 
 struct TrackLevelParams {
     const float* kfIdepth;
@@ -77,6 +78,9 @@ struct TrackParams {
     unsigned int* peerSync[TP_MAX_RANKS];     // each rank's `sync` block as mapped into THIS process (own entry = sync)
     uint8_t* peerMask[TP_MAX_RANKS];          // the tracked frame's level-1 mask on each rank
     unsigned int tailBase;                    // arrivals already counted on the tail barrier
+    // level-1 good flags of the last candidate of a pass: nullptr = in ThreadCarry::lastBits (a thread's level-1 slots fit in its
+    // TP_CARRY_BITS bits), otherwise in this level-1 plane of the context (always for a group launch; see fillTrackParams)
+    uint8_t* lastMask;
 };
 
 // what the kernel hands back (block 0 writes it)
@@ -104,10 +108,9 @@ struct TrackState {
 // the same Gv rows in the same order, so every sum, every LM decision and every result is bit-identical to k_track_persistent's.
 // A native grid of Gs CTAs would deal the chunks out differently and change the fp32 summation order.
 struct TrackGroupSeg {
-    TrackParams p;                   // the stream's parameters (nRanks == 1, debug == 0)
+    TrackParams p;                   // the stream's parameters (nRanks == 1, debug == 0, lastMask set: ThreadCarry::lastBits would
+                                     // need up to ceil(Gv / Gs) times as many bits)
     TrackState* out;                 // its context's mapped result block
-    uint8_t* lastMask;               // level-1 scratch of its context: the last candidate's good flags (ThreadCarry::lastBits
-                                     // would need up to ceil(Gv / Gs) times as many bits)
 };
 
 // where a CTA sits in a group launch (unused by the single-stream instantiation)
@@ -115,7 +118,6 @@ struct SegGrid {
     int b;                           // physical CTA within the segment
     int Gs;                          // physical CTAs of the segment (the barrier counts these)
     int Gv;                          // virtual grid (rows of the combine) = the single-stream launch's grid
-    uint8_t* lastMask;
 };
 
 // Grid-wide barrier.  Arrivals are counted on one word (monotonic: epoch e completes at base + e * gridDim arrivals, the
@@ -233,9 +235,12 @@ struct ThreadCarry {
     bool pcIsPoint;
     float pcx, pcy, pcz, pcVar, pcColor;
     // level-1 good flags of the LAST candidate of the most recent pass, one bit per chunk slot of this thread (the mask itself
-    // always holds candidate 0's flags); committed at the end if that candidate was the last pose the reference evaluates
+    // always holds candidate 0's flags); committed at the end if that candidate was the last pose the reference evaluates.
+    // Only used while the thread's slots k = warp, warp + TP_WARPS, ... number at most TP_CARRY_BITS (TrackParams::lastMask).
     unsigned int lastBits, pointBits;
 };
+static_assert(sizeof(ThreadCarry::lastBits) * 8 == TP_CARRY_BITS && sizeof(ThreadCarry::pointBits) * 8 == TP_CARRY_BITS,
+              "fillTrackParams sends a level through TrackParams::lastMask when a thread has more than TP_CARRY_BITS slots");
 
 // One pass: nPose candidate poses over this CTA's chunks of level `lvl`, CTA reduction, one row per CTA through L2 behind ONE
 // grid barrier, then every CTA sums the rows in block order.  On return sh.sums holds the totals, bit-identical in every CTA.
@@ -317,7 +322,8 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, const SegGrid
     const int Gv = GROUP ? sg.Gv : G * p.nRanks;
     int vb = GROUP ? sg.b : (int)blockIdx.x * p.nRanks + p.rank;
     const int nSlots = (L.nChunks + Gv - 1) / Gv;
-    if (!GROUP && mask) { tc.lastBits = 0u; tc.pointBits = 0u; }
+    const bool lastInPlane = GROUP || p.lastMask != nullptr;
+    if (!lastInPlane && mask) { tc.lastBits = 0u; tc.pointBits = 0u; }
     const int nch = K > 1 ? EV_NCHX : EV_NCH;
     const unsigned int parity = epoch & 1u;
     float* part = p.partials + (size_t)parity * TP_ROW * (GROUP ? (unsigned int)Gv : gridDim.x);
@@ -370,13 +376,13 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, const SegGrid
                     if (K > 2) evalPointLight<false>(px, py, pz, color, var, sh.pose[1], p.C, L.fx, L.fy, L.cx, L.cy, w, h, tap, ext);
                     const int goodL = evalPointLight<true>(px, py, pz, color, var, sh.pose[K - 1], p.C, L.fx, L.fy, L.cx, L.cy, w, h, tap, ext);
                     if (mask) {
-                        if (GROUP) sg.lastMask[i] = (uint8_t)goodL;
+                        if (lastInPlane) p.lastMask[i] = (uint8_t)goodL;
                         else tc.lastBits |= (unsigned int)goodL << slot;
                     }
                 }
                 if (mask) {
                     mask[i] = (uint8_t)good;
-                    if (!GROUP) tc.pointBits |= 1u << slot;
+                    if (!lastInPlane) tc.pointBits |= 1u << slot;
                     if (!GROUP && p.nRanks > 1)                            // the other ranks own other chunks: give them this one's flag
                         for (int d = 0; d < p.nRanks; d++) if (d != p.rank) p.peerMask[d][i] = (uint8_t)good;
                 }
@@ -815,23 +821,28 @@ __device__ __forceinline__ void trackStream(const TrackParams& p, TrackState* __
 
     // The mask holds the flags of candidate 0 of the last level-1 pass; if the last pose the reference evaluates was the chain's
     // last candidate instead, its flags (kept per thread) replace them now.  Same threads, same pixels: no synchronisation.
-    if (GROUP && lm.commitLast && p.minLevel == SE3TRACKING_MIN_LEVEL) {
-        // group launch: the flags are in sg.lastMask, written by this thread in the last pass for every point it evaluated; the
-        // points are found again from the keyframe planes (the test of gridEvaluate)
+    if ((GROUP || p.lastMask) && lm.commitLast && p.minLevel == SE3TRACKING_MIN_LEVEL) {
+        // the flags are in p.lastMask, written by this thread in the last pass for every point it evaluated; the points are found
+        // again from the keyframe planes (the test of gridEvaluate).  A group CTA runs the virtual CTAs sg.b, sg.b + Gs, ...
         const TrackLevelParams& L = p.lvl[SE3TRACKING_MIN_LEVEL];
         const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-        const int nSlots = (L.nChunks + sg.Gv - 1) / sg.Gv;
-        for (int v = sg.b; v < sg.Gv; v += sg.Gs)
+        const int Gv = GROUP ? sg.Gv : (int)gridDim.x * p.nRanks;
+        const int nSlots = (L.nChunks + Gv - 1) / Gv;
+        for (int v = GROUP ? sg.b : (int)blockIdx.x * p.nRanks + p.rank; v < Gv; v += GROUP ? sg.Gs : Gv)
             for (int k = warp; k < nSlots; k += TP_WARPS) {
-                const int j = (tpChunkOf(v, k, sg.Gv) << 5) + lane;
+                const int j = (tpChunkOf(v, k, Gv) << 5) + lane;
                 if (j >= L.nInt) continue;
                 const int yy = j / L.iw;
                 const int i = (j - yy * L.iw + 1) + (yy + 1) * L.w;
                 const float idepth = L.kfIdepth[i], var = L.kfVar[i];
-                if (!(var <= 0 || idepth == 0)) p.goodMask[i] = sg.lastMask[i];
+                if (var <= 0 || idepth == 0) continue;
+                const uint8_t g = p.lastMask[i];
+                p.goodMask[i] = g;
+                if (!GROUP && p.nRanks > 1)
+                    for (int d = 0; d < p.nRanks; d++) if (d != p.rank) p.peerMask[d][i] = g;
             }
     }
-    if (!GROUP && lm.commitLast && p.minLevel == SE3TRACKING_MIN_LEVEL) {
+    if (!GROUP && !p.lastMask && lm.commitLast && p.minLevel == SE3TRACKING_MIN_LEVEL) {
         const TrackLevelParams& L = p.lvl[SE3TRACKING_MIN_LEVEL];
         const int G = (int)gridDim.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
         const int Gv = G * p.nRanks, vb = (int)blockIdx.x * p.nRanks + p.rank;
@@ -901,7 +912,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent_group(const 
     const int s = (int)blockIdx.x / Gs;
     const TrackGroupSeg& g = segs[s];
     SegGrid sg;
-    sg.b = (int)blockIdx.x - s * Gs; sg.Gs = Gs; sg.Gv = Gv; sg.lastMask = g.lastMask;
+    sg.b = (int)blockIdx.x - s * Gs; sg.Gs = Gs; sg.Gv = Gv;
     trackStream<true>(g.p, g.out, sg);
 }
 
@@ -927,6 +938,14 @@ static void flushTrackProfile(lsdgpu_ctx* ctx)
     ctx->trackProfilePending = false;
 }
 
+// level-1 chunk slots of the busiest thread of a single-stream launch: slots k = warp, warp + TP_WARPS, ... of its CTA's share
+static int level1SlotsPerThread(const lsdgpu_ctx* ctx, int nChunks)
+{
+    const int gv = ctx->trackGrid * ctx->nRanks;
+    const int slots = (nChunks + gv - 1) / gv;
+    return (slots + TP_WARPS - 1) / TP_WARPS;
+}
+
 // the parameters of one frame's tracking on this context (single-GPU part; trackPersistent adds the peers of a sharded stream)
 static void fillTrackParams(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const double init_qt[7], const lsdgpu_track_settings* st,
                             TrackParams& P)
@@ -938,8 +957,11 @@ static void fillTrackParams(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const
         L.kfIdepth = kf->idepth[l]; L.kfVar = kf->idepthVar[l]; L.kfColor = kf->image[l]; L.frameGrad = fr->grad[l];
         L.w = c.w; L.h = c.h; L.fx = c.fx; L.fy = c.fy; L.cx = c.cx; L.cy = c.cy;
         L.fxi = c.fxi; L.fyi = c.fyi; L.cxi = c.cxi; L.cyi = c.cyi;
-        L.iw = c.w - 2; L.nInt = (c.w - 2) * (c.h - 2); L.nChunks = (L.nInt + 31) / 32;
+        // no interior on a level 1 or 2 pixels wide or high (1x1 at 16x16): (w-2)*(h-2) would count (-1)*(-1) = 1 point
+        L.iw = c.w - 2; L.nInt = std::max(c.w - 2, 0) * std::max(c.h - 2, 0); L.nChunks = (L.nInt + 31) / 32;
     }
+    // one bit per level-1 slot of a thread in ThreadCarry, or (more slots than bits, e.g. 4096x2160 on 132 SMs) the context's plane
+    P.lastMask = level1SlotsPerThread(ctx, P.lvl[SE3TRACKING_MIN_LEVEL].nChunks) > TP_CARRY_BITS ? ctx->dLastMask : nullptr;
     P.minLevel = SE3TRACKING_MIN_LEVEL;
     P.goodMask = fr->goodMask;
     P.maskFresh = fr->hasGoodMask ? 0 : 1;
@@ -1040,6 +1062,9 @@ static int trackPersistent(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const 
     const int grid = ctx->trackGrid;                                               // one CTA per SM
     void* args[] = { (void*)&P, (void*)&dOut };
     P.debug = ctx->optTrackDebug ? 1 : 0;
+    if (ctx->optTrackDebug)
+        fprintf(stderr, "[track] level-1 slots per thread %d: last-candidate flags in %s\n",
+                level1SlotsPerThread(ctx, P.lvl[SE3TRACKING_MIN_LEVEL].nChunks), P.lastMask ? "the level-1 plane" : "registers");
     P.launchSeq = ++ctx->trackSeq;
     if (ctx->profileTrackKernel) cudaEventRecord(ctx->kBegin, ctx->stream);
     {
@@ -1119,7 +1144,7 @@ static int trackPersistentGroup(int n, lsdgpu_ctx* const* ctxs, FrameSlot* const
         fillTrackParams(ctx, kfs[i], frs[i], initQts[i], sts[i], h[i].p);
         h[i].p.launchSeq = ++ctx->trackSeq;
         h[i].out = (TrackState*)ctx->dTrackStateMapped;
-        h[i].lastMask = ctx->dLastMask;
+        h[i].p.lastMask = ctx->dLastMask;
         if (i > 0) {
             LSD_CHECK(ctx, cudaEventRecord(ctx->groupEvent, ctx->stream));
             LSD_CHECK(c0, cudaStreamWaitEvent(c0->stream, ctx->groupEvent, 0));

@@ -12,6 +12,7 @@ and compares
     distance between the oracle and its diagnostic twin that accumulates the same fp32 terms exactly -- up to 1.7e-4 on the
     bench streams: the sequential fp32 sums of SE3Tracker.cpp carry ~1e-5 relative error into a 6x6 system whose weak
     directions amplify it), and
+  * the device's refPixelWasGood mask against the oracle's own (`mask_mismatch`: pixels that differ), and
   * with the device's pose, residual and good-mask handed to the oracle, the depth map after the step BIT FOR BIT
     (keyframe changes included: the sequential fp32 sum behind the rescale factor, DepthMap.cpp:1286-1294, is reproduced
     exactly by csrc/seqsum.cuh).
@@ -131,6 +132,8 @@ def finish_replay(seq, snap: Snapshot, out, gs, mask_before_clear=None, rescale_
     of.set_thisToParent(qts, okf)
     L.lsdo_frame_set_initialTrackedResidual(of.ptr, float(itr_g))
     if mask_g is not None:
+        # the device's refPixelWasGood against the oracle's own tracking of the step (pixels that differ), before it is replaced
+        out["mask_mismatch"] = int((of.refPixelWasGood(create=True) != mask_g).sum())
         of.refPixelWasGood(create=True)[:] = mask_g
     tracked_after, mapped_after = gs.ctx.get_counters(snap.kf_id) if not snap.kf_change else (None, None)
     if snap.kf_change:
