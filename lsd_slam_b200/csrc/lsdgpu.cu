@@ -674,6 +674,26 @@ static int trackHostLM(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const doub
     return 0;
 }
 
+// `s`, or for a null `s` the main tracker's settings: the defaults without iterations on level 4 (SlamSystem.cpp:80-81)
+static const lsdgpu_track_settings* trackSettingsOrDefault(const lsdgpu_track_settings* s, lsdgpu_track_settings& ds)
+{
+    if (s) return s;
+    lsdgpu_default_track_settings(&ds);
+    ds.maxItsPerLvl[4] = 0;
+    return &ds;
+}
+
+// the Frame side effects of a tracking that did not diverge (SE3Tracker.cpp:479-484)
+static void applyTrackedFrame(FrameSlot* kf, FrameSlot* fr, const lsdgpu_track_result* out)
+{
+    if (out->diverged) return;
+    if (out->trackingWasGood) kf->numFramesTrackedOnThis++;                   // :479-480
+    fr->initialTrackedResidual = out->initialTrackedResidual;                 // :482
+    for (int i = 0; i < 7; i++) fr->thisToParent[i] = out->frameToRef_qt[i];  // :483 sim3FromSE3(.., 1)
+    fr->thisToParent[7] = 1.0;
+    fr->parentId = kf->id;                                                    // :484
+}
+
 extern "C" int lsdgpu_se3_track(lsdgpu_ctx* ctx, int kf_id, int frame_id, const double init_qt[7],
                                 const lsdgpu_track_settings* s, int mode, lsdgpu_track_result* out)
 { LSD_LOCK(ctx);
@@ -684,17 +704,11 @@ extern "C" int lsdgpu_se3_track(lsdgpu_ctx* ctx, int kf_id, int frame_id, const 
     int r = ensureIdepthPyramid(ctx, kf);      // reference->makePointCloud(lvl), SE3Tracker.cpp:321
     if (r) return r;
     lsdgpu_track_settings ds;
-    if (!s) { lsdgpu_default_track_settings(&ds); ds.maxItsPerLvl[4] = 0; s = &ds; }
+    s = trackSettingsOrDefault(s, ds);
     if (mode == 1) r = trackPersistent(ctx, kf, fr, init_qt, s, out);
     else r = trackHostLM(ctx, kf, fr, init_qt, s, out);
     if (r) return r;
-    if (!out->diverged) {
-        if (out->trackingWasGood) kf->numFramesTrackedOnThis++;                   // :479-480
-        fr->initialTrackedResidual = out->initialTrackedResidual;                 // :482
-        for (int i = 0; i < 7; i++) fr->thisToParent[i] = out->frameToRef_qt[i];  // :483 sim3FromSE3(.., 1)
-        fr->thisToParent[7] = 1.0;
-        fr->parentId = kf->id;                                                    // :484
-    }
+    applyTrackedFrame(kf, fr, out);
     return 0;
 }
 
@@ -779,16 +793,9 @@ extern "C" int lsdgpu_se3_track_sharded(lsdgpu_ctx* ctx, int kf_id, int frame_id
     int r = ensureIdepthPyramid(ctx, kf);
     if (r) return r;
     lsdgpu_track_settings ds;
-    if (!s) { lsdgpu_default_track_settings(&ds); ds.maxItsPerLvl[4] = 0; s = &ds; }
-    r = trackHostLM(ctx, kf, fr, init_qt, s, out, shard, n_shards, allreduce, user);
+    r = trackHostLM(ctx, kf, fr, init_qt, trackSettingsOrDefault(s, ds), out, shard, n_shards, allreduce, user);
     if (r) return r;
-    if (!out->diverged) {
-        if (out->trackingWasGood) kf->numFramesTrackedOnThis++;
-        fr->initialTrackedResidual = out->initialTrackedResidual;
-        for (int i = 0; i < 7; i++) fr->thisToParent[i] = out->frameToRef_qt[i];
-        fr->thisToParent[7] = 1.0;
-        fr->parentId = kf->id;
-    }
+    applyTrackedFrame(kf, fr, out);
     return 0;
 }
 
@@ -1326,22 +1333,13 @@ extern "C" int lsdgpu_track_and_map_group(int n, const lsdgpu_group_step* steps,
         r = ensureIdepthPyramid(ctx, kfs[i]);                // as lsdgpu_se3_track
         if (r) return groupPropagate(n, steps, i, r);
         inits[i] = st.frameToRef_init_qt;
-        sts[i] = st.settings;
-        if (!sts[i]) { lsdgpu_default_track_settings(&ds[i]); ds[i].maxItsPerLvl[4] = 0; sts[i] = &ds[i]; }
+        sts[i] = trackSettingsOrDefault(st.settings, ds[i]);
     }
     // 2-5. one launch on steps[0]'s stream for all the frames
     int failed = 0;
     int r = trackPersistentGroup(n, ctxs, kfs, frs, inits, sts, results, &failed);
     if (r) return groupPropagate(n, steps, failed, r);
-    for (int i = 0; i < n; i++) {                            // the Frame side effects of lsdgpu_se3_track
-        const lsdgpu_track_result* out = &results[i];
-        if (out->diverged) continue;
-        if (out->trackingWasGood) kfs[i]->numFramesTrackedOnThis++;                       // SE3Tracker.cpp:479-480
-        frs[i]->initialTrackedResidual = out->initialTrackedResidual;                     // :482
-        for (int k = 0; k < 7; k++) frs[i]->thisToParent[k] = out->frameToRef_qt[k];      // :483
-        frs[i]->thisToParent[7] = 1.0;
-        frs[i]->parentId = kfs[i]->id;                                                    // :484
-    }
+    for (int i = 0; i < n; i++) applyTrackedFrame(kfs[i], frs[i], &results[i]);    // as lsdgpu_se3_track
     // 6. mapping, each step on its own stream; a diverged step maps nothing.  The contexts are independent, so the order across
     // steps is free: the keyframe changes, whose createKeyFrame waits for its stream, go last so that the updates of the other
     // streams are already in flight.

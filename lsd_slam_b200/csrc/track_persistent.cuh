@@ -40,7 +40,6 @@
 #define TP_KMAX 3                    // poses per pass: the try + up to two speculative successors
 #define TP_ROW 64                    // floats per exchange row (256 B, one row per CTA; EV_NCHX = 56 used)
 #define TP_MAX_GROUP 8               // streams one group launch can track (lsdgpu_track_and_map_group)
-#define TP_CARRY_BITS 32             // level-1 chunk slots one thread can carry the last candidate's flags for in registers
 
 struct TrackLevelParams {
     const float* kfIdepth;
@@ -78,8 +77,8 @@ struct TrackParams {
     unsigned int* peerSync[TP_MAX_RANKS];     // each rank's `sync` block as mapped into THIS process (own entry = sync)
     uint8_t* peerMask[TP_MAX_RANKS];          // the tracked frame's level-1 mask on each rank
     unsigned int tailBase;                    // arrivals already counted on the tail barrier
-    // level-1 good flags of the last candidate of a pass: nullptr = in ThreadCarry::lastBits (a thread's level-1 slots fit in its
-    // TP_CARRY_BITS bits), otherwise in this level-1 plane of the context (always for a group launch; see fillTrackParams)
+    // level-1 good flags of the last candidate of a pass (the context's plane; goodMask holds candidate 0's), committed at the end
+    // of the launch if that candidate was the last pose the reference evaluates
     uint8_t* lastMask;
 };
 
@@ -108,16 +107,17 @@ struct TrackState {
 // the same Gv rows in the same order, so every sum, every LM decision and every result is bit-identical to k_track_persistent's.
 // A native grid of Gs CTAs would deal the chunks out differently and change the fp32 summation order.
 struct TrackGroupSeg {
-    TrackParams p;                   // the stream's parameters (nRanks == 1, debug == 0, lastMask set: ThreadCarry::lastBits would
-                                     // need up to ceil(Gv / Gs) times as many bits)
+    TrackParams p;                   // the stream's parameters (nRanks == 1, debug == 0)
     TrackState* out;                 // its context's mapped result block
 };
 
-// where a CTA sits in a group launch (unused by the single-stream instantiation)
+// Where a CTA sits in its launch.  The virtual grid has Gv = nRows * nRanks CTAs; the CTA walks row = b, b + Gs, ... < nRows and
+// evaluates virtual CTA v = row * nRanks + rank into partial row `row`.  k_track_persistent: {blockIdx.x, gridDim.x, gridDim.x},
+// one row per CTA (v = blockIdx.x * nRanks + rank); k_track_persistent_group: {blockIdx.x - s * Gs, Gs, Gv} with nRanks == 1.
 struct SegGrid {
     int b;                           // physical CTA within the segment
     int Gs;                          // physical CTAs of the segment (the barrier counts these)
-    int Gv;                          // virtual grid (rows of the combine) = the single-stream launch's grid
+    int nRows;                       // partial rows the combine adds
 };
 
 // Grid-wide barrier.  Arrivals are counted on one word (monotonic: epoch e completes at base + e * gridDim arrivals, the
@@ -234,13 +234,7 @@ struct ThreadCarry {
     int pcLvl;
     bool pcIsPoint;
     float pcx, pcy, pcz, pcVar, pcColor;
-    // level-1 good flags of the LAST candidate of the most recent pass, one bit per chunk slot of this thread (the mask itself
-    // always holds candidate 0's flags); committed at the end if that candidate was the last pose the reference evaluates.
-    // Only used while the thread's slots k = warp, warp + TP_WARPS, ... number at most TP_CARRY_BITS (TrackParams::lastMask).
-    unsigned int lastBits, pointBits;
 };
-static_assert(sizeof(ThreadCarry::lastBits) * 8 == TP_CARRY_BITS && sizeof(ThreadCarry::pointBits) * 8 == TP_CARRY_BITS,
-              "fillTrackParams sends a level through TrackParams::lastMask when a thread has more than TP_CARRY_BITS slots");
 
 // One pass: nPose candidate poses over this CTA's chunks of level `lvl`, CTA reduction, one row per CTA through L2 behind ONE
 // grid barrier, then every CTA sums the rows in block order.  On return sh.sums holds the totals, bit-identical in every CTA.
@@ -304,7 +298,6 @@ __device__ __forceinline__ void gridTailRanks(const TrackParams& p)
     __syncthreads();
 }
 
-template <bool GROUP>
 __device__ __forceinline__ void gridEvaluate(const TrackParams& p, const SegGrid& sg, int lvl, LMShared& sh, float (*sm)[EV_NCHX],
                                              float (*comb)[TP_ROW], unsigned int& epoch, long long* cyc, ThreadCarry& tc)
 {
@@ -312,34 +305,32 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, const SegGrid
     const TrackLevelParams& L = p.lvl[lvl];
     const int K = sh.nPose;
     const EvalPose P = sh.pose[0];
-    const int w = L.w, h = L.h, iw = L.iw, nInt = L.nInt, G = GROUP ? sg.Gs : (int)gridDim.x;
+    const int w = L.w, h = L.h, iw = L.iw, nInt = L.nInt;
     const float4* fg = L.frameGrad;
     uint8_t* mask = (lvl == SE3TRACKING_MIN_LEVEL) ? p.goodMask : nullptr;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    // chunks of this CTA: tpChunkOf(b, k, G), k = 0 .. nSlots-1 where it exists; warp `warp` takes k = warp, warp + 16, ...
-    // sharded over nRanks GPUs: the CTAs of all ranks form one virtual grid (this CTA is number b * nRanks + rank of it).
-    // In a group launch the CTA runs the virtual CTAs sg.b, sg.b + Gs, ... of the segment's virtual grid in turn.
-    const int Gv = GROUP ? sg.Gv : G * p.nRanks;
-    int vb = GROUP ? sg.b : (int)blockIdx.x * p.nRanks + p.rank;
+    // chunks of virtual CTA v: tpChunkOf(v, k, Gv), k = 0 .. nSlots-1 where it exists; warp `warp` takes k = warp, warp + 16, ...
+    // The CTA runs the virtual CTAs of its rows in turn (SegGrid); sharded over nRanks GPUs, the CTAs of all ranks form one
+    // virtual grid.
+    const int Gv = sg.nRows * p.nRanks;
     const int nSlots = (L.nChunks + Gv - 1) / Gv;
-    const bool lastInPlane = GROUP || p.lastMask != nullptr;
-    if (!lastInPlane && mask) { tc.lastBits = 0u; tc.pointBits = 0u; }
     const int nch = K > 1 ? EV_NCHX : EV_NCH;
     const unsigned int parity = epoch & 1u;
-    float* part = p.partials + (size_t)parity * TP_ROW * (GROUP ? (unsigned int)Gv : gridDim.x);
+    float* part = p.partials + (size_t)parity * TP_ROW * sg.nRows;
+    int row = sg.b;
     do {
+        const int vb = row * p.nRanks + p.rank;
         PointAcc acc;
         float ext[EV_NX];
 #pragma unroll
         for (int c = 0; c < EV_NCH; c++) acc.v[c] = 0.f;
 #pragma unroll
         for (int c = 0; c < EV_NX; c++) ext[c] = 0.f;
-        int slot = 0;
-        for (int k = warp; k < nSlots; k += TP_WARPS, slot++) {
+        for (int k = warp; k < nSlots; k += TP_WARPS) {
             const int chunk = tpChunkOf(vb, k, Gv);
             if (chunk >= L.nChunks) continue;                              // warp-uniform
             const int j = (chunk << 5) + lane;                             // interior pixel number
-            const bool firstChunk = (k == warp) && (!GROUP || vb == sg.b);  // the point cache holds the first virtual CTA's pixel
+            const bool firstChunk = k == warp && row == sg.b;              // the point cache holds the first virtual CTA's pixel
             bool isPoint = false;
             float px = 0.f, py = 0.f, pz = 0.f, var = 0.f, color = 0.f;
             int i = 0;
@@ -375,15 +366,11 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, const SegGrid
                 if (K > 1) {                                               // block-uniform
                     if (K > 2) evalPointLight<false>(px, py, pz, color, var, sh.pose[1], p.C, L.fx, L.fy, L.cx, L.cy, w, h, tap, ext);
                     const int goodL = evalPointLight<true>(px, py, pz, color, var, sh.pose[K - 1], p.C, L.fx, L.fy, L.cx, L.cy, w, h, tap, ext);
-                    if (mask) {
-                        if (lastInPlane) p.lastMask[i] = (uint8_t)goodL;
-                        else tc.lastBits |= (unsigned int)goodL << slot;
-                    }
+                    if (mask) p.lastMask[i] = (uint8_t)goodL;
                 }
                 if (mask) {
                     mask[i] = (uint8_t)good;
-                    if (!lastInPlane) tc.pointBits |= 1u << slot;
-                    if (!GROUP && p.nRanks > 1)                            // the other ranks own other chunks: give them this one's flag
+                    if (p.nRanks > 1)                                      // the other ranks own other chunks: give them this one's flag
                         for (int d = 0; d < p.nRanks; d++) if (d != p.rank) p.peerMask[d][i] = (uint8_t)good;
                 }
             }
@@ -402,14 +389,13 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, const SegGrid
         // ONE grid barrier, then every CTA combines all rows in a fixed order.  (Round 1 laid the buffer out [channel][cta]:
         // 40 four-byte writes per CTA into lines shared with 31 other CTAs -- 5 920 partial-sector writes per pass behind the
         // release of the barrier, and the combine's loads then waited ~5 000 cycles on those lines: 25 % of the kernel, ncu.)
-        // A group launch writes the row of every virtual CTA it stands in for; the next one reuses sm only after the
-        // __syncthreads that ends its chunk loop.
-        if (threadIdx.x < nch) __stcg(part + (size_t)(GROUP ? (unsigned int)vb : blockIdx.x) * TP_ROW + threadIdx.x, ctaSum);
-        vb += G;
-    } while (GROUP && vb < Gv);
+        // A CTA with several rows writes each of them; the next one reuses sm only after the __syncthreads that ends its chunk loop.
+        if (threadIdx.x < nch) __stcg(part + (size_t)row * TP_ROW + threadIdx.x, ctaSum);
+        row += sg.Gs;
+    } while (row < sg.nRows);
     epoch++;
     long long t2 = clock64();
-    gridBarrier(p.sync, p.barrierBase + epoch * (GROUP ? (unsigned int)G : gridDim.x));
+    gridBarrier(p.sync, p.barrierBase + epoch * (unsigned int)sg.Gs);
     long long t3 = clock64();
     // warp wi adds rows wi, wi+16, ... (<= 10): the lower half-warp takes the even ones of those, the upper half the odd ones, each
     // lane one float4 (4 channels) of a 256-byte row -- 5 vector loads per thread, all in flight before the first add.  fp32 adds
@@ -417,7 +403,7 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, const SegGrid
     // the same additions in the same order on the same data, so the totals are bit-identical everywhere, and the sums stay in
     // the precision the per-point accumulators and the reference's own (sequential fp32) sums have.
     {
-        const int nb = GROUP ? Gv : (int)gridDim.x;
+        const int nb = sg.nRows;
         const int half = lane >> 4, q = lane & 15;
         constexpr int NR = (TP_MAXGRID / TP_WARPS + 1) / 2;
         float4 v[NR];
@@ -443,7 +429,7 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, const SegGrid
         sh.sums[threadIdx.x] = t;
     }
     __syncthreads();
-    if (!GROUP && p.nRanks > 1) gridExchangeRanks(p, sh, nch, (p.launchSeq << 16) | (epoch & 0xffffu), epoch & 1u);
+    if (p.nRanks > 1) gridExchangeRanks(p, sh, nch, (p.launchSeq << 16) | (epoch & 0xffffu), epoch & 1u);
     long long t4 = clock64();
     cyc[0] += t1 - t0; cyc[1] += t2 - t1; cyc[2] += t3 - t2; cyc[3] += t4 - t3;
 }
@@ -550,7 +536,7 @@ struct LMState {
     int lvl, iteration, phase, incTry, diverged;
     int chainBase;                   // lm.incTry when the chain of the pass in flight was built
     int statsFrom;                   // where the statistics of the last evaluated pose are: 0 = main block, 1 = extension block
-    int commitLast;                  // 1: the good-mask of the last evaluated pose is in ThreadCarry::lastBits, not yet in the mask
+    int commitLast;                  // 1: the good-mask of the last evaluated pose is in TrackParams::lastMask, not yet in the mask
     int posesEvaluated;
     long long dbg[4];                // warp-0 cycles: decisions, chain building
 };
@@ -768,9 +754,8 @@ __device__ __forceinline__ void lmAdvance(const TrackParams& p, LMState& lm, LMS
     }
 }
 
-// The tracker of one stream.  GROUP = false: the whole grid (k_track_persistent); GROUP = true: one segment of a group launch
-// (k_track_persistent_group), whose position `sg` gives.  Both instantiations run the same passes, decisions and combine.
-template <bool GROUP>
+// The tracker of one stream on the CTAs `sg` describes: the whole grid (k_track_persistent) or one segment of a group launch
+// (k_track_persistent_group).  Both run the same passes, decisions and combine.
 __device__ __forceinline__ void trackStream(const TrackParams& p, TrackState* __restrict__ out, const SegGrid& sg)
 {
     __shared__ alignas(LMShared) unsigned char shStorage[sizeof(LMShared)];   // raw storage: Cand holds a type with a constructor
@@ -786,13 +771,11 @@ __device__ __forceinline__ void trackStream(const TrackParams& p, TrackState* __
     ThreadCarry tc;
     tc.pcLvl = -1; tc.pcIsPoint = false;
     tc.pcx = tc.pcy = tc.pcz = tc.pcVar = tc.pcColor = 0.f;
-    tc.lastBits = 0u; tc.pointBits = 0u;
 
     // fresh refPixelWasGood mask: all true (Frame.h:433); ordered before the level-1 passes by the barriers
     if (p.maskFresh) {
         uint32_t* m32 = reinterpret_cast<uint32_t*>(p.goodMask);
-        if (GROUP) for (int i = sg.b * TP_THREADS + threadIdx.x; i < p.maskBytes / 4; i += sg.Gs * TP_THREADS) m32[i] = 0x01010101u;
-        else for (int i = blockIdx.x * TP_THREADS + threadIdx.x; i < p.maskBytes / 4; i += gridDim.x * TP_THREADS) m32[i] = 0x01010101u;
+        for (int i = sg.b * TP_THREADS + threadIdx.x; i < p.maskBytes / 4; i += sg.Gs * TP_THREADS) m32[i] = 0x01010101u;
     }
 
     if (threadIdx.x == 0) {
@@ -810,7 +793,7 @@ __device__ __forceinline__ void trackStream(const TrackParams& p, TrackState* __
 
     while (true) {
         const int lvl = sh.lvl;
-        gridEvaluate<GROUP>(p, sg, lvl, sh, sm, comb, epoch, cyc, tc);
+        gridEvaluate(p, sg, lvl, sh, sm, comb, epoch, cyc, tc);
         if (threadIdx.x < 32) {
             if (threadIdx.x == 0) { lm.nEval[lvl]++; lm.nPts[lvl] = sh.sums[CH_REFNUM]; }
             lmAdvance(p, lm, sh, threadIdx.x);
@@ -820,17 +803,17 @@ __device__ __forceinline__ void trackStream(const TrackParams& p, TrackState* __
     }
 
     // The mask holds the flags of candidate 0 of the last level-1 pass; if the last pose the reference evaluates was the chain's
-    // last candidate instead, its flags (kept per thread) replace them now.  Same threads, same pixels: no synchronisation.
-    if ((GROUP || p.lastMask) && lm.commitLast && p.minLevel == SE3TRACKING_MIN_LEVEL) {
-        // the flags are in p.lastMask, written by this thread in the last pass for every point it evaluated; the points are found
-        // again from the keyframe planes (the test of gridEvaluate).  A group CTA runs the virtual CTAs sg.b, sg.b + Gs, ...
+    // last candidate instead, its flags (p.lastMask) replace them now.  Same threads, same pixels: no synchronisation.
+    if (lm.commitLast && p.minLevel == SE3TRACKING_MIN_LEVEL) {
+        // this thread wrote p.lastMask in the last pass for every point it evaluated; the points are found again from the keyframe
+        // planes (the test of gridEvaluate), row by row of the CTA as gridEvaluate walks them
         const TrackLevelParams& L = p.lvl[SE3TRACKING_MIN_LEVEL];
         const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-        const int Gv = GROUP ? sg.Gv : (int)gridDim.x * p.nRanks;
+        const int Gv = sg.nRows * p.nRanks;
         const int nSlots = (L.nChunks + Gv - 1) / Gv;
-        for (int v = GROUP ? sg.b : (int)blockIdx.x * p.nRanks + p.rank; v < Gv; v += GROUP ? sg.Gs : Gv)
+        for (int row = sg.b; row < sg.nRows; row += sg.Gs)
             for (int k = warp; k < nSlots; k += TP_WARPS) {
-                const int j = (tpChunkOf(v, k, Gv) << 5) + lane;
+                const int j = (tpChunkOf(row * p.nRanks + p.rank, k, Gv) << 5) + lane;
                 if (j >= L.nInt) continue;
                 const int yy = j / L.iw;
                 const int i = (j - yy * L.iw + 1) + (yy + 1) * L.w;
@@ -838,37 +821,20 @@ __device__ __forceinline__ void trackStream(const TrackParams& p, TrackState* __
                 if (var <= 0 || idepth == 0) continue;
                 const uint8_t g = p.lastMask[i];
                 p.goodMask[i] = g;
-                if (!GROUP && p.nRanks > 1)
+                if (p.nRanks > 1)
                     for (int d = 0; d < p.nRanks; d++) if (d != p.rank) p.peerMask[d][i] = g;
             }
     }
-    if (!GROUP && !p.lastMask && lm.commitLast && p.minLevel == SE3TRACKING_MIN_LEVEL) {
-        const TrackLevelParams& L = p.lvl[SE3TRACKING_MIN_LEVEL];
-        const int G = (int)gridDim.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-        const int Gv = G * p.nRanks, vb = (int)blockIdx.x * p.nRanks + p.rank;
-        const int nSlots = (L.nChunks + Gv - 1) / Gv;
-        int slot = 0;
-        for (int k = warp; k < nSlots; k += TP_WARPS, slot++) {
-            if (!((tc.pointBits >> slot) & 1u)) continue;
-            const int j = (tpChunkOf(vb, k, Gv) << 5) + lane;
-            const int yy = j / L.iw;
-            const int i = (j - yy * L.iw + 1) + (yy + 1) * L.w;
-            const uint8_t g = (uint8_t)((tc.lastBits >> slot) & 1u);
-            p.goodMask[i] = g;
-            if (p.nRanks > 1)
-                for (int d = 0; d < p.nRanks; d++) if (d != p.rank) p.peerMask[d][i] = g;
-        }
-    }
-    if (!GROUP && p.nRanks > 1) gridTailRanks(p);
+    if (p.nRanks > 1) gridTailRanks(p);
 
-    // the per-CTA cycle table (LSDGPU_TRACK_DEBUG) is written by single-stream launches only
-    if (!GROUP && p.debug && threadIdx.x == 0 && blockIdx.x < TP_MAXGRID - 1) {
+    // the per-CTA cycle table (LSDGPU_TRACK_DEBUG) is written by single-stream launches only (fillTrackParams leaves debug 0)
+    if (p.debug && threadIdx.x == 0 && sg.b < TP_MAXGRID - 1) {
         long long tot = clock64() - tStart;
-        for (int i = 0; i < 4; i++) out->cycBlk[blockIdx.x][i] = cyc[i];
-        out->cycBlk[blockIdx.x][5] = tot;
-        out->cycBlk[blockIdx.x][4] = tot - cyc[0] - cyc[1] - cyc[2] - cyc[3];
+        for (int i = 0; i < 4; i++) out->cycBlk[sg.b][i] = cyc[i];
+        out->cycBlk[sg.b][5] = tot;
+        out->cycBlk[sg.b][4] = tot - cyc[0] - cyc[1] - cyc[2] - cyc[3];
     }
-    if ((GROUP ? sg.b : (int)blockIdx.x) == 0 && threadIdx.x == 0) {
+    if (sg.b == 0 && threadIdx.x == 0) {
         // statistics of the LAST EVALUATED pose (SURVEY App. A-1): main block, or the extension block's last candidate
         float fin[EV_NCH];
         for (int c = 0; c < EV_NCH; c++) fin[c] = sh.sums[c];
@@ -895,7 +861,7 @@ __device__ __forceinline__ void trackStream(const TrackParams& p, TrackState* __
         cyc[5] = clock64() - tStart;
         cyc[4] = cyc[5] - cyc[0] - cyc[1] - cyc[2] - cyc[3];
         for (int i = 0; i < 6; i++) out->cyc[i] = cyc[i];
-        if (!GROUP && p.debug) for (int i = 0; i < 4; i++) out->cycBlk[TP_MAXGRID - 1][i] = lm.dbg[i];
+        if (p.debug) for (int i = 0; i < 4; i++) out->cycBlk[TP_MAXGRID - 1][i] = lm.dbg[i];
         __threadfence_system();
         out->doneSeq = p.launchSeq;
     }
@@ -903,7 +869,7 @@ __device__ __forceinline__ void trackStream(const TrackParams& p, TrackState* __
 
 __global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent(const __grid_constant__ TrackParams p, TrackState* __restrict__ out)
 {
-    trackStream<false>(p, out, SegGrid{});
+    trackStream(p, out, SegGrid{ (int)blockIdx.x, (int)gridDim.x, (int)gridDim.x });
 }
 
 // n streams in one cooperative launch of n * Gs CTAs: CTAs [s * Gs, (s + 1) * Gs) track segs[s] on a virtual grid of Gv CTAs
@@ -911,9 +877,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) k_track_persistent_group(const 
 {
     const int s = (int)blockIdx.x / Gs;
     const TrackGroupSeg& g = segs[s];
-    SegGrid sg;
-    sg.b = (int)blockIdx.x - s * Gs; sg.Gs = Gs; sg.Gv = Gv;
-    trackStream<true>(g.p, g.out, sg);
+    trackStream(g.p, g.out, SegGrid{ (int)blockIdx.x - s * Gs, Gs, Gv });
 }
 
 static cudaError_t trackPersistentSetup(lsdgpu_ctx* ctx)
@@ -938,12 +902,15 @@ static void flushTrackProfile(lsdgpu_ctx* ctx)
     ctx->trackProfilePending = false;
 }
 
-// level-1 chunk slots of the busiest thread of a single-stream launch: slots k = warp, warp + TP_WARPS, ... of its CTA's share
-static int level1SlotsPerThread(const lsdgpu_ctx* ctx, int nChunks)
+// one cooperative launch of a tracking kernel (every CTA co-resident: the grid barrier relies on it)
+static cudaError_t launchCooperative(const void* kernel, int grid, cudaStream_t stream, void** args)
 {
-    const int gv = ctx->trackGrid * ctx->nRanks;
-    const int slots = (nChunks + gv - 1) / gv;
-    return (slots + TP_WARPS - 1) / TP_WARPS;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(TP_THREADS); cfg.stream = stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    return cudaLaunchKernelExC(&cfg, kernel, args);
 }
 
 // the parameters of one frame's tracking on this context (single-GPU part; trackPersistent adds the peers of a sharded stream)
@@ -960,8 +927,7 @@ static void fillTrackParams(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const
         // no interior on a level 1 or 2 pixels wide or high (1x1 at 16x16): (w-2)*(h-2) would count (-1)*(-1) = 1 point
         L.iw = c.w - 2; L.nInt = std::max(c.w - 2, 0) * std::max(c.h - 2, 0); L.nChunks = (L.nInt + 31) / 32;
     }
-    // one bit per level-1 slot of a thread in ThreadCarry, or (more slots than bits, e.g. 4096x2160 on 132 SMs) the context's plane
-    P.lastMask = level1SlotsPerThread(ctx, P.lvl[SE3TRACKING_MIN_LEVEL].nChunks) > TP_CARRY_BITS ? ctx->dLastMask : nullptr;
+    P.lastMask = ctx->dLastMask;
     P.minLevel = SE3TRACKING_MIN_LEVEL;
     P.goodMask = fr->goodMask;
     P.maskFresh = fr->hasGoodMask ? 0 : 1;
@@ -1042,6 +1008,15 @@ static void translateTrackState(const lsdgpu_ctx* ctx, const TrackState* hOut, l
     for (int i = 0; i < 3; i++) out->frameToRef_qt[4 + i] = f2r.t[i];
 }
 
+// a stream's completed launch: its barrier counted `barrierCtas` arrivals per pass (the counter is never reset), and its result
+// block becomes `out`
+static void trackLaunchDone(lsdgpu_ctx* ctx, unsigned int barrierCtas, lsdgpu_track_result* out)
+{
+    const TrackState* hOut = (const TrackState*)ctx->hTrackState;
+    ctx->trkBase += (unsigned int)hOut->totalEvals * barrierCtas;
+    translateTrackState(ctx, hOut, out);
+}
+
 // track one frame: launch the kernel on the context's stream, wait for its result block and translate it (SE3Tracker.cpp:453-485)
 static int trackPersistent(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const double init_qt[7],
                            const lsdgpu_track_settings* st, lsdgpu_track_result* out)
@@ -1059,22 +1034,11 @@ static int trackPersistent(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const 
     if (ctx->nRanks > 1) ctx->trkTailBase += (unsigned int)ctx->trackGrid;
     TrackState* dOut = (TrackState*)ctx->dTrackStateMapped;
 
-    const int grid = ctx->trackGrid;                                               // one CTA per SM
     void* args[] = { (void*)&P, (void*)&dOut };
     P.debug = ctx->optTrackDebug ? 1 : 0;
-    if (ctx->optTrackDebug)
-        fprintf(stderr, "[track] level-1 slots per thread %d: last-candidate flags in %s\n",
-                level1SlotsPerThread(ctx, P.lvl[SE3TRACKING_MIN_LEVEL].nChunks), P.lastMask ? "the level-1 plane" : "registers");
     P.launchSeq = ++ctx->trackSeq;
     if (ctx->profileTrackKernel) cudaEventRecord(ctx->kBegin, ctx->stream);
-    {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(TP_THREADS); cfg.stream = ctx->stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
-        cfg.attrs = at; cfg.numAttrs = 1;
-        LSD_CHECK(ctx, cudaLaunchKernelExC(&cfg, (const void*)k_track_persistent, args));
-    }
+    LSD_CHECK(ctx, launchCooperative((const void*)k_track_persistent, ctx->trackGrid, ctx->stream, args));    // one CTA per SM
     ctx->launches++;
     if (ctx->profileTrackKernel) cudaEventRecord(ctx->kEnd, ctx->stream);
     fr->hasGoodMask = true;
@@ -1090,7 +1054,7 @@ static int trackPersistent(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const 
         const int r = waitTrackState(ctx, ctx->stream);
         if (r) return r;
     }
-    ctx->trkBase += (unsigned int)hOut->totalEvals * (unsigned int)ctx->trackGrid;    // the arrival counter is never reset
+    trackLaunchDone(ctx, (unsigned int)ctx->trackGrid, out);
 
     if (ctx->profileTrackKernel) {           // the event pair is read lazily (flushTrackProfile): no extra sync on the path
         ctx->trackKernelBytes += trackAlgorithmicBytes(ctx, hOut);
@@ -1123,7 +1087,6 @@ static int trackPersistent(lsdgpu_ctx* ctx, FrameSlot* kf, FrameSlot* fr, const 
             }
         }
     }
-    translateTrackState(ctx, hOut, out);
     return 0;
 }
 
@@ -1144,7 +1107,6 @@ static int trackPersistentGroup(int n, lsdgpu_ctx* const* ctxs, FrameSlot* const
         fillTrackParams(ctx, kfs[i], frs[i], initQts[i], sts[i], h[i].p);
         h[i].p.launchSeq = ++ctx->trackSeq;
         h[i].out = (TrackState*)ctx->dTrackStateMapped;
-        h[i].p.lastMask = ctx->dLastMask;
         if (i > 0) {
             LSD_CHECK(ctx, cudaEventRecord(ctx->groupEvent, ctx->stream));
             LSD_CHECK(c0, cudaStreamWaitEvent(c0->stream, ctx->groupEvent, 0));
@@ -1157,14 +1119,7 @@ static int trackPersistentGroup(int n, lsdgpu_ctx* const* ctxs, FrameSlot* const
     const TrackGroupSeg* dSegs = (const TrackGroupSeg*)c0->dGroupSegs;
     void* args[] = { (void*)&dSegs, (void*)&Gs, (void*)&Gv };
     if (c0->profileTrackKernel) cudaEventRecord(c0->kBegin, c0->stream);
-    {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(n * Gs); cfg.blockDim = dim3(TP_THREADS); cfg.stream = c0->stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
-        cfg.attrs = at; cfg.numAttrs = 1;
-        LSD_CHECK(c0, cudaLaunchKernelExC(&cfg, (const void*)k_track_persistent_group, args));
-    }
+    LSD_CHECK(c0, launchCooperative((const void*)k_track_persistent_group, n * Gs, c0->stream, args));
     c0->launches++;
     if (c0->profileTrackKernel) cudaEventRecord(c0->kEnd, c0->stream);
     LSD_CHECK(c0, cudaEventRecord(c0->groupEvent, c0->stream));
@@ -1181,10 +1136,8 @@ static int trackPersistentGroup(int n, lsdgpu_ctx* const* ctxs, FrameSlot* const
         *failed = i;
         const int r = waitTrackState(ctx, c0->stream);
         if (r) return r;
-        const TrackState* hOut = (const TrackState*)ctx->hTrackState;
-        ctx->trkBase += (unsigned int)hOut->totalEvals * (unsigned int)Gs;     // this segment's barrier counts Gs CTAs per pass
-        bytes += trackAlgorithmicBytes(ctx, hOut);
-        translateTrackState(ctx, hOut, &outs[i]);
+        bytes += trackAlgorithmicBytes(ctx, (const TrackState*)ctx->hTrackState);
+        trackLaunchDone(ctx, (unsigned int)Gs, &outs[i]);                       // this segment's barrier counts Gs CTAs per pass
     }
     if (c0->profileTrackKernel) {            // one launch for the whole group, accounted on the launching context
         c0->trackKernelBytes += bytes;
