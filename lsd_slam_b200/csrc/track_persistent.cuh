@@ -170,22 +170,29 @@ __device__ __forceinline__ void setEvalPose(EvalPose& P, const lsd::SE3<float>& 
 // instead of 5K: at every step the lanes of a pair exchange HALF of their values.  On return v[0] holds the
 // warp total of channel  chan = sum over used masks of (lane & mask ? half : 0)  (for K = 32: chan == lane).
 // Fixed exchange pattern => bit-identical results wherever the same data is reduced.
+// Each stage is its own instantiation (HALF a compile-time constant), so that every v[i + HALF] is a fixed register: written as one
+// loop over `half >>= 1` the array lived in local memory, a load and a store per element and stage (the CTA reduce was the largest
+// phase of the tracker's pass, DESIGN §6).  The lane's pick between the two values is a bit-mask select.
+template <int HALF, int K, typename T>
+__device__ __forceinline__ void warpReduceStage(T (&v)[K], int lane, int mask)
+{
+    const unsigned int up = (lane & mask) ? 0xffffffffu : 0u;
+#pragma unroll
+    for (int i = 0; i < HALF; i++) {
+        const unsigned int lo = __float_as_uint(v[i]), hi = __float_as_uint(v[i + HALF]);
+        const T keep = __uint_as_float((lo & ~up) | (hi & up));              // (lane & mask) ? v[i + HALF] : v[i]
+        const T send = __uint_as_float((hi & ~up) | (lo & up));              // (lane & mask) ? v[i] : v[i + HALF]
+        v[i] = keep + __shfl_xor_sync(0xffffffffu, send, mask);
+    }
+    if constexpr (HALF > 1) warpReduceStage<HALF / 2>(v, lane, mask >> 1);
+}
 template <int K, typename T>
 __device__ __forceinline__ void warpReduceMulti(T (&v)[K], int lane)
 {
-    int mask = 16;
+    static_assert(K >= 2 && K <= 32 && (K & (K - 1)) == 0, "K is a power of two in [2, 32]");
+    warpReduceStage<K / 2>(v, lane, 16);
 #pragma unroll
-    for (int half = K / 2; half >= 1; half >>= 1, mask >>= 1) {
-        const bool upper = (lane & mask) != 0;
-#pragma unroll
-        for (int i = 0; i < half; i++) {
-            T keep = upper ? v[i + half] : v[i];
-            T send = upper ? v[i] : v[i + half];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, mask);
-        }
-    }
-#pragma unroll
-    for (; mask >= 1; mask >>= 1) v[0] += __shfl_xor_sync(0xffffffffu, v[0], mask);
+    for (int mask = 16 / (K / 2) / 2; mask >= 1; mask >>= 1) v[0] += __shfl_xor_sync(0xffffffffu, v[0], mask);
 }
 // channel held in v[0] by `lane` after warpReduceMulti<K>
 template <int K> __device__ __forceinline__ int warpReduceChannel(int lane)
@@ -377,8 +384,8 @@ __device__ __forceinline__ void gridEvaluate(const TrackParams& p, const SegGrid
         }
         __syncthreads();
         t1 = clock64();
+        if (K > 1) warpReduceExt(ext, lane, sm[warp]);                    // first: its 16 registers are free for the 40 channels
         warpReduceAcc(acc, lane, sm[warp]);
-        if (K > 1) warpReduceExt(ext, lane, sm[warp]);
         __syncthreads();
         float ctaSum = 0.f;
         if (threadIdx.x < nch) {
