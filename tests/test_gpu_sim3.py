@@ -45,6 +45,19 @@ def _sim3_err(a, b):
     return dt, ang, abs(a[7] - b[7]) / b[7]
 
 
+def _check_eval(got, want):
+    """one Sim3 evaluation: the counts exactly, the normal equations and the residual and affine sums to SUM_TOL"""
+    assert got.warpedSize == want.warpedSize
+    assert (got.numTermsD, got.numTermsP, got.num_constraints) == (want.numTermsD, want.numTermsP, want.num_constraints)
+    A, Aw = np.array(got.A), np.array(want.A)
+    assert np.abs(A - Aw).max() <= SUM_TOL * np.abs(Aw).max()
+    bb, bw = np.array(got.b), np.array(want.b)
+    assert np.abs(bb - bw).max() <= SUM_TOL * np.abs(bw).max() + 1e-3 * np.abs(Aw).max() ** 0.5
+    for f in ("sumResD", "sumResP", "mean", "meanD", "meanP", "pointUsage", "affine_a_lastIt"):
+        assert abs(getattr(got, f) - getattr(want, f)) <= SUM_TOL * abs(getattr(want, f)), f
+    assert abs(got.affine_b_lastIt - want.affine_b_lastIt) <= 2e-2
+
+
 def test_sim3_eval_matches_oracle(oracle):
     seq, ctx, trk, of = _setup(oracle)
     for (ref, fr), lvl, a, b in (((0, 6), 4, 1.0, 0.0), ((0, 6), 2, 1.0, 0.0), ((6, 0), 1, 0.97, 1.5), ((0, 12), 3, 1.0, 0.0)):
@@ -52,15 +65,8 @@ def test_sim3_eval_matches_oracle(oracle):
         oracle.lib().lsdo_sim3d_inverse(_d(_init(seq, fr, ref)), _d(r2f))
         got = trk.eval(ref, fr, lvl, r2f, a, b)
         want = oracle.sim3_eval(of[ref], of[fr], lvl, r2f, a, b)
-        assert got.warpedSize == want.warpedSize > 100
-        assert (got.numTermsD, got.numTermsP, got.num_constraints) == (want.numTermsD, want.numTermsP, want.num_constraints)
-        A, Aw = np.array(got.A), np.array(want.A)
-        assert np.abs(A - Aw).max() <= SUM_TOL * np.abs(Aw).max()
-        bb, bw = np.array(got.b), np.array(want.b)
-        assert np.abs(bb - bw).max() <= SUM_TOL * np.abs(bw).max() + 1e-3 * np.abs(Aw).max() ** 0.5
-        for f in ("sumResD", "sumResP", "mean", "meanD", "meanP", "pointUsage", "affine_a_lastIt"):
-            assert abs(getattr(got, f) - getattr(want, f)) <= SUM_TOL * abs(getattr(want, f)), f
-        assert abs(got.affine_b_lastIt - want.affine_b_lastIt) <= 2e-2
+        assert want.warpedSize > 100
+        _check_eval(got, want)
     ctx.close()
 
 
