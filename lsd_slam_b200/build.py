@@ -7,9 +7,10 @@ import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-SRC = os.path.join(HERE, "csrc", "lsdgpu.cu")
+CSRC = os.path.join(HERE, "csrc")
+SRCS = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cu"))     # one unit per subsystem
 OUT = os.path.join(HERE, "liblsdgpu.so")
-DEPS = [os.path.join(HERE, "csrc", f) for f in os.listdir(os.path.join(HERE, "csrc"))] + [os.path.join(ROOT, "include", "lsdgpu.h")]
+DEPS = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(ROOT, "include", "lsdgpu.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -37,7 +38,7 @@ def needs_build() -> bool:
 def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not needs_build():
         return OUT
-    cmd = [nvcc_path()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", OUT, SRC]
+    cmd = [nvcc_path()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", OUT] + SRCS
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("nvcc failed:\n" + r.stdout + r.stderr)

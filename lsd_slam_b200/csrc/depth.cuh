@@ -9,7 +9,10 @@
 //   regularizeDepthMapRow<removeOcclusions>:758-848                        -> k_regularize<bool>
 //   propagateDepth                         :475-653                        -> k_prop_project + k_prop_resolve
 //   createKeyFrame rescale                 :1285-1304                      -> seqsum.cuh (the sequential fp32 sum) + k_rescale
-//   Frame::setDepth                        DataStructures/Frame.cpp:199-243 -> k_set_depth
+//   Frame::setDepth                        DataStructures/Frame.cpp:199-243 -> k_set_depth_pyr, or the SETDEPTH stage
+//                                                                              of k_fill_regularize
+//   Frame::takeReActivationData            DataStructures/Frame.cpp:107-145 -> k_take_reactivation
+//   setFromExistingKF                      :920-962                        -> k_set_from_existing
 // The reference's memcpy(other <- current) + read other / write current (:713, :862) is a ping-pong here:
 // every kernel reads `src` and writes every pixel of `dst`.
 //
@@ -685,28 +688,6 @@ __device__ __forceinline__ void finishSumCount(double s, int c, double* __restri
     }
 }
 
-// Frame::setDepth, Frame.cpp:199-243 (+ sum / count of the exported idepth_smoothed)
-__global__ void __launch_bounds__(256) k_set_depth(HypField cur, float* __restrict__ idepth, float* __restrict__ idepthVar,
-                                                   int n, double* __restrict__ partials, unsigned int* counter, double* __restrict__ out)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    double s = 0.0;
-    int c = 0;
-    if (i < n) {
-        float4 hf = cur.hf[i];
-        int4 hi = cur.hi[i];
-        if (hi.x && hf.z >= -0.05) {
-            idepth[i] = hf.z;
-            idepthVar[i] = hf.w;
-            s = hf.z;
-            c = 1;
-        } else {
-            idepth[i] = -1;
-            idepthVar[i] = -1;
-        }
-    }
-    finishSumCount(s, c, partials, counter, out);
-}
 // regularizeDepthMapFillHoles (DepthMap.cpp:656-718) immediately followed by regularizeDepthMap(false, TH)
 // (:758-880) -- the pair that updateKeyframe (:1135-1143), createKeyFrame (:1270-1277) and finalizeKeyFrame
 // (:1373-1379) always run back to back -- as ONE kernel, optionally (SETDEPTH) followed in the same kernel by
@@ -957,17 +938,6 @@ __global__ void __launch_bounds__(256) k_set_depth_pyr(HypField cur, PyrPtrs id,
     finishSumCount(s, c, partials, counter, out);
 }
 
-// sum of idepth_smoothed over valid hypotheses in double (not used by createKeyFrame any more: seqsum.cuh reproduces the
-// reference's sequential fp32 sum there; kept for diagnostics)
-__global__ void __launch_bounds__(256) k_sum_idepth(HypField cur, int n, double* __restrict__ partials, unsigned int* counter,
-                                                    double* __restrict__ out)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    double s = 0.0;
-    int c = 0;
-    if (i < n && cur.hi[i].x) { s = cur.hf[i].z; c = 1; }
-    finishSumCount(s, c, partials, counter, out);
-}
 // createKeyFrame :1295-1304
 __global__ void __launch_bounds__(256) k_rescale(HypField cur, int n, const double* __restrict__ scal)
 {
@@ -1136,5 +1106,42 @@ __global__ void k_integral_cols(int* __restrict__ integral, int w, int h)
     for (int y = 1; y < h; y++) {
         s += integral[y * w + x];
         integral[y * w + x] = s;
+    }
+}
+
+// Frame::takeReActivationData: entries of invalid pixels keep idepth / validity (only the variance code is written)
+__global__ void __launch_bounds__(256) k_take_reactivation(HypField cur, float* __restrict__ idepthReAct, float* __restrict__ varReAct,
+                                                           uint8_t* __restrict__ validityReAct, int n)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int4 hi = cur.hi[i];
+    if (hi.x) {
+        const float4 hf = cur.hf[i];
+        idepthReAct[i] = hf.x;
+        varReAct[i] = hf.y;
+        validityReAct[i] = (uint8_t)hi.z;
+    } else if (hi.y < -1)                       // blacklisted < MIN_BLACKLIST (util/settings.h:117)
+        varReAct[i] = -2;
+    else
+        varReAct[i] = -1;
+}
+
+// DepthMap::setFromExistingKF: DepthMapPixelHypothesis(idepth, idepth_var, validity) (DepthMapPixelHypothesis.h:80-91) or
+// invalid with the blacklist code; fields the reference leaves untouched on invalid pixels are left untouched here too
+__global__ void __launch_bounds__(256) k_set_from_existing(const float* __restrict__ idepthReAct, const float* __restrict__ varReAct,
+                                                           const uint8_t* __restrict__ validityReAct, HypField cur, int n)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float var = varReAct[i];
+    if (var > 0) {
+        cur.hf[i] = make_float4(idepthReAct[i], var, -1.f, -1.f);
+        cur.hi[i] = make_int4(1, 0, (int)validityReAct[i], 0);
+    } else {
+        int4 hi = cur.hi[i];
+        hi.x = 0;
+        hi.y = (var == -2) ? -2 : 0;            // MIN_BLACKLIST - 1
+        cur.hi[i] = hi;
     }
 }

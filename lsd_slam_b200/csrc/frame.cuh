@@ -13,9 +13,6 @@
 #pragma once
 #include "internal.cuh"
 
-struct PyrPtrs {
-    float* l[LSD_LEVELS];
-};
 // One CTA = one 16x16 level-0 tile -> 8x8, 4x4, 2x2, 1x1 on levels 1..4 (w, h are multiples of 16,
 // SlamSystem.cpp:55).  The 2x2 box sum is exact in fp32 for u8-origin data (SURVEY App. A-11) and is
 // associated like the scalar loop (Frame.cpp:621-624).
@@ -198,28 +195,7 @@ __global__ void __launch_bounds__(256) k_set_depth_gt(const float* __restrict__ 
     }
 }
 
-// Frame::buildIDepthAndIDepthVar for levels 1..4 in one launch: one CTA = one 16x16 level-0 tile.
-__device__ __forceinline__ float2 mergeIdepth4(float2 a, float2 b, float2 c, float2 d)
-{   // Frame.cpp:819-871, sources visited in the order idx, idx+1, idx+sw, idx+sw+1; .x = idepth, .y = var
-    float idepthSumsSum = 0, ivarSumsSum = 0;
-    int num = 0;
-    float2 s[4] = { a, b, c, d };
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        float var = s[k].y;
-        if (var > 0) {
-            float ivar = 1.0f / var;
-            ivarSumsSum += ivar;
-            idepthSumsSum += ivar * s[k].x;
-            num++;
-        }
-    }
-    if (num > 0) {
-        float depth = ivarSumsSum / idepthSumsSum;
-        return make_float2(1.0f / depth, num / ivarSumsSum);
-    }
-    return make_float2(-1.f, -1.f);
-}
+// Frame::buildIDepthAndIDepthVar for levels 1..4 in one launch: one CTA = one 16x16 level-0 tile (mergeIdepth4, internal.cuh).
 __global__ void __launch_bounds__(256) k_idepth_pyramid(PyrPtrs id, PyrPtrs var, int w, int h)
 {
     __shared__ float2 s0[16][17], s1[8][9], s2[4][5], s3[2][3];

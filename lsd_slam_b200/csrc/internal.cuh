@@ -62,6 +62,10 @@ struct FrameSlot {
     int numFramesTrackedOnThis = 0, numMappedOnThis = 0;
 };
 
+struct PyrPtrs {
+    float* l[LSD_LEVELS];
+};
+
 struct HypField {
     float4* hf;
     int4* hi;
@@ -83,6 +87,8 @@ struct RefConst {
 #define LSD_MAX_PERMA_BATCH 4096
 #define LSD_MAX_REFS 16
 #define LSD_MAX_ID_SPAN 64
+#define SEQ_NBIN 24          // sequential fp32 sum (seqsum.cuh): binades 2^0 .. 2^23 are tabulated
+#define SEQ_RUN 256          // pixels per tabulated run (one warp, 8 per lane)
 struct ObserveParams {
     RefConst refs[LSD_MAX_REFS];
     int nRefs;
@@ -204,6 +210,8 @@ struct CtxLock {
 };
 #define LSD_LOCK(ctx) CtxLock lsd_lock_(ctx)
 
+#define LAUNCH(ctx) ((ctx)->launches++)
+
 #define LSD_CHECK(ctx, expr)                                                                              \
     do {                                                                                                  \
         cudaError_t _e = (expr);                                                                          \
@@ -249,6 +257,12 @@ static inline FrameSlot* findSlot(lsdgpu_ctx* ctx, int id)
 }
 
 static inline int divUp(int a, int b) { return (a + b - 1) / b; }
+static inline size_t alignUp(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// ---- host helpers shared by the units of the library (each defined once, in the unit named) ---------------------------
+int ensureIdepthPyramid(lsdgpu_ctx* ctx, FrameSlot* s);     // frames.cu: levels 1..4 of a keyframe's idepth / idepthVar
+cudaError_t trackPersistentSetup(lsdgpu_ctx* ctx);          // tracking.cu: launch shape of the persistent tracker
+void cloudRelease(lsdgpu_ctx* ctx);                         // output.cu: frees the point-cloud reservation
 
 // ---- device helpers shared by all kernels --------------------------------------------------------------
 // util/settings.h:34-35.  UNZERO mixes float and double literals; every use converts back to float.
@@ -266,6 +280,29 @@ __device__ __forceinline__ float interpF(const float* __restrict__ mat, float x,
     float dxdy = dx * dy;
     const float* bp = mat + ix + iy * width;
     return dxdy * __ldg(bp + 1 + width) + (dy - dxdy) * __ldg(bp + width) + (dx - dxdy) * __ldg(bp + 1) + (1 - dx - dy + dxdy) * __ldg(bp);
+}
+
+// Frame::buildIDepthAndIDepthVar: one coarser idepth / idepthVar pixel from its four finer ones (frame.cuh, depth.cuh)
+__device__ __forceinline__ float2 mergeIdepth4(float2 a, float2 b, float2 c, float2 d)
+{   // Frame.cpp:819-871, sources visited in the order idx, idx+1, idx+sw, idx+sw+1; .x = idepth, .y = var
+    float idepthSumsSum = 0, ivarSumsSum = 0;
+    int num = 0;
+    float2 s[4] = { a, b, c, d };
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        float var = s[k].y;
+        if (var > 0) {
+            float ivar = 1.0f / var;
+            ivarSumsSum += ivar;
+            idepthSumsSum += ivar * s[k].x;
+            num++;
+        }
+    }
+    if (num > 0) {
+        float depth = ivarSumsSum / idepthSumsSum;
+        return make_float2(1.0f / depth, num / ivarSumsSum);
+    }
+    return make_float2(-1.f, -1.f);
 }
 
 // Frame::prepareForStereoWith, DataStructures/Frame.cpp:295-317 (host, double -> float like the reference)

@@ -5,8 +5,6 @@
 //   ROSOutput3DWrapper::publishKeyframe, packing loop   IOWrapper/ROS/ROSOutput3DWrapper.cpp:91-110
 //       InputPointDense {float idepth; float idepth_var; uchar color[4];}   IOWrapper/ROS/ROSOutput3DWrapper.h:34-39
 //       (= lsd_slam_viewer/msg/keyframeMsg.msg:20-22 `uint8[] pointcloud`, 12 bytes per pixel of the publish level)
-//   Frame::takeReActivationData                         DataStructures/Frame.cpp:107-145
-//   DepthMap::setFromExistingKF, hypothesis loop        DepthEstimation/DepthMap.cpp:920-958
 #pragma once
 #include "internal.cuh"
 
@@ -26,41 +24,4 @@ __global__ void __launch_bounds__(256) k_pack_pointcloud(const float* __restrict
         v = c * 0x01010101u;
     }
     out[j] = v;
-}
-
-// Frame::takeReActivationData: entries of invalid pixels keep idepth / validity (only the variance code is written)
-__global__ void __launch_bounds__(256) k_take_reactivation(HypField cur, float* __restrict__ idepthReAct, float* __restrict__ varReAct,
-                                                           uint8_t* __restrict__ validityReAct, int n)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int4 hi = cur.hi[i];
-    if (hi.x) {
-        const float4 hf = cur.hf[i];
-        idepthReAct[i] = hf.x;
-        varReAct[i] = hf.y;
-        validityReAct[i] = (uint8_t)hi.z;
-    } else if (hi.y < -1)                       // blacklisted < MIN_BLACKLIST (util/settings.h:117)
-        varReAct[i] = -2;
-    else
-        varReAct[i] = -1;
-}
-
-// DepthMap::setFromExistingKF: DepthMapPixelHypothesis(idepth, idepth_var, validity) (DepthMapPixelHypothesis.h:80-91) or
-// invalid with the blacklist code; fields the reference leaves untouched on invalid pixels are left untouched here too
-__global__ void __launch_bounds__(256) k_set_from_existing(const float* __restrict__ idepthReAct, const float* __restrict__ varReAct,
-                                                           const uint8_t* __restrict__ validityReAct, HypField cur, int n)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const float var = varReAct[i];
-    if (var > 0) {
-        cur.hf[i] = make_float4(idepthReAct[i], var, -1.f, -1.f);
-        cur.hi[i] = make_int4(1, 0, (int)validityReAct[i], 0);
-    } else {
-        int4 hi = cur.hi[i];
-        hi.x = 0;
-        hi.y = (var == -2) ? -2 : 0;            // MIN_BLACKLIST - 1
-        cur.hi[i] = hi;
-    }
 }

@@ -9,25 +9,10 @@
 // is one launch: one CTA per candidate runs the complete level-4 LM loop on its own (the problems are independent, so
 // there is no grid barrier and no exchange at all) with the same evalPoint() / lmAdvance() as the main tracker (one pose per pass: kmax = 1).
 #pragma once
-#include "internal.cuh"
-#include "track.cuh"
-#include "track_persistent.cuh"
+#include "track_common.cuh"
 
 #define QUICK_KF_CHECK_LVL 4            // util/settings.h:104
 #define PERMA_THREADS 256
-
-struct PermaItem {
-    const float4* pc;                   // (x, y, z, colour) per point
-    const float* var;                   // idepthVar per point
-    int n;                              // permaRefNumPts
-    float refToFrame[7];                // initial estimate, already cast to float (SE3Tracker.cpp:125,168)
-};
-struct PermaResult {
-    float refToFrame[7];
-    float pointUsage, goodCount, badCount, meanRes, lastResidual;
-    float affine_a, affine_b;
-    int diverged, nRes, nUpd;
-};
 
 // checkPermaRefOverlap for a list of candidates: CTA b -> usage[b]
 __global__ void __launch_bounds__(128) k_perma_overlap(const PermaItem* __restrict__ items, float fx_l, float fy_l, float cx_l, float cy_l,

@@ -17,10 +17,8 @@
 // s not a positive normal number) is added with a real float add, one element at a time, so the result is the sequential sum
 // for ANY input; the fast path only needs the positive terms the mapper produces.
 #pragma once
-#include <cuda_runtime.h>
+#include "internal.cuh"      // SEQ_NBIN, SEQ_RUN
 
-#define SEQ_NBIN 24          // binades 2^0 .. 2^23 are tabulated
-#define SEQ_RUN 256          // pixels per tabulated run (one warp, 8 per lane)
 #define SEQ_SAT (1 << 28)    // saturation of the increments: > 2^24, so "reached 2^24" survives, and below 2^24 nothing saturates
 
 struct SeqMap { int d0, d1; };   // S -> S + (S even ? d0 : d1)

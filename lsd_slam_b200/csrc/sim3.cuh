@@ -16,27 +16,11 @@
 // on thread 0 -- so there is no grid barrier, no global-memory exchange and no host round trip inside a tracking.
 #pragma once
 #include <cooperative_groups.h>
-#include "internal.cuh"
-#include "track.cuh"
-#include "track_persistent.cuh"
+#include "track_common.cuh"
 
 namespace cg = cooperative_groups;
 
 #define S3_THREADS 512
-#define S3_MAX_BATCH 1024
-
-// reduction channels of one evaluation
-enum {
-    S3_A6 = 0,      // 21: upper triangle of sum v v^T wp            (LGS6::update, LGSX.h:390-396)
-    S3_B6 = 21,     // 6:  sum v rp wp                               (LGS6::b = -this)
-    S3_A4 = 27,     // 10: upper triangle of sum v4 v4^T wd          (LGS4::update, LGSX.h:163-169)
-    S3_B4 = 37,     // 4:  sum v4 rd wd                              (LGS4::b = -this)
-    S3_RESD = 41, S3_RESP = 42, S3_NUMD = 43, S3_NUMP = 44,          // Sim3ResidualStruct; numTermsP == buf_warped_size
-    S3_USAGE = 45, S3_REFNUM = 46,
-    S3_SXX = 47, S3_SYY = 48, S3_SX = 49, S3_SY = 50, S3_SW = 51,
-    S3_NCH = 52
-};
-#define S3_NLGS 41                      // channels [0, 41) are the normal equations
 
 struct Sim3Level {
     int w, h;
@@ -51,25 +35,6 @@ struct Sim3Params {
     int startLevel, finalLevel;
     int evalOnly;                       // 1: one evaluation at level startLevel with the given pose / affine (parity hook)
     float evalA, evalB;
-};
-struct Sim3Item {
-    const float* kfIdepth[LSD_LEVELS];  // reference keyframe (the TrackingReference)
-    const float* kfVar[LSD_LEVELS];
-    const float4* kfGrad[LSD_LEVELS];   // (dx, dy, I, -): gradData and colour of makePointCloud in one texel
-    const float4* frGrad[LSD_LEVELS];   // frame
-    const float* frIdepth[LSD_LEVELS];
-    const float* frVar[LSD_LEVELS];
-    double refToFrame[7];               // initial referenceToFrame: scaled quaternion (x,y,z,w) + translation
-};
-struct Sim3Out {
-    double refToFrame[7];
-    float sums[S3_NCH];                 // the last evaluation
-    float lgs[S3_NLGS];                 // normal-equation sums of the pose ls7 belongs to
-    float resMean, resMeanD, resMeanP;  // finalResidual
-    float pointUsage, affine_a, affine_b;
-    int early;                          // 0: ok, 1: diverged (too few points), 2: increment out of range
-    int nRes[LSD_LEVELS], nUpd[LSD_LEVELS];
-    long long cyc[4];                   // thread-0 clock64 totals: pixel loop, CTA reduce, cluster exchange, serial LM step
 };
 
 struct Sim3Pose {
@@ -212,48 +177,6 @@ LSD_HD void sim3AssembleLGS7(const float* lgs, float A7[49], float b7[7])
         b7[remap[i]] += -lgs[S3_B4 + i];
         for (int j = 0; j < 4; j++) A7[remap[i] * 7 + remap[j]] += A4[i * 4 + j];
     }
-}
-
-// Fully unrolled, register-resident LDL^T without pivoting for the damped 7x7 system; false if a pivot is not strictly
-// positive (the caller then falls back to the pivoted routine of hostmath.h, which is what Eigen's ldlt() does).
-template <int N> __device__ __forceinline__ bool ldltSolveFast(const float* A, const float* b, float* x)
-{
-    float Lm[N][N], D[N];
-    bool ok = true;
-#pragma unroll
-    for (int j = 0; j < N; j++) {
-        float d = A[j * N + j];
-#pragma unroll
-        for (int k = 0; k < j; k++) d -= Lm[j][k] * Lm[j][k] * D[k];
-        D[j] = d;
-        ok = ok && (d > 0.f);
-        const float inv = 1.0f / d;
-#pragma unroll
-        for (int i = j + 1; i < N; i++) {
-            float v = A[i * N + j];
-#pragma unroll
-            for (int k = 0; k < j; k++) v -= Lm[i][k] * Lm[j][k] * D[k];
-            Lm[i][j] = v * inv;
-        }
-    }
-    float y[N];
-#pragma unroll
-    for (int i = 0; i < N; i++) {
-        float s = b[i];
-#pragma unroll
-        for (int k = 0; k < i; k++) s -= Lm[i][k] * y[k];
-        y[i] = s;
-    }
-#pragma unroll
-    for (int i = 0; i < N; i++) y[i] = y[i] / D[i];
-#pragma unroll
-    for (int i = N - 1; i >= 0; i--) {
-        float s = y[i];
-#pragma unroll
-        for (int k = i + 1; k < N; k++) s -= Lm[k][i] * x[k];
-        x[i] = s;
-    }
-    return ok;
 }
 
 // ---- the LM state machine of trackFrameSim3 (thread 0 of every CTA, identical in all CTAs of a cluster) -----------

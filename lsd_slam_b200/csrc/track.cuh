@@ -1,4 +1,5 @@
-// track.cuh -- the fused warp / residual / weight / Jacobian / normal-equation kernel of SE3Tracker.
+// track.cuh -- the fused warp / residual / weight / Jacobian / normal-equation evaluation of SE3Tracker (device code; the
+// stand-alone evaluation kernel k_se3_eval is in tracking.cu, the persistent tracker in track_persistent.cuh).
 //
 // Replaces (paths relative to lsd_slam_core/src/):
 //   TrackingReference::makePointCloud     Tracking/TrackingReference.cpp:96-147   (never materialised: each
@@ -236,85 +237,9 @@ __device__ __forceinline__ int evalPointLight(float px, float py, float pz, floa
     return isGood ? 1 : 0;
 }
 
-// CTA-level reduction of all channels: warp shuffles, then one smem stage.  Result valid in warp 0, lane c.
-template <int NWARPS>
-__device__ __forceinline__ void blockReduceChannels(PointAcc& acc, float (*sm)[EV_NCH], float* blockRow)
-{
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int c = 0; c < EV_NCH; c++) {
-        float v = acc.v[c];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) sm[warp][c] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < EV_NCH) {
-        float s = 0.f;
-#pragma unroll
-        for (int wi = 0; wi < NWARPS; wi++) s += sm[wi][threadIdx.x];
-        blockRow[threadIdx.x] = s;
-    }
-}
-
-#define EVAL_THREADS 256
-
-// Stand-alone evaluation kernel (one launch per LM evaluation; mode-0 tracker and the parity hook).
-__global__ void __launch_bounds__(EVAL_THREADS) k_se3_eval(EvalLevel L, EvalPose P, EvalConsts C,
-                                                           float* __restrict__ partials, unsigned int* counter,
-                                                           float* __restrict__ out)
-{
-    __shared__ float sm[EVAL_THREADS / 32][EV_NCH];
-    __shared__ bool isLast;
-    PointAcc acc;
-#pragma unroll
-    for (int c = 0; c < EV_NCH; c++) acc.v[c] = 0.f;
-
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int w = L.w, h = L.h;
-    if (i < w * h) {
-        const int x = i % w, y = i / w;
-        if (x >= 1 && x < w - 1 && y >= 1 && y < h - 1 && (L.nShards <= 1 || ((i >> 5) % L.nShards) == L.shard)) {
-            const float idepth = L.kfIdepth[i], var = L.kfVar[i];
-            if (!(var <= 0 || idepth == 0)) {                     // TrackingReference.cpp:133
-                const float sc = 1.0f / idepth;                   // :135
-                const float px = sc * (L.fxi * x + L.cxi), py = sc * (L.fyi * y + L.cyi), pz = sc * 1;
-                const float4* fg = L.frameGrad;
-                auto tap = [fg, w](float u, float v, float& o0, float& o1, float& o2) { interp43(fg, u, v, w, o0, o1, o2); };
-                int good = evalPoint(px, py, pz, L.kfColor[i], var, P, C, L.fx, L.fy, L.cx, L.cy, w, h, tap, acc);
-                if (L.goodMask) L.goodMask[i] = (uint8_t)good;
-            }
-        }
-    }
-    blockReduceChannels<EVAL_THREADS / 32>(acc, sm, partials + (size_t)blockIdx.x * EV_NCH);
-
-    // last-CTA-done: deterministic cross-block sum in block order
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        unsigned int t = atomicAdd(counter, 1u);
-        isLast = (t == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (isLast) {
-        __threadfence();
-        // EV_NCH channels x 4 partial lanes each (fixed interleave), then a fixed 4-way combine
-        const int c = threadIdx.x >> 2, part = threadIdx.x & 3;
-        if (c < EV_NCH) {
-            double s = 0.0;
-            for (int b = part; b < (int)gridDim.x; b += 4) s += (double)__ldcg(partials + (size_t)b * EV_NCH + c);
-            s += __shfl_xor_sync(0xffffffffu, s, 1);
-            s += __shfl_xor_sync(0xffffffffu, s, 2);
-            if (part == 0) out[c] = (float)s;
-        }
-        if (threadIdx.x == 0) *counter = 0;
-    }
-}
+#define EVAL_THREADS 256                 // threads per CTA of k_se3_eval (tracking.cu)
 
 // ---- host-side interpretation of the EV_NCH sums (shared by mode 0, the parity hook and mode 1) ----------
-struct EvalSums {
-    float v[EV_NCH];
-};
 LSD_HD void evalFinish(const float* s, lsdgpu_eval_result* r)
 {
     static const unsigned char ij[21][2] = { {0,0},{0,1},{0,2},{0,3},{0,4},{0,5},{1,1},{1,2},{1,3},{1,4},{1,5},
