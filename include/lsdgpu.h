@@ -209,7 +209,7 @@ int lsdgpu_track_and_map_group(int n, const lsdgpu_group_step* steps, lsdgpu_tra
  * otherwise fx fy cx cy 0 (relative to the output size).  Host-only (no context needed): fills the two remap tables
  * (out_width*out_height floats each, may be NULL) and K_out (row-major, the matrix main_on_images.cpp:164-169 hands to
  * SlamSystem).  Returns 0 = tables valid, 1 = undistort() passes the image through (:370-375), -2 = invalid arguments.
- * UndistorterOpenCV (:449-567) delegates to cv::initUndistortRectifyMap / cv::remap and stays on the host. */
+ * The OpenCV model (UndistorterOpenCV, :449-567) has its own entry points below. */
 int lsdgpu_undistorter_ptam_prepare(const float input_calibration[5], int in_width, int in_height, const float output_calibration[5],
                                     int out_width, int out_height, float* remapX, float* remapY, float K_out[9]);
 /* host-only check of a pair of remap tables: every entry is either "no source" (x < 0, as Undistorter.cpp:312-316 writes it)
@@ -220,7 +220,26 @@ int lsdgpu_undistorter_validate_tables(int in_width, int in_height, int out_widt
  * NULL tables = pass-through (then in_width/in_height must equal the context's size).  Tables that fail
  * lsdgpu_undistorter_validate_tables are rejected (the gather kernel does no bounds checks of its own). */
 int lsdgpu_set_undistorter(lsdgpu_ctx* ctx, int in_width, int in_height, const float* remapX, const float* remapY);
-/* UndistorterPTAM::undistort, util/Undistorter.cpp:355-411: raw (in_width*in_height) -> out (w*h), 8 bit */
+/* ---- input staging: UndistorterOpenCV (radial-tangential fx fy cx cy k1 k2 p1 p2) fused into the Frame construction ----------
+ * Found by symbol lookup (dlsym), like lsdgpu_track_and_map_group; LSDGPU_ABI_VERSION is unchanged.
+ * UndistorterOpenCV::UndistorterOpenCV, util/Undistorter.cpp:449-558, with the four lines of the calibration file already parsed.
+ * Host-only (no context needed).  input_calibration = fx fy cx cy k1 k2 p1 p2 (pixels; cx < 1 means relative units, rescaled in
+ * float as :519-534 does); output_mode = -1 "crop" (alpha 0) or -2 "full" (alpha 1).  Fills, each may be NULL:
+ *   map1   2*out_width*out_height int16  (x, y) integer source positions   \  cv::initUndistortRectifyMap(.., CV_16SC2) of
+ *   map2   out_width*out_height uint16   (y_frac << 5 | x_frac), 1/32 px   /  OpenCV 4.13, bit for bit
+ *   K_new  row-major doubles = cv::getOptimalNewCameraMatrix(K, D, in_size, alpha, out_size, NULL, false)
+ *   K_out  row-major floats = the K main_on_images.cpp:164-167 reads back from UndistorterOpenCV::getK() and hands to SlamSystem
+ * Returns 0 = valid, -2 = invalid (bad sizes, an output mode other than crop / full -- "none" and explicit output parameters make
+ * the reference's undistorter invalid, :493-502). */
+int lsdgpu_undistorter_opencv_prepare(const float input_calibration[8], int in_width, int in_height, int output_mode,
+                                      int out_width, int out_height, int16_t* map1, uint16_t* map2, double K_new[9], float K_out[9]);
+/* install OpenCV remap maps (host pointers, w*h entries each; w, h = the context's size) for raw images of in_width x in_height.
+ * They may come from lsdgpu_undistorter_opencv_prepare or from the host's own cv::initUndistortRectifyMap(.., CV_16SC2) (e.g. the
+ * map1 / map2 members of a host-side UndistorterOpenCV, Undistorter.cpp:547-548).  Every tap is bounds-checked on the device (a tap
+ * outside the raw image reads 0, cv::BORDER_CONSTANT), so any maps are accepted.  Installing either model replaces the other. */
+int lsdgpu_set_undistorter_opencv(lsdgpu_ctx* ctx, int in_width, int in_height, const int16_t* map1, const uint16_t* map2);
+/* UndistorterPTAM::undistort, util/Undistorter.cpp:355-411, or UndistorterOpenCV::undistort (:564-567, cv::remap INTER_LINEAR
+ * with a constant 0 border), whichever is installed: raw (in_width*in_height) -> out (w*h), 8 bit */
 int lsdgpu_undistort_u8(lsdgpu_ctx* ctx, const uint8_t* raw, uint8_t* out);
 /* undistort + Frame::Frame(id, w, h, K, ts, const uchar*) + buildImage/buildGradients/buildMaxGradients of all levels:
  * the raw image is copied to the device once and the remap feeds the pyramid kernel directly

@@ -170,6 +170,9 @@ SYMBOLS = [
     ("lsdgpu_undistorter_ptam_prepare", C.c_int, [_fp, C.c_int, C.c_int, _fp, C.c_int, C.c_int, _fp, _fp, _fp]),
     ("lsdgpu_undistorter_validate_tables", C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, _fp, _fp]),
     ("lsdgpu_set_undistorter", C.c_int, [_vp, C.c_int, C.c_int, _fp, _fp]),
+    ("lsdgpu_undistorter_opencv_prepare", C.c_int, [_fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int16),
+                                                    C.POINTER(C.c_uint16), _dp, _fp]),
+    ("lsdgpu_set_undistorter_opencv", C.c_int, [_vp, C.c_int, C.c_int, C.POINTER(C.c_int16), C.POINTER(C.c_uint16)]),
     ("lsdgpu_undistort_u8", C.c_int, [_vp, C.POINTER(C.c_uint8), C.POINTER(C.c_uint8)]),
     ("lsdgpu_frame_upload_distorted_u8", C.c_int, [_vp, C.c_int, C.POINTER(C.c_uint8)]),
     ("lsdgpu_keyframe_pack_pointcloud", C.c_int, [_vp, C.c_int, C.c_int, _vp]),
@@ -269,6 +272,42 @@ class UndistorterPTAM:
             ctx._ck(ctx.L.lsdgpu_set_undistorter(ctx.ptr, self.in_w, self.in_h, None, None))
         else:
             ctx._ck(ctx.L.lsdgpu_set_undistorter(ctx.ptr, self.in_w, self.in_h, self.remapX.ctypes.data_as(_fp), self.remapY.ctypes.data_as(_fp)))
+
+
+class UndistorterOpenCV:
+    """Mirror of lsd_slam::UndistorterOpenCV (util/Undistorter.h:164-233) with the calibration file's lines already parsed:
+    in_calib = fx fy cx cy k1 k2 p1 p2, out_mode "crop" or "full".  Host-only (lsdgpu_undistorter_opencv_prepare): map1 (h, w, 2)
+    int16 and map2 (h, w) uint16 are cv::initUndistortRectifyMap(.., CV_16SC2), K_new (float64) cv::getOptimalNewCameraMatrix,
+    K (float32) the matrix getK() hands to SlamSystem.  `status` is 0, or -2 for an invalid calibration (an output mode other
+    than crop / full included); install(ctx) then raises."""
+
+    MODES = {"crop": -1, "full": -2}
+
+    def __init__(self, in_calib, in_size, out_mode, out_size):
+        self.in_w, self.in_h = in_size
+        self.out_w, self.out_h = out_size
+        ic = np.ascontiguousarray(in_calib, np.float32)
+        assert ic.shape == (8,)
+        self.map1 = np.zeros((self.out_h, self.out_w, 2), np.int16)
+        self.map2 = np.zeros((self.out_h, self.out_w), np.uint16)
+        K_new = np.zeros(9, np.float64)
+        K = np.zeros(9, np.float32)
+        self.status = load().lsdgpu_undistorter_opencv_prepare(
+            ic.ctypes.data_as(_fp), self.in_w, self.in_h, self.MODES.get(out_mode, 0), self.out_w, self.out_h,
+            self.map1.ctypes.data_as(C.POINTER(C.c_int16)), self.map2.ctypes.data_as(C.POINTER(C.c_uint16)),
+            K_new.ctypes.data_as(_dp), K.ctypes.data_as(_fp))
+        self.K_new = K_new.reshape(3, 3)
+        self.K = K.reshape(3, 3)
+
+    def getK(self) -> np.ndarray:
+        return self.K
+
+    def install(self, ctx: "Context"):
+        if self.status != 0:
+            raise LsdGpuError("UndistorterOpenCV: invalid calibration")
+        assert (ctx.w, ctx.h) == (self.out_w, self.out_h)
+        ctx._ck(ctx.L.lsdgpu_set_undistorter_opencv(ctx.ptr, self.in_w, self.in_h, self.map1.ctypes.data_as(C.POINTER(C.c_int16)),
+                                                    self.map2.ctypes.data_as(C.POINTER(C.c_uint16))))
 
 
 def default_track_settings(main_tracker: bool = True) -> TrackSettings:
@@ -434,14 +473,14 @@ class Context:
         return bool(f.value)
 
     def undistort(self, raw_u8: np.ndarray) -> np.ndarray:
-        """UndistorterPTAM::undistort (Undistorter.cpp:355-411) through the installed tables"""
+        """UndistorterPTAM::undistort (Undistorter.cpp:355-411) or UndistorterOpenCV::undistort (:564-567), whichever is installed"""
         raw = np.ascontiguousarray(raw_u8, np.uint8)
         out = np.zeros((self.h, self.w), np.uint8)
         self._ck(self.L.lsdgpu_undistort_u8(self.ptr, raw.ctypes.data_as(C.POINTER(C.c_uint8)), out.ctypes.data_as(C.POINTER(C.c_uint8))))
         return out
 
     def upload_distorted(self, fid: int, raw_u8: np.ndarray):
-        """undistort + Frame construction fused (one H2D copy of the raw image, remap feeds the pyramid kernel)"""
+        """undistort (either model) + Frame construction fused (one H2D copy of the raw image, remap feeds the pyramid kernel)"""
         raw = np.ascontiguousarray(raw_u8, np.uint8)
         self._ck(self.L.lsdgpu_frame_upload_distorted_u8(self.ptr, fid, raw.ctypes.data_as(C.POINTER(C.c_uint8))))
 

@@ -172,6 +172,8 @@ extern "C" void lsdgpu_destroy(lsdgpu_ctx* ctx)
     if (ctx->stageRing) cudaFree(ctx->stageRing);
     if (ctx->dRemapX) cudaFree(ctx->dRemapX);
     if (ctx->dRemapY) cudaFree(ctx->dRemapY);
+    if (ctx->dCvMap1) cudaFree(ctx->dCvMap1);
+    if (ctx->dCvMap2) cudaFree(ctx->dCvMap2);
     if (ctx->dRaw) cudaFree(ctx->dRaw);
     if (ctx->hRaw) cudaFreeHost(ctx->hRaw);
     cudaFreeHost(ctx->hEvOut); cudaFreeHost(ctx->hStage[0]); cudaFreeHost(ctx->hStage[1]); cudaFreeHost(ctx->hStageF);

@@ -1,5 +1,10 @@
 // frames.cu -- frame slots of the C ABI (include/lsdgpu.h): upload, the device prefetch ring, release, download, pose / counter
-// setters and getters, depth import, and the input undistorter (UndistorterPTAM) in front of the frame construction.
+// setters and getters, depth import, and the input undistorters (UndistorterPTAM, UndistorterOpenCV) in front of the frame construction.
+#include <algorithm>
+#include <cfloat>
+#include <climits>
+#include <cmath>
+
 #include "internal.cuh"
 #include "frame.cuh"
 
@@ -26,7 +31,7 @@ static FrameSlot* acquireSlot(lsdgpu_ctx* ctx, int id)
     return nullptr;
 }
 
-static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, bool remap = false);
+static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int src = PYR_U8);
 
 extern "C" int lsdgpu_frame_upload_u8(lsdgpu_ctx* ctx, int frame_id, const uint8_t* gray)
 { LSD_LOCK(ctx);
@@ -79,13 +84,16 @@ extern "C" int lsdgpu_frame_from_stage(lsdgpu_ctx* ctx, int frame_id, int index)
     return buildFrameFromDeviceU8(ctx, s, ctx->stageRing + (size_t)index * ctx->w * ctx->h);
 }
 
-static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, bool remap)
+static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int src)
 {
     const int w = ctx->w, h = ctx->h;
     PyrPtrs pp;
     for (int l = 0; l < LSD_LEVELS; l++) pp.l[l] = s->image[l];
-    if (remap) k_image_pyramid<true><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pp, w, h, ctx->dRemapX, ctx->dRemapY, ctx->rawW, nullptr);
-    else k_image_pyramid<false><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pp, w, h);
+    if (src == PYR_PTAM) k_image_pyramid<PYR_PTAM><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pp, w, h, ctx->dRemapX, ctx->dRemapY, ctx->rawW, nullptr);
+    else if (src == PYR_OPENCV)
+        k_image_pyramid<PYR_OPENCV><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pp, w, h, nullptr, nullptr, ctx->rawW, nullptr,
+                                                                                   ctx->dCvMap1, ctx->dCvMap2, ctx->rawH);
+    else k_image_pyramid<PYR_U8><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pp, w, h);
     LAUNCH(ctx);
     GradPtrs gp;
     for (int l = 0; l < LSD_LEVELS; l++) { gp.img[l] = s->image[l]; gp.grad[l] = s->grad[l]; gp.w[l] = w >> l; gp.h[l] = h >> l; }
@@ -333,17 +341,25 @@ extern "C" int lsdgpu_undistorter_validate_tables(int in_width, int in_height, i
     return 0;
 }
 
+// frees the tables of whichever model is installed and the raw staging (the stream must be idle)
+static void releaseUndistorter(lsdgpu_ctx* ctx)
+{
+    if (ctx->dRemapX) { cudaFree(ctx->dRemapX); ctx->dRemapX = nullptr; }
+    if (ctx->dRemapY) { cudaFree(ctx->dRemapY); ctx->dRemapY = nullptr; }
+    if (ctx->dCvMap1) { cudaFree(ctx->dCvMap1); ctx->dCvMap1 = nullptr; }
+    if (ctx->dCvMap2) { cudaFree(ctx->dCvMap2); ctx->dCvMap2 = nullptr; }
+    if (ctx->dRaw) { cudaFree(ctx->dRaw); ctx->dRaw = nullptr; }
+    if (ctx->hRaw) { cudaFreeHost(ctx->hRaw); ctx->hRaw = nullptr; }
+    ctx->undistorterSet = false;
+}
+
 extern "C" int lsdgpu_set_undistorter(lsdgpu_ctx* ctx, int in_width, int in_height, const float* remapX, const float* remapY)
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     if (in_width <= 0 || in_height <= 0) return lsd_fail(ctx, "bad input size");
     const size_t n = (size_t)ctx->w * ctx->h, nr = (size_t)in_width * in_height;
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-    if (ctx->dRemapX) { cudaFree(ctx->dRemapX); ctx->dRemapX = nullptr; }
-    if (ctx->dRemapY) { cudaFree(ctx->dRemapY); ctx->dRemapY = nullptr; }
-    if (ctx->dRaw) { cudaFree(ctx->dRaw); ctx->dRaw = nullptr; }
-    if (ctx->hRaw) { cudaFreeHost(ctx->hRaw); ctx->hRaw = nullptr; }
-    ctx->undistorterSet = false;
+    releaseUndistorter(ctx);
     if (!remapX || !remapY) {
         if (in_width != ctx->w || in_height != ctx->h) return lsd_fail(ctx, "pass-through undistorter needs input size == context size");
     } else {
@@ -382,12 +398,15 @@ extern "C" int lsdgpu_undistort_u8(lsdgpu_ctx* ctx, const uint8_t* raw, uint8_t*
     int r = uploadRaw(ctx, raw);
     if (r) return r;
     const int n = ctx->w * ctx->h;
-    if (!ctx->dRemapX) {                                              // result = image, Undistorter.cpp:370-375
+    if (!ctx->dRemapX && !ctx->dCvMap1) {                             // result = image, Undistorter.cpp:370-375
         LSD_CHECK(ctx, cudaMemcpyAsync(out, ctx->dRaw, n, cudaMemcpyDeviceToHost, ctx->stream));
     } else {
         uint8_t* dOut = ctx->dStageU8[ctx->stageIdx];
         LSD_CHECK(ctx, cudaEventSynchronize(ctx->stageDone[ctx->stageIdx]));
-        k_undistort<<<divUp(n, 256), 256, 0, ctx->stream>>>(ctx->dRaw, ctx->rawW, ctx->dRemapX, ctx->dRemapY, n, dOut);
+        if (ctx->dCvMap1)
+            k_undistort_opencv<<<divUp(n, 256), 256, 0, ctx->stream>>>(ctx->dRaw, ctx->rawW, ctx->rawH, ctx->dCvMap1, ctx->dCvMap2, n, dOut);
+        else
+            k_undistort<<<divUp(n, 256), 256, 0, ctx->stream>>>(ctx->dRaw, ctx->rawW, ctx->dRemapX, ctx->dRemapY, n, dOut);
         LAUNCH(ctx);
         LSD_CHECK(ctx, cudaGetLastError());
         LSD_CHECK(ctx, cudaMemcpyAsync(out, dOut, n, cudaMemcpyDeviceToHost, ctx->stream));
@@ -403,5 +422,139 @@ extern "C" int lsdgpu_frame_upload_distorted_u8(lsdgpu_ctx* ctx, int frame_id, c
     if (!s) return lsd_fail(ctx, "no free frame slot (release frames or raise max_frames)");
     int r = uploadRaw(ctx, raw);
     if (r) return r;
-    return buildFrameFromDeviceU8(ctx, s, ctx->dRaw, ctx->dRemapX != nullptr);
+    return buildFrameFromDeviceU8(ctx, s, ctx->dRaw, ctx->dCvMap1 ? PYR_OPENCV : ctx->dRemapX ? PYR_PTAM : PYR_U8);
+}
+
+// ------------------------------------------------------------------------------------------------------
+// input staging: UndistorterOpenCV
+// ------------------------------------------------------------------------------------------------------
+// The constructor UndistorterOpenCV::UndistorterOpenCV (util/Undistorter.cpp:449-558) after parsing: cv::getOptimalNewCameraMatrix
+// and cv::initUndistortRectifyMap(.., CV_16SC2) restated as OpenCV 4.13 computes them for the 4-coefficient model (no rotation,
+// no tilt, no rational / thin-prism terms: the zero terms of OpenCV's general expressions are left out, which changes no bit
+// of finite results).  All arithmetic is double, in OpenCV's order of operations.
+namespace {
+// cvRound / saturate_cast<int>(double): round half to even; out of range (and NaN) gives INT_MIN as cvtsd2si does
+int cvRoundD(double v)
+{
+    return (v > -2147483648.5 && v < 2147483647.5) ? (int)std::nearbyint(v) : INT_MIN;
+}
+short saturateShort(int v) { return (short)(v < -32768 ? -32768 : v > 32767 ? 32767 : v); }
+}
+
+extern "C" int lsdgpu_undistorter_opencv_prepare(const float input_calibration[8], int iw, int ih, int output_mode, int ow, int oh,
+                                                 int16_t* map1, uint16_t* map2, double K_new[9], float K_out[9])
+{
+    if (!input_calibration || iw <= 0 || ih <= 0 || ow <= 0 || oh <= 0) return -2;
+    if (output_mode != -1 && output_mode != -2) return -2;         // "none" and explicit output parameters: valid = false (:493-502)
+    float ic[8];
+    for (int i = 0; i < 8; i++) ic[i] = input_calibration[i];
+    if (ic[2] < 1.0f) {                                             // relative units (:519-534), in float as written
+        ic[0] *= iw; ic[2] *= iw;
+        ic[1] *= ih; ic[3] *= ih;
+    }
+    // originalK_ (CV_64F from the floats) and distCoeffs (CV_32F 4x1, converted to double by OpenCV)
+    const double fx = ic[0], fy = ic[1], cx = ic[2], cy = ic[3];
+    const double k1 = ic[4], k2 = ic[5], p1 = ic[6], p2 = ic[7];
+    const double alpha = output_mode == -2 ? 1 : 0;
+
+    // getOptimalNewCameraMatrix(K, D, in_size, alpha, out_size, nullptr, false): undistortPoints of a 9x9 grid over the input image
+    // (fixed 5 iterations, with the icdist < 0 fallback of OpenCV 4.x), inscribed and circumscribed rectangles, alpha blend.  With
+    // strong distortion the grid folds (interior points land outside the border); 4.13 then still frames the border.
+    const int N = 9;
+    const double ifx = 1. / fx, ify = 1. / fy;
+    double iX0 = -FLT_MAX, iX1 = FLT_MAX, iY0 = -FLT_MAX, iY1 = FLT_MAX;
+    double oX0 = FLT_MAX, oX1 = -FLT_MAX, oY0 = FLT_MAX, oY1 = -FLT_MAX;
+    for (int gy = 0; gy < N; gy++)
+        for (int gx = 0; gx < N; gx++) {
+            const double u = (double)gx * (iw - 1) / (N - 1), v = (double)gy * (ih - 1) / (N - 1);
+            double x = (u - cx) * ifx, y = (v - cy) * ify;
+            const double x0 = x, y0 = y;
+            for (int j = 0; j < 5; j++) {
+                const double r2 = x * x + y * y;
+                const double icdist = 1 / (1 + (k2 * r2 + k1) * r2);
+                if (icdist < 0) {
+                    x = (u - cx) * ifx;
+                    y = (v - cy) * ify;
+                    break;
+                }
+                const double deltaX = 2 * p1 * x * y + p2 * (r2 + 2 * x * x);
+                const double deltaY = p1 * (r2 + 2 * y * y) + 2 * p2 * x * y;
+                x = (x0 - deltaX) * icdist;
+                y = (y0 - deltaY) * icdist;
+            }
+            if (gx == 0 || gx == N - 1 || gy == 0 || gy == N - 1) {   // 4.13: the circumscribed rectangle bounds the border points only
+                oX0 = std::min(oX0, x); oX1 = std::max(oX1, x);
+                oY0 = std::min(oY0, y); oY1 = std::max(oY1, y);
+            }
+            if (gx == 0) iX0 = std::max(iX0, x);
+            if (gx == N - 1) iX1 = std::min(iX1, x);
+            if (gy == 0) iY0 = std::max(iY0, y);
+            if (gy == N - 1) iY1 = std::min(iY1, y);
+        }
+    const double fx0 = (ow - 1) / (iX1 - iX0), fy0 = (oh - 1) / (iY1 - iY0), cx0 = -fx0 * iX0, cy0 = -fy0 * iY0;
+    const double fx1 = (ow - 1) / (oX1 - oX0), fy1 = (oh - 1) / (oY1 - oY0), cx1 = -fx1 * oX0, cy1 = -fy1 * oY0;
+    double M[9] = { fx0 * (1 - alpha) + fx1 * alpha, 0, cx0 * (1 - alpha) + cx1 * alpha,
+                    0, fy0 * (1 - alpha) + fy1 * alpha, cy0 * (1 - alpha) + cy1 * alpha,
+                    0, 0, 1 };
+    if (K_new) for (int i = 0; i < 9; i++) K_new[i] = M[i];
+    if (K_out) {                                                    // K_ = K_new transposed (:557), read back by main_on_images.cpp:164-167
+        for (int i = 0; i < 9; i++) K_out[i] = 0.f;
+        K_out[0] = (float)M[0]; K_out[2] = (float)M[2];
+        K_out[4] = (float)M[4]; K_out[5] = (float)M[5];
+        K_out[8] = 1.f;
+    }
+    if (!map1 || !map2) return 0;
+
+    // initUndistortRectifyMap(K, D, I, K_new, out_size, CV_16SC2): iR = K_new^-1 by cv::invert's 3x3 DECOMP_LU branch (cofactors
+    // times 1 / det3), then per pixel the normalised ray, the distortion, the projection and 5-bit fixed point
+    const double det = M[0] * (M[4] * M[8] - M[5] * M[7]) - M[1] * (M[3] * M[8] - M[5] * M[6]) + M[2] * (M[3] * M[7] - M[4] * M[6]);
+    if (det == 0) return -2;
+    const double d = 1. / det;
+    const double ir[9] = { (M[4] * M[8] - M[5] * M[7]) * d, (M[2] * M[7] - M[1] * M[8]) * d, (M[1] * M[5] - M[2] * M[4]) * d,
+                           (M[5] * M[6] - M[3] * M[8]) * d, (M[0] * M[8] - M[2] * M[6]) * d, (M[2] * M[3] - M[0] * M[5]) * d,
+                           (M[3] * M[7] - M[4] * M[6]) * d, (M[1] * M[6] - M[0] * M[7]) * d, (M[0] * M[4] - M[1] * M[3]) * d };
+    // The row walk is OpenCV's AVX2 one: the ray (X, Y, W) advances by 8 * ir[0..] per block of 8 pixels and is offset by k * ir[0..]
+    // inside a block; a scalar tail (out_width % 8 pixels) advances pixel by pixel.  The walk only changes the last bits of the
+    // ray, which reach the maps where a pixel projects ~1e7 px or more outside the image (a folded "full" view), never elsewhere.
+    auto pixel = [&](int i, int j, double X, double Y, double W) {
+        const double w = 1. / W, x = X * w, y = Y * w;
+        const double x2 = x * x, y2 = y * y;
+        const double r2 = x2 + y2, _2xy = 2 * x * y;
+        const double kr = 1 + (k2 * r2 + k1) * r2;
+        const double xd = x * kr + p1 * _2xy + p2 * (r2 + 2 * x2);
+        const double yd = y * kr + p1 * (r2 + 2 * y2) + p2 * _2xy;
+        const double u = fx * xd + cx, v = fy * yd + cy;
+        const int iu = cvRoundD(u * 32.0), iv = cvRoundD(v * 32.0);
+        const size_t o = (size_t)i * ow + j;
+        map1[2 * o] = saturateShort(iu >> 5);
+        map1[2 * o + 1] = saturateShort(iv >> 5);
+        map2[o] = (uint16_t)((iv & 31) * 32 + (iu & 31));
+    };
+    for (int i = 0; i < oh; i++) {
+        double _x = i * ir[1] + ir[2], _y = i * ir[4] + ir[5], _w = i * ir[7] + ir[8];
+        int j = 0;
+        for (; j <= ow - 8; j += 8, _x += 8 * ir[0], _y += 8 * ir[3], _w += 8 * ir[6])
+            for (int k = 0; k < 8; k++) pixel(i, j + k, _x + k * ir[0], _y + k * ir[3], _w + k * ir[6]);
+        for (; j < ow; j++, _x += ir[0], _y += ir[3], _w += ir[6]) pixel(i, j, _x, _y, _w);
+    }
+    return 0;
+}
+
+extern "C" int lsdgpu_set_undistorter_opencv(lsdgpu_ctx* ctx, int in_width, int in_height, const int16_t* map1, const uint16_t* map2)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    if (in_width <= 0 || in_height <= 0) return lsd_fail(ctx, "bad input size");
+    if (!map1 || !map2) return lsd_fail(ctx, "UndistorterOpenCV needs both maps");
+    const size_t n = (size_t)ctx->w * ctx->h, nr = (size_t)in_width * in_height;
+    LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+    releaseUndistorter(ctx);
+    LSD_CHECK(ctx, cudaMalloc((void**)&ctx->dCvMap1, n * sizeof(short2)));
+    LSD_CHECK(ctx, cudaMalloc((void**)&ctx->dCvMap2, n * sizeof(uint16_t)));
+    LSD_CHECK(ctx, cudaMemcpy(ctx->dCvMap1, map1, n * sizeof(short2), cudaMemcpyHostToDevice));
+    LSD_CHECK(ctx, cudaMemcpy(ctx->dCvMap2, map2, n * sizeof(uint16_t), cudaMemcpyHostToDevice));
+    LSD_CHECK(ctx, cudaMalloc((void**)&ctx->dRaw, nr));
+    LSD_CHECK(ctx, cudaHostAlloc((void**)&ctx->hRaw, nr, cudaHostAllocDefault));
+    ctx->rawW = in_width; ctx->rawH = in_height;
+    ctx->undistorterSet = true;
+    return 0;
 }

@@ -146,6 +146,8 @@ struct lsdgpu_ctx {
     void* dSim3Outs = nullptr;
     float* dRemapX = nullptr;            // UndistorterPTAM remap tables (separate allocation), raw-image staging
     float* dRemapY = nullptr;
+    short2* dCvMap1 = nullptr;           // UndistorterOpenCV remap maps (CV_16SC2 integer part, CV_16UC1 fractions), separate allocations
+    uint16_t* dCvMap2 = nullptr;
     uint8_t* dRaw = nullptr;
     uint8_t* hRaw = nullptr;
     int rawW = 0, rawH = 0;

@@ -4,6 +4,7 @@
 // Prints one line per tracked frame: "<id> qx qy qz qw tx ty tz good".
 #include <cstdio>
 #include <cstdlib>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -13,7 +14,11 @@ using namespace lsd_slam;
 
 int main(int argc, char** argv)
 {
-    if (argc < 2) { std::fprintf(stderr, "usage: host_demo <frames.bin> [kf_every] | host_demo --undistorter <calib.cfg> <tables.bin>\n"); return 2; }
+    if (argc < 2) {
+        std::fprintf(stderr, "usage: host_demo <frames.bin> [kf_every] | host_demo --undistorter <calib.cfg> <tables.bin>"
+                             " | host_demo --undistorter-any <calib.cfg> <tables.bin>\n");
+        return 2;
+    }
     if (std::string(argv[1]) == "--undistorter" && argc >= 4) {
         // host-only (no GPU needed): parse a PTAM/ATAN calibration file as util/Undistorter.cpp:100-166 does, print K and the
         // sizes, dump the remap tables for the parity test
@@ -29,6 +34,29 @@ int main(int argc, char** argv)
             std::fwrite(u.remapTableY().data(), 4, u.remapTableY().size(), o);
             std::fclose(o);
         }
+        return 0;
+    }
+    if (std::string(argv[1]) == "--undistorter-any" && argc >= 4) {
+        // host-only: getUndistorterForFile (util/Undistorter.cpp:38-88) picks the model from the first line; prints
+        // "<valid> <model: 0 PTAM, 1 OpenCV> in_w in_h out_w out_h", then K, and dumps the tables (PTAM: remapX, remapY floats;
+        // OpenCV: map1 int16 pairs, map2 uint16).  An unreadable or invalid file prints "0".
+        std::unique_ptr<Undistorter> u(getUndistorterForFile(argv[2]));
+        if (!u) { std::printf("0\n"); return 0; }
+        const auto* cv = dynamic_cast<const UndistorterOpenCV*>(u.get());
+        std::printf("1 %d %d %d %d %d\n", cv ? 1 : 0, u->getInputWidth(), u->getInputHeight(), u->getOutputWidth(), u->getOutputHeight());
+        for (int i = 0; i < 9; i++) std::printf("%.9g ", u->getK().m[i]);
+        std::printf("\n");
+        FILE* o = std::fopen(argv[3], "wb");
+        if (!o) return 2;
+        if (cv) {
+            std::fwrite(cv->map1().data(), 2, cv->map1().size(), o);
+            std::fwrite(cv->map2().data(), 2, cv->map2().size(), o);
+        } else {
+            const auto* p = static_cast<const UndistorterPTAM*>(u.get());
+            std::fwrite(p->remapTableX().data(), 4, p->remapTableX().size(), o);
+            std::fwrite(p->remapTableY().data(), 4, p->remapTableY().size(), o);
+        }
+        std::fclose(o);
         return 0;
     }
     const int kfEvery = argc > 2 ? std::atoi(argv[2]) : 0;

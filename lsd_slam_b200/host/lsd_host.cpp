@@ -286,6 +286,58 @@ void UndistorterPTAM::undistort(DeviceContext& dev, const unsigned char* image, 
     dev.check(lsdgpu_undistort_u8(dev.raw(), image, result), "UndistorterPTAM::undistort");
 }
 
+UndistorterOpenCV::UndistorterOpenCV(const char* configFileName)
+{   // parsing as Undistorter.cpp:449-513; the tables are lsdgpu_undistorter_opencv_prepare (:515-558)
+    for (int i = 0; i < 9; i++) K_.m[i] = 0.f;
+    for (float& v : inputCalibration) v = 0.f;
+    std::ifstream infile(configFileName);
+    if (!infile.good()) return;
+    std::string l1, l2, l3, l4;
+    std::getline(infile, l1); std::getline(infile, l2); std::getline(infile, l3); std::getline(infile, l4);
+    float* ic = inputCalibration;
+    valid = std::sscanf(l1.c_str(), "%f %f %f %f %f %f %f %f", &ic[0], &ic[1], &ic[2], &ic[3], &ic[4], &ic[5], &ic[6], &ic[7]) == 8
+            && std::sscanf(l2.c_str(), "%d %d", &in_width, &in_height) == 2;
+    int mode = 0;                                                      // "none" / anything else: not rectifying (:493-502)
+    if (l3 == "crop") mode = -1;
+    else if (l3 == "full") mode = -2;
+    if (std::sscanf(l4.c_str(), "%d %d", &out_width, &out_height) != 2) valid = false;
+    if (!valid || mode == 0 || out_width <= 0 || out_height <= 0) { valid = false; return; }
+    map1_.resize((size_t)2 * out_width * out_height);
+    map2_.resize((size_t)out_width * out_height);
+    double K_new[9];
+    valid = lsdgpu_undistorter_opencv_prepare(ic, in_width, in_height, mode, out_width, out_height, map1_.data(), map2_.data(),
+                                              K_new, K_.m) == 0;
+}
+
+void UndistorterOpenCV::install(DeviceContext& dev) const
+{
+    if (!valid) throw LsdGpuError("UndistorterOpenCV: invalid calibration");
+    if (dev.width() != out_width || dev.height() != out_height) throw LsdGpuError("UndistorterOpenCV: output size differs from the device context");
+    dev.check(lsdgpu_set_undistorter_opencv(dev.raw(), in_width, in_height, map1_.data(), map2_.data()), "UndistorterOpenCV::install");
+}
+
+void UndistorterOpenCV::undistort(DeviceContext& dev, const unsigned char* image, unsigned char* result) const
+{
+    dev.check(lsdgpu_undistort_u8(dev.raw(), image, result), "UndistorterOpenCV::undistort");
+}
+
+Undistorter* getUndistorterForFile(const char* configFilename)
+{   // Undistorter.cpp:38-88 (the search for the file in the working directory and the prints left out)
+    std::ifstream f(configFilename);
+    if (!f.good()) return nullptr;
+    std::string l1;
+    std::getline(f, l1);
+    f.close();
+    float ic[8];
+    Undistorter* u;
+    if (std::sscanf(l1.c_str(), "%f %f %f %f %f %f %f %f", &ic[0], &ic[1], &ic[2], &ic[3], &ic[4], &ic[5], &ic[6], &ic[7]) == 8)
+        u = new UndistorterOpenCV(configFilename);
+    else
+        u = new UndistorterPTAM(configFilename);
+    if (!u->isValid()) { delete u; return nullptr; }
+    return u;
+}
+
 DepthMap::DepthMap(DeviceContext& dev, int w, int h, const Matrix3f&) : dev_(dev), width_(w), height_(h)
 {
     if (w != dev.width() || h != dev.height()) throw LsdGpuError("DepthMap: size differs from the device context");

@@ -190,10 +190,30 @@ private:
     int width_, height_;
 };
 
+// util/Undistorter.h:31-90: what the two camera models have in common.  Both undistort on the device of a DeviceContext.
+class Undistorter {
+public:
+    virtual ~Undistorter() = default;
+    // undistort a raw 8-bit image (in_width x in_height) on the device of `dev`, whose size must be the output size
+    virtual void undistort(DeviceContext& dev, const unsigned char* image, unsigned char* result) const = 0;
+    // install the tables so that Frame(dev, id, w, h, K, ts, rawImage, /*distorted=*/true) feeds raw images to the device
+    virtual void install(DeviceContext& dev) const = 0;
+    virtual const Matrix3f& getK() const = 0;
+    virtual int getOutputWidth() const = 0;
+    virtual int getOutputHeight() const = 0;
+    virtual int getInputWidth() const = 0;
+    virtual int getInputHeight() const = 0;
+    virtual bool isValid() const = 0;
+};
+
+// Undistorter::getUndistorterForFile, util/Undistorter.cpp:38-88: 8 numbers on the first line select UndistorterOpenCV, anything
+// else UndistorterPTAM; nullptr when the file cannot be read or the undistorter is invalid.  The caller owns the result.
+Undistorter* getUndistorterForFile(const char* configFilename);
+
 // util/Undistorter.h:96-160 (SURVEY 8f row 3).  The ATAN/PTAM calibration file has four lines:
 //   fx fy cx cy dist   |   in_width in_height   |   "crop" / "full" / "none" / fx fy cx cy 0   |   out_width out_height
-// An OpenCV-model file (8 numbers on the first line, Undistorter.cpp:70-79) is rejected: that model stays on the host.
-class UndistorterPTAM {
+// An OpenCV-model file (8 numbers on the first line, Undistorter.cpp:70-79) is rejected here: UndistorterOpenCV reads it.
+class UndistorterPTAM : public Undistorter {
 public:
     explicit UndistorterPTAM(const char* configFileName);
     // undistort a raw 8-bit image (in_width x in_height) on the device of `dev`, whose size must be the output size
@@ -216,6 +236,34 @@ private:
     int out_width = 0, out_height = 0, in_width = 0, in_height = 0;
     std::vector<float> remapX, remapY;
     bool valid = false, passThrough = false;
+};
+
+// util/Undistorter.h:164-239.  The OpenCV (radial-tangential) calibration file has four lines:
+//   fx fy cx cy k1 k2 p1 p2   |   in_width in_height   |   "crop" / "full"   |   out_width out_height
+// ("none" or explicit output parameters make it invalid, Undistorter.cpp:493-502).  The tables are built on the host without
+// OpenCV (lsdgpu_undistorter_opencv_prepare, bit-identical to OpenCV 4.13's); the remap runs on the device.
+class UndistorterOpenCV : public Undistorter {
+public:
+    explicit UndistorterOpenCV(const char* configFileName);
+    void undistort(DeviceContext& dev, const unsigned char* image, unsigned char* result) const override;
+    void install(DeviceContext& dev) const override;
+    const Matrix3f& getK() const override { return K_; }
+    int getOutputWidth() const override { return out_width; }
+    int getOutputHeight() const override { return out_height; }
+    int getInputWidth() const override { return in_width; }
+    int getInputHeight() const override { return in_height; }
+    bool isValid() const override { return valid; }
+    // cv::initUndistortRectifyMap(.., CV_16SC2): (x, y) int16 pairs and the uint16 fractions, out_width*out_height each
+    const std::vector<int16_t>& map1() const { return map1_; }
+    const std::vector<uint16_t>& map2() const { return map2_; }
+
+private:
+    Matrix3f K_;
+    float inputCalibration[8];
+    int out_width = 0, out_height = 0, in_width = 0, in_height = 0;
+    std::vector<int16_t> map1_;
+    std::vector<uint16_t> map2_;
+    bool valid = false;
 };
 
 // DepthEstimation/DepthMap.h
