@@ -357,6 +357,12 @@ class Context:
             setattr(g, k, v)
         self._ck(self.L.lsdgpu_set_globals(self.ptr, C.byref(g)))
 
+    def get_globals(self) -> dict:
+        """the run-time settings the context's next calls use (lsdgpu_get_globals), by field name"""
+        g = Globals()
+        self._ck(self.L.lsdgpu_get_globals(self.ptr, C.byref(g)))
+        return {name: getattr(g, name) for name, _ in Globals._fields_}
+
     def synchronize(self):
         self._ck(self.L.lsdgpu_synchronize(self.ptr))
 

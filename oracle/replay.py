@@ -62,13 +62,15 @@ def map_report(a, b):
     return rep
 
 
-def replay_step(seq, snap: Snapshot, fid: int, image_u8, gs, settings=None):
-    """Replay on the oracle the step GpuStream `gs` has JUST executed for frame `fid` from state `snap`.
-    Returns a dict with the pose error, counter equality and the map comparison."""
+def replay_step(seq, snap: Snapshot, fid: int, image_u8, gs, settings=None, globals_kw=None):
+    """Replay on the oracle the step GpuStream `gs` has JUST executed for frame `fid` from state `snap`, under the run-time settings
+    of util/settings.cpp:80-88 the context holds (or `globals_kw` instead, e.g. to show that other values give another result).
+    Returns a dict with the pose error, counter equality and the map comparison; "globals" is the settings the oracle used."""
     from lsd_slam_b200 import abi
     ctx = gs.ctx
     fl = False
-    po.set_globals(fl)
+    g = ctx.get_globals() if globals_kw is None else dict(globals_kw)
+    po.set_globals(fl, **g)
     L = po.lib(fl)
     st = settings or po.default_track_settings(fl)
     # keyframe + depth map in the device's pre-step state
@@ -87,18 +89,18 @@ def replay_step(seq, snap: Snapshot, fid: int, image_u8, gs, settings=None):
 
     # the reference's OWN summation noise on this step: the same tracking with every sum accumulated exactly (diagnostic twin of
     # the oracle, lsdo_globals.exactTrackingSums) -- what the sequential fp32 sums of SE3Tracker.cpp approximate
-    po.set_globals(fl, exactTrackingSums=1)
+    po.set_globals(fl, exactTrackingSums=1, **g)
     xkf, _xdm = make_kf()
     xf = po.Frame(fid, image_u8, seq.K, fast=fl)
     pose_x = np.array(po.se3_track(xkf, xf, snap.last_pose, st).frameToRef_qt, np.float64)
-    po.set_globals(fl)
+    po.set_globals(fl, **g)
     okf, odm = make_kf()
     of = po.Frame(fid, image_u8, seq.K, fast=fl)
     r = po.se3_track(okf, of, snap.last_pose, st)
     res = gs.tracker.last
     pose_g = np.array(res.frameToRef_qt, np.float64)
     pose_o = np.array(r.frameToRef_qt, np.float64)
-    out = {"frame": fid, "kf_change": snap.kf_change}
+    out = {"frame": fid, "kf_change": snap.kf_change, "globals": g}
     out["pose_rel"], out["rot_rad"] = pose_err(pose_g, pose_o)
     out["ref_noise_rel"], out["ref_noise_rot"] = pose_err(pose_o, pose_x)      # reference (fp32 sequential sums) vs exact sums
     out["pose_rel_exact"], _ = pose_err(pose_g, pose_x)                        # device vs exact sums
@@ -159,17 +161,22 @@ def finish_replay(seq, snap: Snapshot, out, gs, mask_before_clear=None, rescale_
     return out
 
 
-def run_with_replay(seq, frames, n_frames, kf_every=20, sample=None, mode=1, device=0, max_frames=8):
+def run_with_replay(seq, frames, n_frames, kf_every=20, sample=None, mode=1, device=0, max_frames=8, globals_kw=None,
+                    before_step=None):
     """GpuStream over frames 1..n_frames-1 with the oracle replaying the steps in `sample` (None = every step).
-    Returns the list of per-step reports.  The stream itself never sees the oracle (it continues from ITS OWN state)."""
+    Returns the list of per-step reports.  The stream itself never sees the oracle (it continues from ITS OWN state).
+    globals_kw: the context's run-time settings (default: the reference's); before_step(k, ctx) runs before step k, e.g. to change
+    them between two frames as a dynamic-reconfigure callback does.  The oracle is back at the default settings afterwards."""
     from lsd_slam_b200 import abi
     from lsd_slam_b200.stream import GpuStream
     images = {k: frames[k][0] for k in range(n_frames)}
-    ctx = abi.Context(seq.w, seq.h, seq.K, device=device, max_frames=max_frames)
+    ctx = abi.Context(seq.w, seq.h, seq.K, device=device, max_frames=max_frames, **(globals_kw or {}))
     gs = GpuStream(ctx, mode=mode, kf_every=kf_every, fused_call=False)
     gs.init_gt(0, frames[0][0], frames[0][1])
     reports = []
     for k in range(1, n_frames):
+        if before_step is not None:
+            before_step(k, ctx)
         if sample is not None and k not in sample:
             gs.step(k, frames[k][0])
             continue
@@ -190,4 +197,5 @@ def run_with_replay(seq, frames, n_frames, kf_every=20, sample=None, mode=1, dev
         out = finish_replay(seq, snap, out, gs, mask_before_clear=mask_holder.get("mask"))
         reports.append(out)
     ctx.close()
+    po.set_globals(False)
     return reports

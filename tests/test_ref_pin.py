@@ -11,6 +11,7 @@ The reference side of every comparison is recorded in tests/golden/ref_pin_320x2
 which runs the same functions below on the reference-compiled library): bit-exact observations as SHA-256 digests of their
 bytes, the others as values.  The tests run the C restatement and check each observation against the record, so they need
 neither the reference sources nor oracle/_ref."""
+import contextlib
 import ctypes as C
 import hashlib
 import os
@@ -74,6 +75,25 @@ class Pin:
 
 _gold = None
 
+# the run-time settings of util/settings.cpp:80-88 the cases run under, on both flavours; empty = the reference's defaults.
+# tests/test_ref_pin_globals.py runs cases under others (the ranges of cfg/LSDParams.cfg:13-34).
+_SETTINGS: dict = {}
+
+
+def set_globals(fl, **kw):
+    return po.set_globals(fl, **_SETTINGS, **kw)
+
+
+@contextlib.contextmanager
+def settings(**g):
+    """run cases under the run-time settings `g` (each unset one at its default)"""
+    global _SETTINGS
+    old, _SETTINGS = _SETTINGS, dict(g)
+    try:
+        yield
+    finally:
+        _SETTINGS = old
+
 
 def _check(case):
     global _gold
@@ -87,7 +107,7 @@ class Side:
 
     def __init__(self, seq, frames, fl, init="gt"):
         self.seq, self.frames, self.fl = seq, frames, fl
-        po.set_globals(fl)
+        set_globals(fl)
         img0, d0 = frames[0]
         self.kf = po.Frame(0, img0, seq.K, fast=fl)
         self.dm = po.DepthMap(seq.w, seq.h, seq.K, fast=fl)
@@ -115,6 +135,7 @@ def _gt_qts(seq, k):
 # ---- the comparisons: each runs one flavour and hands its observations to `pin` -----------------------------------------
 def frame_builders(pin, fl, seq, frames):
     """Frame.cpp:35-54, 491-630, 643-680, 690-767, 245-293, 775-877"""
+    set_globals(fl)
     img, d0 = frames[0]
     a = po.Frame(0, img, seq.K, fast=fl)
     a.setDepthFromGroundTruth(d0)
@@ -269,7 +290,7 @@ def create_keyframe_and_finalize(pin, fl, seq, frames_in):
 def se3_single_evaluation(pin, fl, seq, frames):
     """calcResidualAndBuffers + calcWeightsAndResidual + calculateWarpUpdate (SE3Tracker.cpp:885-1029, 749-790,
     1258-1299, LGSX.h:184-402), the reference's private members called directly"""
-    po.set_globals(fl)
+    set_globals(fl)
     kf = po.Frame(0, frames[0][0], seq.K, fast=fl)
     kf.setDepthFromGroundTruth(frames[0][1])
     f = po.Frame(3, frames[3][0], seq.K, fast=fl)
@@ -297,7 +318,7 @@ def se3_single_evaluation(pin, fl, seq, frames):
 
 def _se3_track_sequence(pin, fl, seq, frames, exact):
     """SE3Tracker::trackFrame over a tracked + mapped sequence: pose, every reported statistic, the good-mask"""
-    po.set_globals(fl, useSSE=1) if fl is True else po.set_globals(fl)
+    set_globals(fl, useSSE=1) if fl is True else set_globals(fl)
     kf = po.Frame(0, frames[0][0], seq.K, fast=fl)
     kf.setDepthFromGroundTruth(frames[0][1])
     dm = po.DepthMap(seq.w, seq.h, seq.K, fast=fl)
@@ -348,6 +369,7 @@ def bench_loop_with_keyframe_changes(pin, fl, seq, frames):
     """the loop bench.py and the full-size GPU tests run (oracle/cpu_stream.py: track, map, forced finalizeKeyFrame +
     createKeyFrame every 10 frames): every pose equal as doubles, final map identical"""
     from oracle.cpu_stream import CpuStream
+    set_globals(fl)
     cs = CpuStream(seq, fl, kf_every=10)
     cs.init_gt(0, *frames[0])
     for k in range(1, 26):
