@@ -245,6 +245,25 @@ void lsdo_depthmap_propagateDepth(lsdo_depthmap* d, lsdo_frame* new_kf);
 void lsdo_ref_prepareForStereoWith(lsdo_frame* frame, lsdo_frame* kf, const double thisToOther_qts[8], const float K[9], float out[30]);
 /* per-stage EMA timers of the reference (DepthMap.cpp:1126-1162), ms of the last call */
 void lsdo_depthmap_last_timings(const lsdo_depthmap* d, float out_ms[8]);
+/* diagnostic branch counters of doLineStereo and propagateDepth, summed over every depth map of the process (C restatement only:
+ * they show which branches a test reaches; no float is read or written by them) */
+enum {
+    LSDO_BR_DEPTH_X,          /* x-dominant depth formula, DepthMap.cpp:1876-1886 */
+    LSDO_BR_DEPTH_Y,          /* y-dominant depth formula, :1887-1898 */
+    LSDO_BR_FIRSTX_GATE,      /* first/last sample point outside the image, :1463-1469 */
+    LSDO_BR_RESCALE_GATE,     /* rescaleFactor outside (0.7, 1.4), :1470 */
+    LSDO_BR_NEAR_CLAMP,       /* pClose behind the near plane, max_idepth clamped, :1491-1495 */
+    LSDO_BR_EPL_CROP,         /* eplLength > MAX_EPL_LENGTH_CROP, :1520-1524 */
+    LSDO_BR_CLIP_LEFT, LSDO_BR_CLIP_RIGHT, LSDO_BR_CLIP_TOP, LSDO_BR_CLIP_BOTTOM,     /* pClose clipped at a border, :1567-1592 */
+    LSDO_BR_SUBPIXEL_PRE, LSDO_BR_SUBPIXEL_POST, LSDO_BR_SUBPIXEL_NONE,             /* subpixel refinement outcome, :1768-1845 */
+    LSDO_BR_PROP_SKIP,        /* propagateDepth: occluded source skipped, :592-593 */
+    LSDO_BR_PROP_INVALIDATE,  /* propagateDepth: target replaced by a nearer source, :600 */
+    LSDO_BR_PROP_MERGE,       /* propagateDepth: source merged into a consistent target, :619-631 */
+    LSDO_BR_PROP_MERGE_CAP,   /* propagateDepth: merged validity capped, :626-627 */
+    LSDO_BR_COUNT
+};
+void lsdo_depth_branch_counts(int64_t out[LSDO_BR_COUNT]);
+void lsdo_depth_branch_counts_reset(void);
 
 #ifdef __cplusplus
 }

@@ -202,6 +202,9 @@ def lib(fast=False):
     sig("lsdo_depthmap_propagateDepth", None, vp, vp)
     sig("lsdo_depthmap_last_timings", None, vp, fp)
     sig("lsdo_ref_prepareForStereoWith", None, vp, vp, dp, fp, fp)
+    if not isinstance(fast, str):            # diagnostic counters of the C restatement only
+        sig("lsdo_depth_branch_counts", None, C.POINTER(C.c_int64))
+        sig("lsdo_depth_branch_counts_reset", None)
     _libs[name] = L
     return L
 
@@ -221,6 +224,23 @@ def default_track_settings(fast=False, main_tracker: bool = True) -> TrackSettin
         for lvl in range(4, LEVELS):
             s.maxItsPerLvl[lvl] = 0
     return s
+
+
+# the diagnostic branch counters of the C restatement's depth map, in the order of lsd_oracle.h's LSDO_BR_* enum
+BRANCHES = ("depth_x", "depth_y", "firstx_gate", "rescale_gate", "near_clamp", "epl_crop",
+            "clip_left", "clip_right", "clip_top", "clip_bottom", "subpixel_pre", "subpixel_post", "subpixel_none",
+            "prop_skip", "prop_invalidate", "prop_merge", "prop_merge_cap")
+
+
+def branch_counts(fast=False) -> dict:
+    """how often each branch of doLineStereo and propagateDepth ran since the last reset, over every depth map of the process"""
+    out = np.zeros(len(BRANCHES), np.int64)
+    lib(fast).lsdo_depth_branch_counts(out.ctypes.data_as(C.POINTER(C.c_int64)))
+    return dict(zip(BRANCHES, out.tolist()))
+
+
+def branch_counts_reset(fast=False) -> None:
+    lib(fast).lsdo_depth_branch_counts_reset()
 
 
 def set_globals(fast=False, **kw) -> Globals:
