@@ -131,9 +131,9 @@ def line_counts(ref_root):
 
 
 def write_ref_pin_and_line_counts(pyoracle, seq, ref_root):
-    from tests import test_ref_pin
+    from tests import pin_cases
     frames = {k: seq.render(k) for k in range(26)}
-    np.savez_compressed(os.path.join(HERE, "ref_pin_320x240.npz"), **test_ref_pin.record(seq, frames))
+    np.savez_compressed(os.path.join(HERE, "ref_pin_320x240.npz"), **pin_cases.record(seq, frames))
     with open(os.path.join(HERE, "reference_line_counts.json"), "w") as f:
         json.dump(line_counts(ref_root), f, indent=0)
         f.write("\n")

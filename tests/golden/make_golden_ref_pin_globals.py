@@ -1,5 +1,5 @@
 """Generates tests/golden/ref_pin_globals_320x240.npz: the reference-compiled side (oracle/_ref/liblsd_ref.so) of every comparison
-of tests/test_ref_pin_globals.py, i.e. the case functions of tests/test_ref_pin.py under non-default run-time settings, on the
+of tests/test_ref_pin_globals.py, i.e. the case functions of tests/pin_cases.py under non-default run-time settings, on the
 seeded 320x240 synthetic stream.  The archive is written with fixed member timestamps and in key order, so that a re-run
 reproduces it byte for byte.
 Run:  python -m tests.golden.make_golden_ref_pin_globals
@@ -35,9 +35,9 @@ if __name__ == "__main__":
     pyoracle.build()
     if not pyoracle.ref_available():
         raise SystemExit("oracle/_ref is not built and the reference sources are absent: this fixture cannot be regenerated here")
-    from tests import test_ref_pin_globals
+    from tests import pin_cases
     seq = synth.Sequence(320, 240, seed=1234)
     frames = {k: seq.render(k) for k in range(26)}
-    res = test_ref_pin_globals.record(seq, frames)
+    res = pin_cases.record_globals(seq, frames)
     save_npz_reproducible(OUT, res)
     print(f"{OUT}: {len(res)} arrays")

@@ -1,5 +1,5 @@
 """Generates tests/golden/ref_pin_motions_320x240.npz: the reference-compiled side (oracle/_ref/liblsd_ref.so) of every comparison
-of tests/test_ref_pin_motions.py, i.e. the case functions of tests/test_ref_pin.py and two constructed cases under the camera
+of tests/test_ref_pin_motions.py, i.e. the case functions of tests/pin_cases.py and two constructed cases under the camera
 motions of tests/motions.py, on the seeded 320x240 synthetic streams.  Written with save_npz_reproducible, so that a re-run
 reproduces it byte for byte.
 Run:  python -m tests.golden.make_golden_ref_pin_motions
@@ -19,7 +19,7 @@ if __name__ == "__main__":
     pyoracle.build()
     if not pyoracle.ref_available():
         raise SystemExit("oracle/_ref is not built and the reference sources are absent: this fixture cannot be regenerated here")
-    from tests import test_ref_pin_motions
-    res = test_ref_pin_motions.record()
+    from tests import pin_cases
+    res = pin_cases.record_motions()
     save_npz_reproducible(OUT, res)
     print(f"{OUT}: {len(res)} arrays")

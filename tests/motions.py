@@ -35,3 +35,14 @@ class Frames:
         if k not in self._cache:
             self._cache[k] = self.seq.render(k)
         return self._cache[k]
+
+
+_streams: dict = {}
+
+
+def stream(motion):
+    """(320x240 sequence, lazily rendered frames) of the motion, shared by every test that reads it"""
+    if motion not in _streams:
+        seq = sequence(motion)
+        _streams[motion] = (seq, Frames(seq))
+    return _streams[motion]

@@ -13,46 +13,12 @@ import pytest
 
 from lsd_slam_b200 import abi, synth
 from lsd_slam_b200.stream import GpuStream
+from tests.util import CLOUD_FILTERS, oracle_cloud, same_cloud
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 GOLDEN = json.load(open(os.path.join(ROOT, "tests", "golden", "cloud_viewer.json")))
-FILTERS = [None, {"minNearSupport": 1}, {"minNearSupport": 9}, {"scaledDepthVarTH": 0.01, "absDepthVarTH": 0.02},
-           {"scaledDepthVarTH": 100.0, "absDepthVarTH": 100.0}]
-
-
-def _level_cam(ctx, level):
-    """Frame::fx(level) etc. as ROSOutput3DWrapper.cpp:85-88 puts them into the message (Frame.cpp:403-459)"""
-    fx, fy, cx, cy = np.float32(ctx.K[0, 0]), np.float32(ctx.K[1, 1]), np.float32(ctx.K[0, 2]), np.float32(ctx.K[1, 2])
-    cx0, cy0 = cx, cy
-    for lv in range(1, level + 1):
-        fx, fy = np.float32(np.float64(fx) * 0.5), np.float32(np.float64(fy) * 0.5)
-        cx = np.float32((np.float64(cx0) + 0.5) / (1 << lv) - 0.5)
-        cy = np.float32((np.float64(cy0) + 0.5) / (1 << lv) - 0.5)
-    return float(fx), float(fy), float(cx), float(cy)
-
-
-def _oracle(ctx, kf_ids, c2w, level, filt, layout):
-    from oracle import cloud
-    cam = _level_cam(ctx, level)
-    outs, counts = [], []
-    for i, kf in enumerate(kf_ids):
-        pc = ctx.pack_pointcloud(kf, level).reshape(ctx.h >> level, ctx.w >> level)
-        vert, ply, total, shown = cloud.keyframe(pc.view(cloud.INPUT_POINT_DENSE), cam, c2w[i], filt)
-        outs.append(vert if layout == abi.CLOUD_VERTEX else ply)
-        counts.append((total, shown))
-    return np.concatenate(outs).view(np.uint32).reshape(-1, 4), np.array(counts, np.int32).reshape(-1, 2)
-
-
-def _same(gpu, ref):
-    """byte-identical, except that NaN equals NaN"""
-    g, r = np.ascontiguousarray(gpu).view(np.uint32).reshape(-1, 4), np.asarray(ref).reshape(-1, 4)
-    assert g.shape == r.shape
-    gn, rn = np.isnan(g.view(np.float32)), np.isnan(r.view(np.float32))
-    assert (gn == rn).all()
-    assert (g[~gn] == r[~rn]).all()
-    return int(gn.sum())
 
 
 _stream_cache = {}
@@ -82,11 +48,11 @@ def test_stream_keyframes_match_oracle(w, h, level, layout):
     gs = _stream(w, h)
     ctx, ids, c2w = gs.ctx, gs.keyframe_ids, gs.keyframe_cam_to_world_f7()
     assert not np.allclose(c2w[-1], c2w[0])
-    for filt in FILTERS:
+    for filt in CLOUD_FILTERS:
         pts, counts = ctx.export_pointcloud(ids, c2w, level=level, filter=filt, layout=layout)
-        ref, ref_counts = _oracle(ctx, ids, c2w, level, filt, layout)
+        ref, ref_counts = oracle_cloud(ctx, ids, c2w, level, filt, layout)
         assert (counts == ref_counts).all(), filt
-        _same(pts, ref)
+        same_cloud(pts, ref)
         if filt is None:
             assert len(pts) > 1000
 
@@ -108,11 +74,11 @@ def test_adversarial_planes_match_oracle():
     n_nan = 0
     for level in (0, 1):
         for layout in (abi.CLOUD_PLY, abi.CLOUD_VERTEX):
-            for filt in FILTERS:
+            for filt in CLOUD_FILTERS:
                 pts, counts = ctx.export_pointcloud(ids, c2ws, level=level, filter=filt, layout=layout)
-                ref, ref_counts = _oracle(ctx, ids, c2ws, level, filt, layout)
+                ref, ref_counts = oracle_cloud(ctx, ids, c2ws, level, filt, layout)
                 assert (counts == ref_counts).all()
-                n_nan += _same(pts, ref)
+                n_nan += same_cloud(pts, ref)
     assert n_nan > 0
     ctx.close()
 

@@ -5,79 +5,14 @@ import numpy as np
 import pytest
 
 from lsd_slam_b200 import abi
-from tests.util import IDENT, hyp_equal_report
+from tests import device_cases as cases
+from tests.util import IDENT, Pair, hyp_equal_report, pose_err, sim3_inverse, sim3_mul, tracked_pair
 
 pytestmark = pytest.mark.gpu
 
 
-class Pair:
-    """The same state on both sides: oracle objects + a GPU context, driven through identical calls."""
-
-    def __init__(self, ctx, oracle, seq, frames, init="gt"):
-        self.ctx, self.o, self.seq, self.frames = ctx, oracle, seq, frames
-        img0, d0 = frames[0]
-        self.okf = oracle.Frame(0, img0, seq.K)
-        self.odm = oracle.DepthMap(seq.w, seq.h, seq.K)
-        self.gdm = abi.DepthMap(ctx)
-        ctx.upload(0, img0)
-        if init == "gt":
-            self.okf.setDepthFromGroundTruth(d0)
-            self.odm.initializeFromGTDepth(self.okf)
-            ctx.set_depth_gt(0, d0)
-            self.gdm.initializeFromGTDepth(0)
-        else:
-            self.odm.initializeRandomly(self.okf)            # glibc rand() on the host (DepthMap.cpp:898)
-            self.gdm.setHypotheses(0, self.odm.current().copy(), reactivated=False, do_set_depth=True)
-        self.oframes = {0: self.okf}
-
-    def add_frame(self, k, pose_qt=None, itr=0.0):
-        """upload frame k on both sides with the SAME pose (ground truth unless given)"""
-        img, _ = self.frames[k]
-        of = self.o.Frame(k, img, self.seq.K)
-        qts = np.concatenate([self.seq.frame_to_ref_qt(k) if pose_qt is None else pose_qt, [1.0]])
-        of.set_thisToParent(qts, self.okf)
-        self.ctx.upload(k, img)
-        self.ctx.set_pose(k, qts, 0, itr)
-        # an untracked oracle frame has initialTrackedResidual == 0: keep itr = 0 on the GPU side too
-        self.oframes[k] = of
-        return of
-
-    def sync_counters(self):
-        t, m = self.o.lib().lsdo_frame_numFramesTrackedOnThis(self.okf.ptr), self.o.lib().lsdo_frame_numMappedOnThis(self.okf.ptr)
-        self.ctx.set_counters(0, t, m)
-
-    def compare(self, exact=True, rtol=1e-3, max_flag_mismatch=0):
-        a, b = self.gdm.current(), self.odm.current()
-        rep = hyp_equal_report(a, b)
-        assert rep["valid_mismatch"] <= max_flag_mismatch, rep
-        assert rep["blacklist_mismatch"] <= max_flag_mismatch, rep
-        assert rep["validity_mismatch"] <= max_flag_mismatch, rep
-        for f in ("idepth", "idepth_var", "idepth_smoothed", "idepth_var_smoothed", "nextStereoFrameMinID"):
-            if exact:
-                assert rep[f + "_bitdiff"] == 0, rep
-            else:
-                assert rep[f + "_maxrel"] <= rtol or rep[f + "_bitdiff"] <= max_flag_mismatch, rep
-        return rep
-
-
-def _tracked_pair(ctx, oracle, seq, frames, ks, init="gt"):
-    """frames tracked BY THE ORACLE; the oracle's pose, residual and good-mask are pushed to the GPU side so that
-    both depth maps see identical inputs"""
-    p = Pair(ctx, oracle, seq, frames, init)
-    last = IDENT
-    for k in ks:
-        img, _ = frames[k]
-        of = oracle.Frame(k, img, seq.K)
-        r = oracle.se3_track(p.okf, of, last)
-        last = np.array(r.frameToRef_qt)
-        p.oframes[k] = of
-        ctx.upload(k, img)
-        ctx.set_pose(k, of.thisToParent(), 0, r.initialTrackedResidual)
-    return p
-
-
 def test_observe_update_bit_exact(gpu_ctx_small, oracle, seq_small, frames_small):
-    p = _tracked_pair(gpu_ctx_small, oracle, seq_small, frames_small, [1, 2])
+    p = tracked_pair(gpu_ctx_small, oracle, seq_small, frames_small, [1, 2])
     p.sync_counters()
     # no good-mask on the GPU side -> drop it on the oracle side too (refPixelWasGoodNoCreate == 0)
     for k in (1, 2):
@@ -123,29 +58,7 @@ def test_random_init_update_sequence_bit_exact(gpu_ctx_small, oracle, seq_small,
 
 
 def test_fill_holes_and_regularize_bit_exact(gpu_ctx_small, oracle, seq_small, frames_small):
-    p = Pair(gpu_ctx_small, oracle, seq_small, frames_small, "random")
-    # punch holes + blacklist some pixels so that all fill-hole branches trigger
-    cur = p.odm.current().copy()
-    rng = np.random.default_rng(3)
-    holes = rng.random(cur.shape) < 0.3
-    cur["isValid"][holes] = 0
-    cur["blacklisted"][rng.random(cur.shape) < 0.05] = -3
-    cur["validity_counter"] = rng.integers(0, 30, cur.shape)
-    p.odm.set_current(cur)
-    p.gdm.setHypotheses(0, cur, do_set_depth=False)
-    p.odm.regularizeFillHoles()
-    p.gdm.regularizeFillHoles()
-    p.compare(exact=True)
-    assert np.array_equal(p.gdm.integral(), _integral(p.gdm.current()))
-    for occl in (False, True):
-        p.odm.regularize(occl, 24)
-        p.gdm.regularize(occl, 24)
-        p.compare(exact=True)
-
-
-def _integral(cur):
-    v = np.where(cur["isValid"] > 0, cur["validity_counter"], 0).astype(np.int64)
-    return v.cumsum(0).cumsum(1).astype(np.int32)
+    cases.fill_holes_and_regularize(gpu_ctx_small, oracle, seq_small, frames_small)
 
 
 def test_integral_buffer_matches_oracle(gpu_ctx_small, oracle, seq_small, frames_small):
@@ -158,69 +71,14 @@ def test_integral_buffer_matches_oracle(gpu_ctx_small, oracle, seq_small, frames
 
 @pytest.mark.parametrize("with_mask", [False, True])
 def test_propagate_and_create_keyframe(gpu_ctx_small, oracle, seq_small, frames_small, with_mask):
-    p = _tracked_pair(gpu_ctx_small, oracle, seq_small, frames_small, [2, 5, 9])
-    for k in (2, 5, 9):
-        oracle.lib().lsdo_frame_set_depthHasBeenUpdatedFlag(p.okf.ptr, 0)
-        gpu_ctx_small.L.lsdgpu_ref_import(gpu_ctx_small.ptr, 0)
-        p.sync_counters()
-        if not with_mask:
-            oracle.lib().lsdo_frame_clear_refPixelWasGood(p.oframes[k].ptr)
-        else:
-            # give the GPU frame the oracle's good mask by tracking it there as well (mask parity is tested
-            # in test_gpu_track); tracking overwrites the pose, so restore the oracle's
-            trk = abi.SE3Tracker(gpu_ctx_small, mode=0)
-            trk.trackFrame(0, k, IDENT if k == 2 else p.oframes[k].thisToParent()[:7])
-            gpu_ctx_small.set_pose(k, p.oframes[k].thisToParent(), 0, oracle.lib().lsdo_frame_initialTrackedResidual(p.oframes[k].ptr))
-            gpu_ctx_small.set_counters(0, *[oracle.lib().lsdo_frame_numFramesTrackedOnThis(p.okf.ptr), oracle.lib().lsdo_frame_numMappedOnThis(p.okf.ptr)])
-        p.odm.updateKeyframe([p.oframes[k]])
-        p.gdm.updateKeyframe([k])
-    if not with_mask:
-        p.compare(exact=True)
-    # propagate only
-    before_o = p.odm.current().copy()
-    p.odm.propagateDepth(p.oframes[9])
-    p.gdm.propagateDepth(9)
-    rep = p.compare(exact=not with_mask, rtol=1e-3, max_flag_mismatch=0 if not with_mask else 40)
-    assert rep["n_valid"] > 5000
-    # restore and run the whole createKeyFrame on both sides
-    p.odm.set_current(before_o)
-    p.gdm.setHypotheses(0, before_o, do_set_depth=False)
-    p.odm.createKeyFrame(p.oframes[9])
-    q = p.gdm.createKeyFrame(9)
-    qo = p.oframes[9].thisToParent()
-    # the rescale factor comes from the reference's sequential fp32 `sumIdepth +=` (DepthMap.cpp:1286-1294): the device reproduces
-    # that sum bit for bit (csrc/seqsum.cuh) whenever it sums the same hypotheses -- without the tracking mask the maps are
-    # identical before the sum, so everything after it is too
-    assert np.allclose(q[:7], qo[:7], atol=1e-12)
-    if not with_mask:
-        assert np.float32(q[7]).tobytes() == np.float32(qo[7]).tobytes()
-        p.compare(exact=True)
-    else:
-        assert abs(q[7] - qo[7]) <= 2e-5 * qo[7]
-        p.compare(exact=False, rtol=2e-5, max_flag_mismatch=40)
-    assert gpu_ctx_small.L.lsdgpu_depth_active_keyframe(gpu_ctx_small.ptr) == 9
-    idg, ido = gpu_ctx_small.download(9, abi.BUF_IDEPTH, 0), p.oframes[9].idepth(0)
-    assert ((idg > 0) != (ido > 0)).sum() <= (0 if not with_mask else 40)
-    both = (idg > 0) & (ido > 0)
-    if not with_mask:
-        assert np.array_equal(idg, ido)
-    assert np.max(np.abs(idg[both] - ido[both]) / ido[both]) <= 2e-5
-
-
-def _sim3(oracle, fn, *args):
-    import ctypes as C
-    dp = C.POINTER(C.c_double)
-    out = np.zeros(8, np.float64)
-    arrs = [np.ascontiguousarray(a, np.float64) for a in args]
-    getattr(oracle.lib(), fn)(*[a.ctypes.data_as(dp) for a in arrs], out.ctypes.data_as(dp))
-    return out
+    cases.propagate_and_create_keyframe(gpu_ctx_small, oracle, seq_small, frames_small, with_mask)
 
 
 def test_update_keyframe_with_frames_tracked_on_the_previous_keyframe(gpu_ctx_small, oracle, seq_small, frames_small):
     """DepthMap.cpp:1085-1099: frames still queued when the keyframe changes were tracked on the OLD keyframe; they are mapped with
     refToKf = activeKeyFrame->getScaledCamToWorld().inverse() * frame->getScaledCamToWorld() and without their tracking mask
     (:245, :322).  The caller passes that product in lsdgpu_ref_desc; every field of every pixel equals the oracle's.
-    (Scene rescaled to mean inverse depth 1 on keyframe 0 -- see test_ref_pin.test_create_keyframe_and_finalize_bit_exact.)"""
+    (Scene rescaled to mean inverse depth 1 on keyframe 0 -- see the pin's create_keyframe_and_finalize.)"""
     d0 = frames_small[0][1]
     sc = float(np.mean(1.0 / d0[d0 > 0]))
     frames = {k: (frames_small[k][0], (frames_small[k][1] * sc).astype(np.float32)) for k in range(13)}
@@ -261,11 +119,8 @@ def test_update_keyframe_with_frames_tracked_on_the_previous_keyframe(gpu_ctx_sm
     # ids only: refused, with a pointer to the descriptor call
     with pytest.raises(abi.LsdGpuError, match="update_keyframe_refs"):
         p.gdm.updateKeyframe([4])
-    c2w9 = of9.thisToParent()                                     # keyframe 0 is the first frame: its camToWorld is the identity
-    items = []
-    for k in (4, 5):
-        c2wk = p.oframes[k].thisToParent()
-        items.append((k, _sim3(oracle, "lsdo_sim3d_mul", _sim3(oracle, "lsdo_sim3d_inverse", c2w9), c2wk)))
+    w2c9 = sim3_inverse(oracle, of9.thisToParent())              # keyframe 0 is the first frame: its camToWorld is the identity
+    items = [(k, sim3_mul(oracle, w2c9, p.oframes[k].thisToParent())) for k in (4, 5)]
     before = p.gdm.current().copy()
     p.odm.updateKeyframe([p.oframes[4], p.oframes[5]])
     p.gdm.updateKeyframe(items)
@@ -299,7 +154,6 @@ def test_finalize_keyframe(gpu_ctx_small, oracle, seq_small, frames_small):
 def test_full_loop_parity(gpu_ctx_small, oracle, seq_small, frames_small):
     """track + map loop run independently on both sides (each side consumes ITS OWN poses): inverse depth
     within 1e-3 relative per pixel, poses within 1e-4 (north_star)."""
-    from tests.util import pose_err
     p = Pair(gpu_ctx_small, oracle, seq_small, frames_small, "gt")
     trk = abi.SE3Tracker(gpu_ctx_small, mode=1)
     last_o = last_g = IDENT

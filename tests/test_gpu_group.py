@@ -7,118 +7,40 @@ import numpy as np
 import pytest
 
 from lsd_slam_b200 import abi, synth
-from lsd_slam_b200.stream import GpuStream, GpuStreamGroup
+from tests.device_cases import run_streams
+from tests.util import assert_same
 
 pytestmark = pytest.mark.gpu
-KF_EVERY = 20
 LOOK_AWAY = np.array([0, 0.7071067811865476, 0, 0.7071067811865476, 0, 0, 0], np.float64)   # 90 deg about y: no point stays in view
-
-_frames_cache = {}
-
-
-def _frames(w, h, s, n):
-    """stream s: its own synthetic sequence (seed 1234 + 1000 s, as scripts/bench_streams.py)"""
-    key = (w, h, s)
-    seq, fr = _frames_cache.get(key, (None, []))
-    if seq is None:
-        seq = synth.Sequence(w, h, seed=1234 + 1000 * s)
-    while len(fr) < n:
-        fr.append(seq.render(len(fr)))
-    _frames_cache[key] = (seq, fr)
-    return seq, fr
-
-
-def _make_streams(w, h, phases, n_frames):
-    streams, frames = [], []
-    for s, ph in enumerate(phases):
-        seq, fr = _frames(w, h, s, n_frames)
-        ctx = abi.Context(w, h, seq.K, max_frames=8)
-        gs = GpuStream(ctx, mode=1, kf_every=KF_EVERY, kf_phase=ph)
-        gs.init_gt(0, fr[0][0], fr[0][1])
-        streams.append(gs)
-        frames.append(fr)
-    return streams, frames
-
-
-def _observe(gs, fid, qts):
-    ctx = gs.ctx
-    pose, parent, itr = ctx.get_pose(fid)
-    return {"result": bytes(gs.tracker.last), "pose": pose.tobytes(), "parent": parent, "itr": np.float32(itr).tobytes(),
-            "new_kf_qts": None if qts is None else np.asarray(qts).tobytes(),
-            "counters": (ctx.get_counters(fid), ctx.get_counters(gs.kf_id)),
-            "mask": ctx.download(fid, abi.BUF_GOODMASK).tobytes(),
-            "depth": gs.map.current().tobytes()}
-
-
-def _run(w, h, phases, n_steps, grouped, before_step=None):
-    """grouped(k): step k is one group call (True) or one single call per stream (False).  before_step(k, streams) may change
-    the streams' state first.  Returns per step and stream what _observe saw, and whether the step diverged."""
-    streams, frames = _make_streams(w, h, phases, n_steps + 1)
-    group = GpuStreamGroup(streams)
-    log = []
-    try:
-        for k in range(1, n_steps + 1):
-            if before_step:
-                before_step(k, streams)
-            kf = [gs.next_is_keyframe_change() for gs in streams]
-            if grouped(k):
-                try:
-                    group.step([k] * len(streams), images=[f[k][0] for f in frames])
-                except RuntimeError:
-                    pass
-                qts = [group._qts[i].copy() if kf[i] else None for i in range(len(streams))]
-            else:
-                qts = []
-                for i, (gs, f) in enumerate(zip(streams, frames)):
-                    try:
-                        gs.step(k, f[k][0])
-                    except RuntimeError:
-                        pass
-                    qts.append(gs._qts.copy() if kf[i] else None)
-            log.append([dict(_observe(gs, k, q), diverged=bool(gs.tracker.diverged), kf=kf[i])
-                        for i, (gs, q) in enumerate(zip(streams, qts))])
-    finally:
-        for gs in streams:
-            gs.ctx.close()
-    return log
-
-
-def _assert_same(a, b):
-    assert len(a) == len(b)
-    for k, (sa, sb) in enumerate(zip(a, b), start=1):
-        for s, (oa, ob) in enumerate(zip(sa, sb)):
-            for key in oa:
-                assert oa[key] == ob[key], f"step {k}, stream {s}: {key} differs"
-
 
 @pytest.mark.parametrize("n", [1, 2, 3, 8])
 def test_group_equals_single_calls_640x480(n):
     """25 frames, one keyframe change per stream, in a different step for every stream: groups mix update and create"""
     phases = [2 * s for s in range(n)]              # keyframe changes at steps 20, 18, 16, ...
-    single = _run(640, 480, phases, 25, lambda k: False)
-    group = _run(640, 480, phases, 25, lambda k: True)
+    single = run_streams(640, 480, phases, 25, lambda k: False)
+    group = run_streams(640, 480, phases, 25, lambda k: True)
     changes = [[k for k, step in enumerate(single, start=1) if step[s]["kf"]] for s in range(n)]
     assert all(len(c) == 1 for c in changes) and len({c[0] for c in changes}) == n
     assert not any(o["diverged"] for step in single for o in step)
-    _assert_same(group, single)
+    assert_same(group, single)
 
 
 def test_group_equals_single_calls_1280x1024_n8():
     """at 1280x1024 a CTA of an 8-stream group stands in for up to 9 virtual CTAs of ~5 level-1 slots per warp each: more
     good-mask flags per thread than one 32-bit word holds"""
     phases = [15 + s % 5 for s in range(8)]         # keyframe changes at steps 5, 4, 3, 2, 1, 5, 4, 3
-    single = _run(1280, 1024, phases, 5, lambda k: False)
-    group = _run(1280, 1024, phases, 5, lambda k: True)
+    single = run_streams(1280, 1024, phases, 5, lambda k: False)
+    group = run_streams(1280, 1024, phases, 5, lambda k: True)
     assert all(sum(step[s]["kf"] for step in single) == 1 for s in range(8))
-    _assert_same(group, single)
+    assert_same(group, single)
 
 
 def test_group_and_single_calls_alternated():
     """group and single calls on the same contexts: the barrier bookkeeping of either launch stays right after the other"""
     phases = [10, 12, 14]                            # keyframe changes at steps 10, 8, 6
-    single = _run(640, 480, phases, 12, lambda k: False)
-    mixed = _run(640, 480, phases, 12, lambda k: k % 2 == 0)
-    _assert_same(mixed, single)
+    single = run_streams(640, 480, phases, 12, lambda k: False)
+    mixed = run_streams(640, 480, phases, 12, lambda k: k % 2 == 0)
+    assert_same(mixed, single)
 
 
 def test_group_divergence_skips_only_that_streams_mapping():
@@ -128,11 +50,11 @@ def test_group_divergence_skips_only_that_streams_mapping():
         if k == 3:
             streams[1].last_pose = LOOK_AWAY.copy()
     phases = [0, 0, 0]
-    single = _run(640, 480, phases, 3, lambda k: False, look_away)
-    group = _run(640, 480, phases, 3, lambda k: True, look_away)
+    single = run_streams(640, 480, phases, 3, lambda k: False, look_away)
+    group = run_streams(640, 480, phases, 3, lambda k: True, look_away)
     assert [o["diverged"] for o in group[2]] == [False, True, False]
     assert group[2][1]["depth"] == group[1][1]["depth"]       # the diverged stream's map did not change
-    _assert_same(group, single)
+    assert_same(group, single)
 
 
 def _ctx(w, h, seed=1234):

@@ -13,7 +13,7 @@ import pytest
 from lsd_slam_b200 import abi, synth
 from lsd_slam_b200.stream import GpuStream, GpuStreamGroup
 from oracle.replay import run_with_replay
-from tests.test_gpu_cloud import _oracle, _same
+from tests.util import assert_step_ok, oracle_cloud, same_cloud
 
 pytestmark = pytest.mark.gpu
 
@@ -75,11 +75,9 @@ def test_one_step_replayed_on_the_oracle():
     flags at a threshold may differ); the exact check of the flags is the group comparison above"""
     seq, frames = _setup()
     (r,) = run_with_replay(seq, frames, 2, kf_every=0, max_frames=4)
-    assert r["pose_rel"] <= 1e-4 + r["ref_noise_rel"], (r["pose_rel"], r["ref_noise_rel"])
-    assert r["rot_rad"] <= 1e-6 + r["ref_noise_rot"], r["rot_rad"]
+    assert_step_ok(r)
     assert r["counts_equal"]
     assert r["mask_mismatch"] <= 1e-3 * (seq.w // 2) * (seq.h // 2), r["mask_mismatch"]
-    assert r["map_ok"], r["map"]
 
 
 def test_level0_cloud_matches_oracle():
@@ -92,9 +90,9 @@ def test_level0_cloud_matches_oracle():
         c2w = np.array([[0.1, -0.2, 0.05, 0.97, 0.3, -0.1, 0.2]], np.float32)
         for layout in (abi.CLOUD_PLY, abi.CLOUD_VERTEX):
             pts, counts = ctx.export_pointcloud([0], c2w, level=0, layout=layout)
-            ref, ref_counts = _oracle(ctx, [0], c2w, 0, None, layout)
+            ref, ref_counts = oracle_cloud(ctx, [0], c2w, 0, None, layout)
             assert (counts == ref_counts).all()
-            _same(pts, ref)
+            same_cloud(pts, ref)
             assert len(pts) > 100000
     finally:
         ctx.close()

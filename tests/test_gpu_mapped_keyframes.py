@@ -15,20 +15,16 @@ import pytest
 
 from lsd_slam_b200 import abi, synth
 from lsd_slam_b200.stream import IDENT, GpuStream, sim3_mul_qts
-from tests.test_gpu_sim3 import POSE_TOL, _check_eval, _check_track, _oracle_track, _sim3_err
-from tests.util import pose_err
+from tests.util import (POSE_TOL, check_perma_overlap, check_perma_track, check_sim3_eval, check_sim3_track, oracle_sim3_track,
+                        se3_inverse, sim3_err, sim3_inverse)
 
 pytestmark = pytest.mark.gpu
 
 KF_EVERY = 5
 N_FRAMES = 16                   # keyframe changes at frames 5, 10 and 15: keyframes 0, 5 and 10 finished, 15 active
 PERMA_FRAME = 12                # a frame that is not a keyframe, for trackFrameOnPermaref
-DT = (0.01, -0.005, 0.004)      # the perturbation of test_gpu_sim3._init
+DT = (0.01, -0.005, 0.004)      # the perturbation of util.sim3_init
 AB = ((1.0, 0.0), (0.97, 1.5))
-
-
-def _d(a):
-    return a.ctypes.data_as(C.POINTER(C.c_double))
 
 
 def _set_depth(oracle, frame, hyp):
@@ -90,20 +86,16 @@ class MappedRun:
 
     def frame_to_ref(self, oracle, ref, fr, perturb=True):
         """the relative Sim3 SlamSystem starts from: reference->getScaledCamToWorld().inverse() * frame->getScaledCamToWorld()
-        (scale ratio of the two keyframes included), with test_gpu_sim3's perturbation of translation and scale"""
+        (scale ratio of the two keyframes included), with util.sim3_init's perturbation of translation and scale"""
         c2w = dict(zip(self.gs.keyframe_ids, self.gs.keyframe_cam_to_world))
-        inv = np.zeros(8)
-        oracle.lib().lsdo_sim3d_inverse(_d(np.ascontiguousarray(c2w[ref])), _d(inv))
-        q = sim3_mul_qts(inv, c2w[fr])
+        q = sim3_mul_qts(sim3_inverse(oracle, c2w[ref]), c2w[fr])
         if perturb:
             q[4:7] += DT
             q[7] *= 1.02
         return q
 
     def ref_to_frame(self, oracle, ref, fr, perturb=True):
-        r2f = np.zeros(8)
-        oracle.lib().lsdo_sim3d_inverse(_d(self.frame_to_ref(oracle, ref, fr, perturb)), _d(r2f))
-        return r2f
+        return sim3_inverse(oracle, self.frame_to_ref(oracle, ref, fr, perturb))
 
     def pairs(self):
         return [(a, b) for a in self.kfs for b in self.kfs if a != b]
@@ -150,7 +142,7 @@ def test_sim3_eval_on_mapped_keyframes(mapped, oracle):
                     got = trk.eval(ref, fr, lvl, r2f, a, b)
                     want = oracle.sim3_eval(of[ref], of[fr], lvl, r2f, a, b)
                     assert want.warpedSize > 10, (ref, fr, lvl)
-                    _check_eval(got, want)
+                    check_sim3_eval(got, want)
                     n_no_depth += want.numTermsD < want.numTermsP      # warped onto frame pixels without depth (sim3.cuh:116-117)
     assert n_no_depth > 0
 
@@ -165,7 +157,7 @@ def test_sim3_eval_settings_on_mapped_keyframes(mapped, oracle):
         r2f = mapped.ref_to_frame(oracle, ref, fr)
         for lvl in (4, 3, 2, 1):
             a, b = AB[lvl % 2]
-            _check_eval(trk.eval(ref, fr, lvl, r2f, a, b), oracle.sim3_eval(mapped.of[ref], mapped.of[fr], lvl, r2f, a, b, settings=st))
+            check_sim3_eval(trk.eval(ref, fr, lvl, r2f, a, b), oracle.sim3_eval(mapped.of[ref], mapped.of[fr], lvl, r2f, a, b, settings=st))
 
 
 def test_track_frame_sim3_on_mapped_keyframes(mapped, oracle):
@@ -175,9 +167,9 @@ def test_track_frame_sim3_on_mapped_keyframes(mapped, oracle):
         init = mapped.frame_to_ref(oracle, ref, fr)
         for lo, hi in ((4, 1), (3, 2)):
             est = trk.trackFrameSim3(ref, fr, init, lo, hi)
-            want, exact = _oracle_track(oracle, mapped.of[ref], mapped.of[fr], init, lo, hi)
-            _check_track(trk.last, want)
-            _check_track(trk.last, exact, res_tol=5e-4)
+            want, exact = oracle_sim3_track(oracle, mapped.of[ref], mapped.of[fr], init, lo, hi)
+            check_sim3_track(trk.last, want)
+            check_sim3_track(trk.last, exact, res_tol=5e-4)
             assert np.array_equal(est, np.array(trk.last.frameToRef_qts))
             n_converged += not want.diverged
     assert n_converged >= len(mapped.pairs())
@@ -191,7 +183,7 @@ def _check_batch(run, oracle):
     for (ref, fr), init, r in zip(pairs, inits, res):
         trk.trackFrameSim3(ref, fr, init, 4, 1)
         assert bytes(trk.last) == bytes(r)
-        _check_track(r, oracle.sim3_track(run.of[ref], run.of[fr], init, 4, 1))
+        check_sim3_track(r, oracle.sim3_track(run.of[ref], run.of[fr], init, 4, 1))
 
 
 def test_track_frame_sim3_batch_on_mapped_keyframes(mapped, oracle):
@@ -218,29 +210,7 @@ def test_cluster_sizes_agree_on_mapped_keyframes(mapped, oracle, monkeypatch):
         out[cs] = trk.last
     for cs in (1, 2, 4):
         assert list(out[cs].numCalcResidualCalls) == list(out[8].numCalcResidualCalls)
-        assert max(_sim3_err(out[cs].frameToRef_qts, out[8].frameToRef_qts)) < POSE_TOL
-
-
-def _overlap_poses(oracle, rng, n):
-    poses = []
-    for _ in range(n):
-        a = rng.normal(0, [0.2, 0.2, 0.3, 0.05, 0.05, 0.05])
-        q = np.zeros(7)
-        oracle.lib().lsdo_se3d_exp(oracle._dp(a), oracle._dp(q))
-        poses.append(q)
-    return poses
-
-
-def _check_overlap(se3, oracle, prs, rng):
-    """test_check_perma_ref_overlap_batch's checks on a batch of perturbed poses over the keyframes of prs"""
-    ids, poses = [], []
-    for k in prs:
-        ids += [k] * 5
-        poses += _overlap_poses(oracle, rng, 5)
-    got = se3.checkPermaRefOverlap(ids, np.array(poses))
-    want = np.array([prs[k].overlap(q) for k, q in zip(ids, poses)], np.float32)
-    assert np.allclose(got, want, rtol=2e-5, atol=1e-6), np.abs(got - want).max()
-    return want
+        assert max(sim3_err(out[cs].frameToRef_qts, out[8].frameToRef_qts)) < POSE_TOL
 
 
 def test_perma_ref_on_mapped_keyframes(mapped, oracle):
@@ -250,7 +220,7 @@ def test_perma_ref_on_mapped_keyframes(mapped, oracle):
     for k in mapped.kfs:
         prs[k] = oracle.PermaRef(mapped.of[k])
         assert se3.setPermaRef(k) == prs[k].n > 30
-    want = _check_overlap(se3, oracle, prs, np.random.default_rng(3))
+    want = check_perma_overlap(se3, oracle, prs, np.random.default_rng(3))
     assert want.min() < 0.9 < want.max()
 
     # trackFrameOnPermaref for a frame that is not a keyframe, from its ground-truth pose (translation in the keyframe's map
@@ -263,25 +233,12 @@ def test_perma_ref_on_mapped_keyframes(mapped, oracle):
     for k in prs:
         gt = seq.frame_to_ref_qt(PERMA_FRAME, ref=k)
         gt[4:7] /= scale[k]
-        gt_inv = np.zeros(7)
-        oracle.lib().lsdo_se3d_inverse(oracle._dp(gt), oracle._dp(gt_inv))
+        gt_inv = se3_inverse(oracle, gt)
         for init in (gt_inv, IDENT):
             ids.append(k)
             inits.append(init)
     res = se3.trackFrameOnPermaref(ids, PERMA_FRAME, np.array(inits))
-    n_good = 0
-    for k, init, g in zip(ids, inits, res):
-        o = prs[k].track(of, init)
-        assert bool(g.diverged) == bool(o.diverged)
-        if o.diverged:
-            continue
-        dt, ang = pose_err(np.array(g.frameToRef_qt), np.array(o.frameToRef_qt))
-        assert dt <= 1e-4 and ang <= 2e-6, (k, dt, ang)
-        assert list(g.numCalcResidualCalls) == list(o.numCalcResidualCalls)
-        assert abs(g.lastResidual - o.lastResidual) <= 1e-3 * abs(o.lastResidual) + 1e-6
-        assert bool(g.trackingWasGood) == bool(o.trackingWasGood)
-        assert abs(g.pointUsage - o.pointUsage) <= 1e-4
-        n_good += int(o.trackingWasGood)
+    n_good = sum(check_perma_track(g, prs[k].track(of, init)) for k, init, g in zip(ids, inits, res))
     assert n_good >= 2
     ctx.release(PERMA_FRAME)
 
@@ -364,7 +321,7 @@ def test_adversarial_map_edges(mapped, oracle):
     se3 = abi.SE3Tracker(ctx)
     pr = oracle.PermaRef(okf)
     assert se3.setPermaRef(kf) == pr.n
-    _check_overlap(se3, oracle, {kf: pr}, np.random.default_rng(5))
+    check_perma_overlap(se3, oracle, {kf: pr}, np.random.default_rng(5))
 
     of = dict(mapped.of)
     of[kf] = okf
@@ -373,11 +330,11 @@ def test_adversarial_map_edges(mapped, oracle):
         r2f = mapped.ref_to_frame(oracle, ref, fr)
         for lvl in range(abi.LEVELS):
             for a, b in AB:
-                _check_eval(trk.eval(ref, fr, lvl, r2f, a, b), oracle.sim3_eval(of[ref], of[fr], lvl, r2f, a, b))
+                check_sim3_eval(trk.eval(ref, fr, lvl, r2f, a, b), oracle.sim3_eval(of[ref], of[fr], lvl, r2f, a, b))
         init = mapped.frame_to_ref(oracle, ref, fr)
         trk.trackFrameSim3(ref, fr, init, 4, 1)
-        want, exact = _oracle_track(oracle, of[ref], of[fr], init)
+        want, exact = oracle_sim3_track(oracle, of[ref], of[fr], init)
         assert trk.diverged == bool(want.diverged)
         if not want.diverged:
-            _check_track(trk.last, want)
-            _check_track(trk.last, exact, res_tol=5e-4)
+            check_sim3_track(trk.last, want)
+            check_sim3_track(trk.last, exact, res_tol=5e-4)

@@ -10,7 +10,7 @@ branches run -- on each motion:
   * propagateDepth and createKeyFrame bit for bit, without a tracking mask and with the device's mask handed to the oracle;
   * the wide-baseline update and the propagation collisions of the pin (forward, backward): bit for bit, the latter also with
     the device's own tracking mask handed to the oracle;
-  * SE3 evaluation on levels 4-1 and trackFrame in modes 0 and 1: the tolerances of test_gpu_track.py;
+  * SE3 evaluation on levels 4-1 and trackFrame in modes 0 and 1: the tolerances of tests/util.py's checks;
   * a replayed closed loop of 20 frames with a keyframe every 8 (oracle/replay.py): the map bit for bit after every step;
   * at 640x480, a closed loop of forward and of roll sampled every 4th step, keyframe changes included."""
 import numpy as np
@@ -18,18 +18,16 @@ import pytest
 
 from lsd_slam_b200 import abi
 from oracle import replay
+from tests import device_cases as cases
 from tests import motions
-from tests import test_gpu_depth as gd
-from tests import test_gpu_globals as gg
-from tests import test_ref_pin_motions as pm
-from tests.test_gpu_depth import Pair
-from tests.util import IDENT
+from tests.pin_cases import ONLY, PROPAGATION_FRAME, WIDE_BASELINE_FRAME
+from tests.util import IDENT, Pair, assert_step_ok, kf_depth_equal, new_depth, se3_inverse, tracked_pair
 
 pytestmark = pytest.mark.gpu
 
 MOTIONS = list(motions.MOTIONS)
-COLLIDE = list(pm.ONLY["propagation_collisions"])
-WIDE = list(pm.ONLY["wide_baseline"])
+COLLIDE = list(ONLY["propagation_collisions"])
+WIDE = list(ONLY["wide_baseline"])
 
 
 @pytest.fixture(params=MOTIONS)
@@ -40,7 +38,7 @@ def motion(request):
 @pytest.fixture()
 def stream(motion):
     """(320x240 sequence, lazily rendered frames) of the motion, shared with the pin"""
-    return pm.stream(motion)
+    return motions.stream(motion)
 
 
 @pytest.fixture()
@@ -54,15 +52,15 @@ def ctx(oracle, stream):
 
 # ---- depth map, bit for bit -------------------------------------------------------------------------------------------------
 def test_observe_from_gt_depth_bit_exact(ctx, oracle, stream):
-    gg.test_observe_from_gt_depth_bit_exact(ctx, oracle, *stream)
+    cases.observe_from_gt(ctx, oracle, *stream)
 
 
 def test_update_keyframe_sequence_bit_exact(ctx, oracle, stream):
-    gg.test_update_keyframe_sequence_bit_exact(ctx, oracle, *stream)
+    cases.update_keyframe_sequence(ctx, oracle, *stream)
 
 
 def test_random_init_observe_and_update_bit_exact(ctx, oracle, stream):
-    gg.test_random_init_observe_and_update_bit_exact(ctx, oracle, *stream)
+    cases.random_init_observe_and_update(ctx, oracle, *stream)
 
 
 def test_fill_holes_and_regularize_on_the_observed_map_bit_exact(ctx, oracle, stream):
@@ -85,17 +83,17 @@ def test_fill_holes_and_regularize_on_the_observed_map_bit_exact(ctx, oracle, st
 
 
 def test_propagate_and_create_keyframe(ctx, oracle, stream):
-    gd.test_propagate_and_create_keyframe(ctx, oracle, *stream, False)
+    cases.propagate_and_create_keyframe(ctx, oracle, *stream, False)
 
 
 def test_propagate_and_create_keyframe_with_tracking_mask_bit_exact(ctx, oracle, stream):
-    """test_gpu_depth.test_propagate_and_create_keyframe with the tracking mask, from identical inputs: each frame is tracked on
+    """device_cases.propagate_and_create_keyframe with the tracking mask, from identical inputs: each frame is tracked on
     the device and its good mask is handed to the oracle, as oracle/replay.py does.  That test's own with-mask variant lets each
     side use its own tracker's mask; the two masks differ on up to 1e-3 of the pixels (test_gpu_track.py), and under the backward
     and roll motions those pixels move the regularised depth of their neighbours after createKeyFrame by up to 1.1e-3, beyond
     the 2e-5 it allows.  With the same mask on both sides every step is bit for bit."""
     seq, frames = stream
-    p = gd._tracked_pair(ctx, oracle, seq, frames, [2, 5, 9])
+    p = tracked_pair(ctx, oracle, seq, frames, [2, 5, 9])
     trk = abi.SE3Tracker(ctx, mode=0)
     for k in (2, 5, 9):
         of = p.oframes[k]
@@ -125,33 +123,33 @@ def test_propagate_and_create_keyframe_with_tracking_mask_bit_exact(ctx, oracle,
 
 
 def test_finalize_create_keyframe_and_refs_bit_exact(ctx, oracle, stream):
-    gg.test_finalize_create_keyframe_and_refs_bit_exact(ctx, oracle, *stream)
+    cases.finalize_create_and_refs(ctx, oracle, *stream)
 
 
 @pytest.mark.parametrize("motion", WIDE)
 def test_wide_baseline_bit_exact(ctx, oracle, stream, motion):
-    """pm.wide_baseline: one update with a frame whose depth ratio to the keyframe leaves doLineStereo's rescale gate"""
+    """the pin's wide_baseline: one update with a frame whose depth ratio to the keyframe leaves doLineStereo's rescale gate"""
     seq, frames = stream
     p = Pair(ctx, oracle, seq, frames, "gt")
-    k = pm.WIDE_BASELINE_FRAME
+    k = WIDE_BASELINE_FRAME
     of = p.add_frame(k)
-    gg._new_depth(p, k)
+    new_depth(p)
     p.odm.updateKeyframe([of])
     p.gdm.updateKeyframe([k])
     assert p.compare(exact=True)["n_valid"] > 10000
-    gg._kf_depth_equal(ctx, p.okf, 0)
+    kf_depth_equal(ctx, p.okf, 0)
 
 
 @pytest.mark.parametrize("motion", COLLIDE)
 @pytest.mark.parametrize("variant", ["no mask", "mask", "validity 200"])
 def test_propagation_collisions_bit_exact(ctx, oracle, stream, motion, variant):
-    """pm.propagation_collisions: a random map propagated along the optical axis, so that sources at inconsistent depths land on
+    """the pin's propagation_collisions: a random map propagated along the optical axis, so that sources at inconsistent depths land on
     one pixel and k_prop_resolve must skip the occluded ones and replace a target by a nearer source in the reference's raster
     order.  "mask": the device's tracking mask of the new keyframe (SE3 evaluation at level 1 near the true pose), handed to the
     oracle, so both sides propagate from identical inputs.  "validity 200": every merge exceeds the validity cap."""
     seq, frames = stream
     p = Pair(ctx, oracle, seq, frames, "random")
-    k = pm.PROPAGATION_FRAME
+    k = PROPAGATION_FRAME
     if variant == "validity 200":
         cur = p.odm.current().copy()
         cur["validity_counter"][cur["isValid"] != 0] = 200
@@ -159,8 +157,7 @@ def test_propagation_collisions_bit_exact(ctx, oracle, stream, motion, variant):
         p.gdm.setHypotheses(0, cur, do_set_depth=False)
     of = p.add_frame(k)
     if variant == "mask":
-        inv = np.zeros(7)
-        oracle.lib().lsdo_se3d_inverse(gg._d(seq.frame_to_ref_qt(k)), gg._d(inv))
+        inv = se3_inverse(oracle, seq.frame_to_ref_qt(k))
         abi.SE3Tracker(ctx).eval(0, k, 1, inv.astype(np.float32), write_mask=True)
         mask = ctx.download(k, abi.BUF_GOODMASK)
         assert 0.05 < mask.mean() < 0.98
@@ -174,13 +171,13 @@ def test_propagation_collisions_bit_exact(ctx, oracle, stream, motion, variant):
 
 # ---- trackers ---------------------------------------------------------------------------------------------------------------
 def test_se3_eval_each_level(ctx, oracle, stream):
-    gg.test_se3_eval_each_level(ctx, oracle, *stream)
+    cases.se3_eval_each_level(ctx, oracle, *stream, sum_noise=True)
 
 
 @pytest.mark.parametrize("mode", [0, 1])
 @pytest.mark.parametrize("k", [3, 8])
 def test_se3_track(ctx, oracle, stream, mode, k):
-    gg.test_se3_track(ctx, oracle, *stream, mode, k)
+    cases.se3_track(ctx, oracle, *stream, mode, k)
 
 
 # ---- closed loops -----------------------------------------------------------------------------------------------------------
@@ -190,7 +187,7 @@ def test_closed_loop_replay(oracle, stream):
     reps = replay.run_with_replay(seq, frames, 20, kf_every=8)
     assert len(reps) == 19 and [r["frame"] for r in reps if r["kf_change"]] == [8, 16]
     for r in reps:
-        gg._assert_step_ok(r)
+        assert_step_ok(r)
 
 
 @pytest.mark.parametrize("motion", ["forward", "roll"])
@@ -200,4 +197,4 @@ def test_closed_loop_replay_640(oracle, motion):
     reps = replay.run_with_replay(seq, motions.Frames(seq), 20, kf_every=8, sample=set(range(4, 20, 4)))
     assert [r["frame"] for r in reps] == [4, 8, 12, 16] and [r["frame"] for r in reps if r["kf_change"]] == [8, 16]
     for r in reps:
-        gg._assert_step_ok(r)
+        assert_step_ok(r)

@@ -5,8 +5,7 @@ import numpy as np
 import pytest
 
 from lsd_slam_b200 import abi
-from tests.test_gpu_depth import Pair
-from tests.util import hyp_equal_report
+from tests.util import Pair, hyp_equal_report
 
 pytestmark = pytest.mark.gpu
 

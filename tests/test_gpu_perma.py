@@ -4,7 +4,8 @@ import numpy as np
 import pytest
 
 from lsd_slam_b200 import abi, synth
-from tests.util import IDENT, pose_err
+from tests import device_cases as cases
+from tests.util import IDENT, check_perma_overlap
 
 pytestmark = pytest.mark.gpu
 
@@ -12,72 +13,26 @@ pytestmark = pytest.mark.gpu
 def _setup(oracle, w=640, h=480, kf_ids=(0, 6, 12)):
     seq = synth.Sequence(w, h, seed=1234)
     ctx = abi.Context(w, h, seq.K, max_frames=8)
-    trk = abi.SE3Tracker(ctx)
-    okfs, prs = {}, {}
-    for k in kf_ids:
-        img, d = seq.render(k)
-        ctx.upload(k, img)
-        ctx.set_depth_gt(k, d)
-        okf = oracle.Frame(k, img, seq.K)
-        okf.setDepthFromGroundTruth(d)
-        okfs[k] = okf
-        prs[k] = oracle.PermaRef(okf)
-        assert trk.setPermaRef(k) == prs[k].n > 200
-    return seq, ctx, trk, okfs, prs
+    trk, prs = cases.perma_setup(ctx, oracle, seq, kf_ids, 200)
+    return seq, ctx, trk, prs
 
 
 def test_check_perma_ref_overlap_batch(oracle):
-    seq, ctx, trk, okfs, prs = _setup(oracle)
-    rng = np.random.default_rng(3)
-    ids, poses = [], []
-    for k in prs:
-        for _ in range(5):
-            a = rng.normal(0, [0.2, 0.2, 0.3, 0.05, 0.05, 0.05])
-            q = np.zeros(7)
-            oracle.lib().lsdo_se3d_exp(oracle._dp(a), oracle._dp(q))
-            ids.append(k)
-            poses.append(q)
-    got = trk.checkPermaRefOverlap(ids, np.array(poses))
-    want = np.array([prs[k].overlap(q) for k, q in zip(ids, poses)], np.float32)
-    assert np.allclose(got, want, rtol=2e-5, atol=1e-6), np.abs(got - want).max()
+    seq, ctx, trk, prs = _setup(oracle)
+    want = check_perma_overlap(trk, oracle, prs, np.random.default_rng(3))
     assert want.min() < 0.9 < want.max()             # the candidates really differ
     ctx.close()
 
 
 def test_track_frame_on_permaref_batch(oracle):
-    seq, ctx, trk, okfs, prs = _setup(oracle)
-    img, _ = seq.render(9)
-    ctx.upload(9, img)
-    of = oracle.Frame(9, img, seq.K)
-    ids, inits = [], []
-    for k in prs:                                     # ground-truth relative pose, identity, and a perturbed start
-        gt = seq.frame_to_ref_qt(9, ref=k)
-        gt_inv = np.zeros(7)
-        oracle.lib().lsdo_se3d_inverse(oracle._dp(gt), oracle._dp(gt_inv))
-        for init in (gt_inv, IDENT):
-            ids.append(k)
-            inits.append(init)
-    res = trk.trackFrameOnPermaref(ids, 9, np.array(inits))
-    n_good = 0
-    for k, init, g in zip(ids, inits, res):
-        o = prs[k].track(of, init)
-        assert bool(g.diverged) == bool(o.diverged)
-        if o.diverged:
-            continue
-        dt, ang = pose_err(np.array(g.frameToRef_qt), np.array(o.frameToRef_qt))
-        assert dt <= 1e-4 and ang <= 2e-6, (k, dt, ang)
-        assert list(g.numCalcResidualCalls) == list(o.numCalcResidualCalls)
-        assert abs(g.lastResidual - o.lastResidual) <= 1e-3 * abs(o.lastResidual) + 1e-6
-        assert bool(g.trackingWasGood) == bool(o.trackingWasGood)
-        assert abs(g.pointUsage - o.pointUsage) <= 1e-4
-        n_good += int(o.trackingWasGood)
-    assert n_good >= 3
+    seq, ctx, trk, prs = _setup(oracle)
+    assert cases.perma_batch(ctx, oracle, seq, trk, prs, 9) >= 3
     ctx.close()
 
 
 def test_perma_batch_of_many_candidates_is_consistent(oracle):
     """256 copies of the same candidate in one launch give 256 identical results (no cross-CTA state)"""
-    seq, ctx, trk, okfs, prs = _setup(oracle, kf_ids=(0,))
+    seq, ctx, trk, prs = _setup(oracle, kf_ids=(0,))
     img, _ = seq.render(4)
     ctx.upload(4, img)
     res = trk.trackFrameOnPermaref([0] * 256, 4, np.tile(IDENT, (256, 1)))

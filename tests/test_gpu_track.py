@@ -6,52 +6,23 @@ import numpy as np
 import pytest
 
 from lsd_slam_b200 import abi
-from tests.util import IDENT, pose_err, rot_angle
+from tests import device_cases as cases
+from tests.device_cases import se3_setup
+from tests.util import IDENT, check_se3_eval, pose_err, se3_inverse
 
 pytestmark = pytest.mark.gpu
-
-EVAL_RTOL = 2e-4
-
-
-def _setup(ctx, oracle, seq, frames, k):
-    img0, d0 = frames[0]
-    ctx.upload(0, img0)
-    ctx.set_depth_gt(0, d0)
-    okf = oracle.Frame(0, img0, seq.K)
-    okf.setDepthFromGroundTruth(d0)
-    imgk, _ = frames[k]
-    ctx.upload(k, imgk)
-    of = oracle.Frame(k, imgk, seq.K)
-    return okf, of
-
-
-def _cmp_eval(g, o):
-    A_g, A_o = np.array(g.A).reshape(6, 6), np.array(o.A).reshape(6, 6)
-    scale = np.sqrt(np.outer(np.diag(A_o), np.diag(A_o)))
-    assert np.abs(A_g - A_o).max() / 1.0 <= EVAL_RTOL * scale.max()
-    assert np.all(np.abs(A_g - A_o) <= EVAL_RTOL * scale + 1e-12)
-    b_g, b_o = np.array(g.b), np.array(o.b)
-    assert np.all(np.abs(b_g - b_o) <= EVAL_RTOL * np.sqrt(np.diag(A_o)) * np.sqrt(max(o.lsError, 1e-12)) + 1e-9)
-    assert g.warpedSize == o.warpedSize
-    assert g.goodCount == o.goodCount and g.badCount == o.badCount
-    for f in ("lsError", "meanWeightedRes", "meanUnweightedRes", "pointUsage", "affine_a_lastIt", "sxx", "syy", "sx", "sy", "sw"):
-        assert abs(getattr(g, f) - getattr(o, f)) <= EVAL_RTOL * abs(getattr(o, f)) + 1e-7, f
-    assert abs(g.affine_b_lastIt - o.affine_b_lastIt) <= 5e-3
-    assert abs(g.meanRes - o.meanRes) <= 1e-4 + EVAL_RTOL * abs(o.meanRes)
 
 
 @pytest.mark.parametrize("level", [4, 3, 2, 1])
 def test_single_evaluation_parity(gpu_ctx_small, oracle, seq_small, frames_small, level):
-    okf, of = _setup(gpu_ctx_small, oracle, seq_small, frames_small, 3)
+    okf, of = se3_setup(gpu_ctx_small, oracle, seq_small, frames_small, 3)
     trk = abi.SE3Tracker(gpu_ctx_small)
     # identity and a pose near the truth
-    gt = seq_small.frame_to_ref_qt(3)
-    inv = np.zeros(7)
-    oracle.lib().lsdo_se3d_inverse(oracle._dp(gt), oracle._dp(inv))
+    inv = se3_inverse(oracle, seq_small.frame_to_ref_qt(3))
     for pose, a, b in ((IDENT.astype(np.float32), 1.0, 0.0), (inv.astype(np.float32), 0.98, 1.5)):
         g = trk.eval(0, 3, level, pose, a, b, write_mask=True)
         o = oracle.se3_eval(okf, of, level, pose, a, b, write_mask=True)
-        _cmp_eval(g, o)
+        check_se3_eval(g, o)
         if level == 1:
             mg = gpu_ctx_small.download(3, abi.BUF_GOODMASK)
             mo = of.refPixelWasGood()
@@ -61,25 +32,7 @@ def test_single_evaluation_parity(gpu_ctx_small, oracle, seq_small, frames_small
 @pytest.mark.parametrize("mode", [0, 1])
 @pytest.mark.parametrize("k", [1, 3, 8])
 def test_track_frame_pose_parity(gpu_ctx_small, oracle, seq_small, frames_small, mode, k):
-    okf, of = _setup(gpu_ctx_small, oracle, seq_small, frames_small, k)
-    trk = abi.SE3Tracker(gpu_ctx_small, mode=mode)
-    pose_g = trk.trackFrame(0, k, IDENT)
-    r = oracle.se3_track(okf, of, IDENT)
-    pose_o = np.array(r.frameToRef_qt)
-    dt, ang = pose_err(pose_g, pose_o)
-    assert dt <= 1e-4, (dt, pose_g, pose_o)
-    assert ang <= 1e-4 * max(rot_angle(pose_o), 1e-2) + 1e-7, ang
-    assert trk.trackingWasGood == bool(r.trackingWasGood) and trk.diverged == bool(r.diverged)
-    assert abs(trk.lastResidual - r.lastResidual) <= 1e-3 * abs(r.lastResidual) + 1e-6
-    assert abs(trk.pointUsage - r.pointUsage) <= 1e-4
-    assert abs(trk.lastGoodCount - r.lastGoodCount) <= 2 and abs(trk.lastBadCount - r.lastBadCount) <= 2
-    assert list(trk.last.numCalcResidualCalls) == list(r.numCalcResidualCalls)
-    assert list(trk.last.numCalcWarpUpdateCalls) == list(r.numCalcWarpUpdateCalls)
-    q, pid, itr = gpu_ctx_small.get_pose(k)
-    assert pid == 0 and abs(itr - r.initialTrackedResidual) <= 1e-3 * abs(r.initialTrackedResidual) + 1e-6
-    assert gpu_ctx_small.get_counters(0)[0] == 1          # numFramesTrackedOnThis++ (SE3Tracker.cpp:480)
-    mg = gpu_ctx_small.download(k, abi.BUF_GOODMASK)
-    assert (mg != of.refPixelWasGood()).mean() < 1e-3
+    cases.se3_track(gpu_ctx_small, oracle, seq_small, frames_small, mode, k)
 
 
 @pytest.mark.parametrize("mode", [0, 1])
@@ -87,7 +40,7 @@ def test_affine_lighting_off_and_zero_motion(seq_small, frames_small, oracle, mo
     oracle.set_globals(useAffineLightningEstimation=0)      # the ROS default (cfg/LSDParams.cfg:28)
     try:
         ctx = abi.Context(seq_small.w, seq_small.h, seq_small.K, max_frames=4, useAffineLightningEstimation=0)
-        okf, of = _setup(ctx, oracle, seq_small, frames_small, 2)
+        okf, of = se3_setup(ctx, oracle, seq_small, frames_small, 2)
         trk = abi.SE3Tracker(ctx, mode=mode)
         pg = trk.trackFrame(0, 2, IDENT)
         r = oracle.se3_track(okf, of, IDENT)
@@ -105,7 +58,7 @@ def test_affine_lighting_off_and_zero_motion(seq_small, frames_small, oracle, mo
 @pytest.mark.parametrize("mode", [0, 1])
 def test_divergence_returns_identity(gpu_ctx_small, oracle, seq_small, frames_small, mode):
     """an initial estimate that looks away from the scene: < 1% of the points warp inside (SE3Tracker.cpp:324-329)"""
-    okf, of = _setup(gpu_ctx_small, oracle, seq_small, frames_small, 1)
+    okf, of = se3_setup(gpu_ctx_small, oracle, seq_small, frames_small, 1)
     far = np.array([0, 0.7071067811865476, 0, 0.7071067811865476, 0, 0, 0], np.float64)     # 90 deg about y
     trk = abi.SE3Tracker(gpu_ctx_small, mode=mode)
     p = trk.trackFrame(0, 1, far)
@@ -117,7 +70,7 @@ def test_divergence_returns_identity(gpu_ctx_small, oracle, seq_small, frames_sm
 def test_tracker_modes_and_parity_hook_interleave_on_one_context(gpu_ctx_small, oracle, seq_small, frames_small):
     """mode-1 track, single evaluation (parity hook), mode-0 track, mode-1 track again on ONE context: the persistent kernel's
     monotonic barrier counter and the evaluation kernel's last-block counter must not share a word (each would break the other)"""
-    okf, of = _setup(gpu_ctx_small, oracle, seq_small, frames_small, 3)
+    okf, of = se3_setup(gpu_ctx_small, oracle, seq_small, frames_small, 3)
     r = oracle.se3_track(okf, of, IDENT)
     pose_o = np.array(r.frameToRef_qt)
     ctx = gpu_ctx_small
@@ -126,7 +79,7 @@ def test_tracker_modes_and_parity_hook_interleave_on_one_context(gpu_ctx_small, 
     poses, counts = [], []
     for step in ("m1", "eval", "m0", "eval", "m1", "m1", "m0"):
         if step == "eval":
-            _cmp_eval(t1.eval(0, 3, 2, IDENT.astype(np.float32), 1.0, 0.0), o_ev)
+            check_se3_eval(t1.eval(0, 3, 2, IDENT.astype(np.float32), 1.0, 0.0), o_ev)
             continue
         trk = t1 if step == "m1" else t0
         poses.append(trk.trackFrame(0, 3, IDENT))

@@ -2,85 +2,37 @@
 
 A user changes the six globals of util/settings.cpp:80-88 between frames with ROS dynamic reconfigure
 (cfg/LSDParams.cfg:13-34, IOWrapper/ROS/rosReconfigure.h:81-91).  tests/test_ref_pin.py holds the C restatement to the
-reference-compiled library at the defaults only; this module runs the same case functions under each setting below, one at a
-time, and under one combined ROS-like set, and checks every observation against tests/golden/ref_pin_globals_320x240.npz
+reference-compiled library at the defaults only; this module runs the same case functions under each setting of
+tests/pin_cases.SETS, one at a time, and under one combined ROS-like set, and checks every observation against tests/golden/ref_pin_globals_320x240.npz
 (recorded from oracle/_ref/liblsd_ref.so by python -m tests.golden.make_golden_ref_pin_globals).  Each set runs only the cases
 that read its setting: the depth-map cases for the mapping settings, the SE3 cases for the tracking ones, the track + map loop
 for all of them.
 
 Non-vacuity: every set changes at least one recorded observation against the default record, and the two minUseGrad values
 are thresholds some pixels of frame 0 sit exactly on, so `<` and `<=` give different point sets there."""
-import os
-
 import numpy as np
 import pytest
 
 from oracle import pyoracle as po
-from tests import test_ref_pin as pin
+from tests import pin_cases as pin
 
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_pin_globals_320x240.npz")
-
-DEPTH = ("depthmap_update_sequence", "depthmap_random_init_every_branch", "depthmap_individual_passes",
-         "create_keyframe_and_finalize")
-TRACK = ("se3_single_evaluation", "se3_track_scalar")
-LOOP = ("bench_loop_with_keyframe_changes",)
-
-# set name -> (settings, cases that read them)
-SETS = {
-    "allowNegativeIdepths=0": (dict(allowNegativeIdepths=0), DEPTH + LOOP),
-    "useSubpixelStereo=0": (dict(useSubpixelStereo=0), DEPTH + LOOP),
-    "minUseGrad=2.5": (dict(minUseGrad=2.5), ("frame_builders",) + DEPTH + TRACK + LOOP),
-    "minUseGrad=10": (dict(minUseGrad=10.0), ("frame_builders",) + DEPTH + TRACK + LOOP),
-    "cameraPixelNoise2=1": (dict(cameraPixelNoise2=1.0), DEPTH + TRACK + LOOP),
-    "cameraPixelNoise2=36": (dict(cameraPixelNoise2=36.0), DEPTH + TRACK + LOOP),
-    "depthSmoothingFactor=0": (dict(depthSmoothingFactor=0.0), DEPTH + LOOP),
-    "depthSmoothingFactor=3": (dict(depthSmoothingFactor=3.0), DEPTH + LOOP),
-    "useAffineLightningEstimation=0": (dict(useAffineLightningEstimation=0), TRACK + LOOP),
-    "combined": (dict(minUseGrad=7.5, cameraPixelNoise2=9.0, depthSmoothingFactor=2.0, allowNegativeIdepths=0,
-                      useSubpixelStereo=0, useAffineLightningEstimation=0), ("frame_builders",) + DEPTH + TRACK + LOOP),
-}
-PAIRS = [(s, c) for s, (_, cases) in SETS.items() for c in cases]
-
-
-def _run(set_name, case, gold, seq, frames):
-    """runs one case under one set on the C restatement (gold = the record) or on the reference-compiled library (gold = None);
-    returns the case's Pin.  The libraries are back at the defaults afterwards."""
-    g, _ = SETS[set_name]
-    fn, fl, ref_fl = pin.CASES[case]
-    fl = ref_fl if gold is None else fl
-    p = pin.Pin(f"{set_name}/{case}", gold)
-    try:
-        with pin.settings(**g):
-            fn(p, fl, seq, frames)
-    finally:
-        po.set_globals(fl)
-    return p
-
-
-def record(seq, frames):
-    """every (set, case) on the reference-compiled library (needs oracle/_ref): the arrays of the golden file"""
-    out = {}
-    for s, c in PAIRS:
-        out.update(_run(s, c, None, seq, frames).rec)
-    return out
-
-
+PAIRS = pin.SETTINGS_PAIRS
 _gold = None
 
 
 def _load():
     global _gold
     if _gold is None:
-        _gold = np.load(GOLD)
+        _gold = np.load(pin.GOLD_GLOBALS)
     return _gold
 
 
 @pytest.mark.parametrize("set_name,case", PAIRS, ids=[f"{s}-{c}" for s, c in PAIRS])
 def test_matches_reference_compiled_under_settings(seq_small, frames_small, set_name, case):
-    _run(set_name, case, _load(), seq_small, frames_small)
+    pin.run_under_settings(set_name, case, _load(), seq_small, frames_small)
 
 
-@pytest.mark.parametrize("set_name", list(SETS))
+@pytest.mark.parametrize("set_name", list(pin.SETS))
 def test_each_set_changes_the_recorded_outputs(set_name):
     """the record of every set differs from the default record somewhere: the setting reached the reference's code"""
     g, d = _load(), np.load(pin.GOLD)
@@ -94,6 +46,6 @@ def test_min_use_grad_values_are_ties_on_frame0(seq_small, frames_small):
     """Frame 0 has pixels whose maxGradients equal each minUseGrad value exactly, so the pins above separate `<` from `<=`."""
     po.set_globals(False)
     mg = po.Frame(0, frames_small[0][0], seq_small.K).maxGradients(0)[2:-2]      # the defined interior, see frame_builders
-    for s, (g, _) in SETS.items():
+    for s, (g, _) in pin.SETS.items():
         if "minUseGrad" in g:
             assert int((mg == np.float32(g["minUseGrad"])).sum()) > 0, s

@@ -2,7 +2,7 @@
 
 Every other pin runs the synthetic stream's default twist: mostly sideways, so every epipolar line the depth map searches is close
 to horizontal and points the same way, the epipole lies far outside the image, and propagation never lands two sources at
-inconsistent depths on one pixel.  This module runs the case functions of tests/test_ref_pin.py that read the geometry under the
+inconsistent depths on one pixel.  This module runs the case functions of tests/pin_cases.py that read the geometry under the
 vertical, forward, backward and roll motions, plus two cases the default stream cannot reach:
   * wide_baseline: keyframe 0 on ground truth, one updateKeyframe with frame 40 (forward, backward) -- depth ratios outside
     doLineStereo's rescale gate, sample points outside the image;
@@ -14,55 +14,14 @@ python -m tests.golden.make_golden_ref_pin_motions.
 
 Non-vacuity: the C restatement's branch counters (oracle/lsd_oracle.h, LSDO_BR_*) show that each (motion, case) reaches the
 branches listed for it in REACHES at least that many times, and each motion's record differs from the default record."""
-import os
-
 import numpy as np
 import pytest
 
 from oracle import pyoracle as po
 from tests import motions
-from tests import test_ref_pin as pin
+from tests import pin_cases as pin
 
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_pin_motions_320x240.npz")
-
-WIDE_BASELINE_FRAME = 40
-PROPAGATION_FRAME = 8
-
-
-def wide_baseline(p, fl, seq, frames):
-    """updateKeyframe with one frame far from the keyframe, on ground-truth depth and poses"""
-    s = pin.Side(seq, frames, fl, "gt")
-    k = WIDE_BASELINE_FRAME
-    s.add_frame(k, pin._gt_qts(seq, k))
-    s.dm.updateKeyframe([s.fr[k]])
-    assert p.hyp(f"updateKeyframe[{k}]", s.dm.current()) > 10000
-
-
-def propagation_collisions(p, fl, seq, frames):
-    """propagateDepth of a random map: its sources disagree about depth, so under a motion along the optical axis many land on one
-    pixel at inconsistent depths (DepthMap.cpp:588-601); validity 200 makes every merge exceed the cap of :626"""
-    k = PROPAGATION_FRAME
-    mask = (np.random.default_rng(8).random((seq.h // 2, seq.w // 2)) > 0.15).astype(np.uint8)
-    for what, m, validity in (("no mask", None, None), ("mask", mask, None), ("validity 200", None, 200)):
-        s = pin.Side(seq, frames, fl, "random")
-        if validity is not None:
-            cur = s.dm.current().copy()
-            cur["validity_counter"][cur["isValid"] != 0] = validity
-            s.dm.set_current(cur)
-        s.add_frame(k, pin._gt_qts(seq, k), mask=m)
-        s.dm.propagateDepth(s.fr[k])
-        assert p.hyp(f"propagateDepth[{k}] {what}", s.dm.current()) > 5000
-
-
-# the case functions of tests/test_ref_pin.py that read the camera motion
-GEOMETRY = ("prepare_for_stereo", "depthmap_update_sequence", "depthmap_random_init_every_branch", "depthmap_individual_passes",
-            "create_keyframe_and_finalize", "se3_single_evaluation", "se3_track_scalar", "bench_loop_with_keyframe_changes")
-# case -> (function, C-restatement flavour, reference-compiled flavour), as test_ref_pin.CASES
-CASES = {c: pin.CASES[c] for c in GEOMETRY}
-CASES["wide_baseline"] = (wide_baseline, False, "ref")
-CASES["propagation_collisions"] = (propagation_collisions, False, "ref")
-ONLY = {"wide_baseline": ("forward", "backward"), "propagation_collisions": ("forward", "backward")}
-PAIRS = [(m, c) for m in motions.MOTIONS for c in CASES if m in ONLY.get(c, (m,))]
+PAIRS = pin.MOTION_PAIRS
 
 # (motion, case) -> {branch: at least this many runs} on the C restatement (pyoracle.BRANCHES), about half the measured count.
 # prepare_for_stereo and se3_single_evaluation run no depth-map pass: they read the motion through the frames and poses only.
@@ -141,53 +100,20 @@ REACHES = {
              subpixel_post=10000, prop_merge=400),
 }
 
-
-_streams: dict = {}
-
-
-def stream(motion):
-    if motion not in _streams:
-        seq = motions.sequence(motion)
-        _streams[motion] = (seq, motions.Frames(seq))
-    return _streams[motion]
-
-
-def _run(motion, case, gold):
-    """runs one case under one motion on the C restatement (gold = the record) or on the reference-compiled library
-    (gold = None); returns the case's Pin"""
-    fn, fl, ref_fl = CASES[case]
-    fl = ref_fl if gold is None else fl
-    seq, frames = stream(motion)
-    p = pin.Pin(f"{motion}/{case}", gold)
-    try:
-        fn(p, fl, seq, frames)
-    finally:
-        po.set_globals(fl)
-    return p
-
-
-def record():
-    """every (motion, case) on the reference-compiled library (needs oracle/_ref): the arrays of the golden file"""
-    out = {}
-    for m, c in PAIRS:
-        out.update(_run(m, c, None).rec)
-    return out
-
-
 _gold = None
 
 
 def _load():
     global _gold
     if _gold is None:
-        _gold = np.load(GOLD)
+        _gold = np.load(pin.GOLD_MOTIONS)
     return _gold
 
 
 @pytest.mark.parametrize("motion,case", PAIRS, ids=[f"{m}-{c}" for m, c in PAIRS])
 def test_matches_reference_compiled_under_motion(motion, case):
     po.branch_counts_reset()
-    _run(motion, case, _load())
+    pin.run_under_motion(motion, case, _load())
     got = po.branch_counts()
     low = {b: (got[b], n) for b, n in REACHES[(motion, case)].items() if got[b] < n}
     assert not low, f"{motion}/{case}: branches reached fewer times than stated (got, stated): {low}"
@@ -225,7 +151,7 @@ def test_default_cases_leave_those_branches_unreached(seq_small, frames_small):
     motion never run those branches"""
     po.set_globals(False)
     po.branch_counts_reset()
-    for c in GEOMETRY:
+    for c in pin.GEOMETRY:
         fn, fl, _ = pin.CASES[c]
         fn(pin.Pin(c), fl, seq_small, frames_small)
     got = po.branch_counts()
