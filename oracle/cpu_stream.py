@@ -17,8 +17,11 @@ IDENT = np.array([0, 0, 0, 1, 0, 0, 0], np.float64)
 
 
 class CpuStream:
-    def __init__(self, seq, flavour=False, kf_every: int = 20, settings=None):
-        self.seq, self.fl, self.kf_every = seq, flavour, kf_every
+    def __init__(self, seq, flavour=False, kf_every: int = 20, settings=None, keep_keyframes: bool = False):
+        """keep_keyframes: hold every finished keyframe's Frame in `finished` (with the depth finalizeKeyFrame left in it),
+        as the keyframe graph does, instead of dropping it once the next keyframe is made"""
+        self.seq, self.fl, self.kf_every, self.keep_keyframes = seq, flavour, kf_every, keep_keyframes
+        self.finished: list = []
         self.L = po.lib(flavour)
         self.st = settings or po.default_track_settings(flavour)
         self.kf = None
@@ -55,6 +58,8 @@ class CpuStream:
         if kf_change:
             self.dm.finalizeKeyFrame()
             self.dm.createKeyFrame(f)
+            if self.keep_keyframes:
+                self.finished.append(self.kf)
             self.kf = f
             self.last = IDENT.copy()
             self.kf_changes.append(fid)

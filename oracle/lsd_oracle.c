@@ -118,8 +118,22 @@ static float tree_sum_f(const float* v, int n)
     return tree_sum_f(v, h) + tree_sum_f(v+h, n-h);
 }
 
-/* Eigen LDLT (Cholesky/LDLT.h, unblocked lower, largest-|diagonal| pivoting) + solve, float; N <= 8 */
-static int ldlt_solve_n(int N, const float* Ain, const float* bin, float* x)
+/* diagnostic counters of the Sim3 tracker and the permaRef overlap (lsd_oracle.h, LSDO_S3_*): relaxed atomic adds that read
+ * and write no float, as the depth map's in lsd_oracle_depth.inc */
+static int64_t sim3Counts[LSDO_S3_COUNT];
+#define COUNT_S3(b) __atomic_fetch_add(&sim3Counts[b], 1, __ATOMIC_RELAXED)
+void lsdo_sim3_branch_counts(int64_t out[LSDO_S3_COUNT])
+{
+    for (int i = 0; i < LSDO_S3_COUNT; i++) out[i] = __atomic_load_n(&sim3Counts[i], __ATOMIC_RELAXED);
+}
+void lsdo_sim3_branch_counts_reset(void)
+{
+    for (int i = 0; i < LSDO_S3_COUNT; i++) __atomic_store_n(&sim3Counts[i], 0, __ATOMIC_RELAXED);
+}
+
+/* Eigen LDLT (Cholesky/LDLT.h, unblocked lower, largest-|diagonal| pivoting) + solve, float; N <= 8.
+ * *permuted (if given) is set when the pivoting swapped a row. */
+static int ldlt_solve_n(int N, const float* Ain, const float* bin, float* x, int* permuted)
 {
     float A[8][8]; int tr[8]; float cutoff = 0;
     for (int i = 0; i < N; i++) for (int j = 0; j < N; j++) A[i][j] = Ain[i*N+j];
@@ -163,10 +177,11 @@ static int ldlt_solve_n(int N, const float* Ain, const float* bin, float* x)
     for (int i = N-2; i >= 0; i--) { float pr[8]; int n = N-1-i; for (int j = 0; j < n; j++) pr[j] = A[i+1+j][i]*y[i+1+j]; y[i] -= tree_sum_f(pr, n); }
     for (int k = N-1; k >= 0; k--) if (tr[k] != k) { float t = y[k]; y[k] = y[tr[k]]; y[tr[k]] = t; }
     for (int i = 0; i < N; i++) x[i] = y[i];
+    if (permuted) { *permuted = 0; for (int k = 0; k < N; k++) *permuted |= tr[k] != k; }
     return 0;
 }
-int lsdo_ldlt6_solve(const float Ain[36], const float bin[6], float x[6]) { return ldlt_solve_n(6, Ain, bin, x); }
-int lsdo_ldlt7_solve(const float Ain[49], const float bin[7], float x[7]) { return ldlt_solve_n(7, Ain, bin, x); }
+int lsdo_ldlt6_solve(const float Ain[36], const float bin[6], float x[6]) { return ldlt_solve_n(6, Ain, bin, x, 0); }
+int lsdo_ldlt7_solve(const float Ain[49], const float bin[7], float x[7]) { return ldlt_solve_n(7, Ain, bin, x, 0); }
 
 /* ---- Sophus SE3 in float and double; qt = (qx,qy,qz,qw, tx,ty,tz) ----
  * generated twice through a macro so that the float flavour really computes in float
@@ -1214,8 +1229,9 @@ float lsdo_checkPermaRefOverlap(int w0, int h0, const float K4[9], const float* 
         float v_new = (Wxp[1]/Wxp[2])*fy_l + cy_l;
         if ((u_new > 0 && v_new > 0 && u_new < w2 && v_new < h2)) {
             float depthChange = p[2] / Wxp[2];
+            if (!(depthChange < 1)) COUNT_S3(LSDO_PERMA_USAGE_CLAMP);
             usageCount += depthChange < 1 ? depthChange : 1;
-        }
+        } else COUNT_S3(LSDO_PERMA_OUTSIDE);
     }
     return usageCount / (float)numPts;
 }

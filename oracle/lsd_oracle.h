@@ -220,6 +220,10 @@ int   lsdo_frame_setPermaRef(lsdo_frame* kf, float* posData, float* colorAndVarD
 float lsdo_checkPermaRefOverlap(int w0, int h0, const float K4[9], const float* permaPos, int numPts, const double refToFrame_qt[7]);
 int   lsdo_trackFrameOnPermaref(int w0, int h0, const float* permaPos, const float* permaColVar, int numPts,
                                 lsdo_frame* frame, const double refToFrame_qt[7], lsdo_track_result* out /* frameToRef_qt holds referenceToFrame */);
+/* the reference-compiled library only: SE3Tracker's own two calls on a keyframe whose setPermaRef ran (the reference reads the
+ * snapshot from the Frame); the LM call counters are locals there and come back as -1 */
+float lsdo_ref_checkPermaRefOverlap(lsdo_frame* kf, const double refToFrame_qt[7]);
+int   lsdo_ref_trackFrameOnPermaref(lsdo_frame* kf, lsdo_frame* frame, const double refToFrame_qt[7], lsdo_track_result* out);
 
 /* ---- DepthMap (DepthEstimation/DepthMap.cpp) ---- */
 lsdo_depthmap* lsdo_depthmap_create(int w, int h, const float K[9]);
@@ -264,6 +268,21 @@ enum {
 };
 void lsdo_depth_branch_counts(int64_t out[LSDO_BR_COUNT]);
 void lsdo_depth_branch_counts_reset(void);
+/* the same for the Sim3 tracker's scalar path, the permaRef overlap and the 7x7 solve (C restatement only) */
+enum {
+    LSDO_S3_OUTSIDE,          /* calcSim3Buffers: point warped outside the image, Sim3Tracker.cpp:486 */
+    LSDO_S3_NO_DEPTH,         /* calcSim3Buffers: warped onto a frame pixel without depth (var_frameDepth <= 0), :531-541 */
+    LSDO_S3_USAGE_CLAMP,      /* calcSim3Buffers: depthChange >= 1, usage clamped to 1, :579-580 */
+    LSDO_S3_AFFINE_CLAMP,     /* calcSim3Buffers: |residual_p| >= 2, affine weight 2/|r|, :514 */
+    LSDO_S3_HUBER,            /* calcSim3WeightsAndResidual: weighted residual >= huber_d, :795 */
+    LSDO_S3_LDLT7_SOLVE,      /* trackFrameSim3's 7x7 LDLT solves, Sim3Tracker.cpp:224 */
+    LSDO_S3_LDLT7_PIVOT,      /* ... of which the pivoting permuted a row (Eigen LDLT) */
+    LSDO_PERMA_OUTSIDE,       /* checkPermaRefOverlap: point outside, SE3Tracker.cpp:148 */
+    LSDO_PERMA_USAGE_CLAMP,   /* checkPermaRefOverlap: depthChange >= 1, :150-151 */
+    LSDO_S3_COUNT
+};
+void lsdo_sim3_branch_counts(int64_t out[LSDO_S3_COUNT]);
+void lsdo_sim3_branch_counts_reset(void);
 
 #ifdef __cplusplus
 }

@@ -184,6 +184,8 @@ def lib(fast=False):
     sig("lsdo_frame_setPermaRef", C.c_int, vp, fp, fp)
     sig("lsdo_checkPermaRefOverlap", C.c_float, C.c_int, C.c_int, fp, fp, C.c_int, dp)
     sig("lsdo_trackFrameOnPermaref", C.c_int, C.c_int, C.c_int, fp, fp, C.c_int, vp, dp, C.POINTER(TrackResult))
+    sig("lsdo_ref_checkPermaRefOverlap", C.c_float, vp, dp)
+    sig("lsdo_ref_trackFrameOnPermaref", C.c_int, vp, vp, dp, C.POINTER(TrackResult))
     sig("lsdo_depthmap_create", vp, C.c_int, C.c_int, fp)
     sig("lsdo_depthmap_destroy", None, vp)
     sig("lsdo_depthmap_reset", None, vp)
@@ -205,6 +207,8 @@ def lib(fast=False):
     if not isinstance(fast, str):            # diagnostic counters of the C restatement only
         sig("lsdo_depth_branch_counts", None, C.POINTER(C.c_int64))
         sig("lsdo_depth_branch_counts_reset", None)
+        sig("lsdo_sim3_branch_counts", None, C.POINTER(C.c_int64))
+        sig("lsdo_sim3_branch_counts_reset", None)
     _libs[name] = L
     return L
 
@@ -243,6 +247,22 @@ def branch_counts_reset(fast=False) -> None:
     lib(fast).lsdo_depth_branch_counts_reset()
 
 
+# the same for the Sim3 tracker, the 7x7 solve and the permaRef overlap, in the order of lsd_oracle.h's LSDO_S3_* enum
+SIM3_BRANCHES = ("sim3_outside", "sim3_no_depth", "sim3_usage_clamp", "sim3_affine_clamp", "sim3_huber", "ldlt7_solve",
+                 "ldlt7_pivot", "perma_outside", "perma_usage_clamp")
+
+
+def sim3_branch_counts(fast=False) -> dict:
+    """how often each counted branch of the Sim3 tracker's scalar path and of checkPermaRefOverlap ran since the last reset"""
+    out = np.zeros(len(SIM3_BRANCHES), np.int64)
+    lib(fast).lsdo_sim3_branch_counts(out.ctypes.data_as(C.POINTER(C.c_int64)))
+    return dict(zip(SIM3_BRANCHES, out.tolist()))
+
+
+def sim3_branch_counts_reset(fast=False) -> None:
+    lib(fast).lsdo_sim3_branch_counts_reset()
+
+
 def set_globals(fast=False, **kw) -> Globals:
     g = Globals()
     lib(fast).lsdo_default_globals(C.byref(g))
@@ -262,6 +282,7 @@ class Frame:
         Kf = np.ascontiguousarray(K, np.float32).reshape(9)
         self.ptr = self.L.lsdo_frame_create_u8(fid, self.w, self.h, _fp(Kf), img.ctypes.data_as(C.POINTER(C.c_uint8)))
         self.id = fid
+        self.fl = fast
 
     def __del__(self):
         if getattr(self, "ptr", None):
@@ -349,7 +370,8 @@ class Frame:
 
 
 class PermaRef:
-    """Frame::setPermaRef snapshot of a keyframe's level-4 point cloud (Frame.cpp:149-174)"""
+    """Frame::setPermaRef snapshot of a keyframe's level-4 point cloud (Frame.cpp:149-174).  The C restatement takes the
+    snapshot's arrays; the reference-compiled library reads them from the keyframe, which this object therefore keeps."""
 
     def __init__(self, kf: Frame):
         w, h = kf.size(4)
@@ -359,16 +381,23 @@ class PermaRef:
         self.n = kf.L.lsdo_frame_setPermaRef(kf.ptr, _fp(self.pos), _fp(self.colvar))
         self.K4 = kf.K(4)[0].copy()
         self.L = kf.L
+        self.kf = kf
+        self.ref = isinstance(kf.fl, str)
 
     def overlap(self, refToFrame_qt) -> float:
         q = np.ascontiguousarray(refToFrame_qt, np.float64)
+        if self.ref:
+            return float(self.L.lsdo_ref_checkPermaRefOverlap(self.kf.ptr, _dp(q)))
         K4 = np.ascontiguousarray(self.K4, np.float32).reshape(9)
         return float(self.L.lsdo_checkPermaRefOverlap(self.w0, self.h0, _fp(K4), _fp(self.pos), self.n, _dp(q)))
 
     def track(self, frame: Frame, refToFrame_qt) -> TrackResult:
         q = np.ascontiguousarray(refToFrame_qt, np.float64)
         r = TrackResult()
-        self.L.lsdo_trackFrameOnPermaref(self.w0, self.h0, _fp(self.pos), _fp(self.colvar), self.n, frame.ptr, _dp(q), C.byref(r))
+        if self.ref:
+            self.L.lsdo_ref_trackFrameOnPermaref(self.kf.ptr, frame.ptr, _dp(q), C.byref(r))
+        else:
+            self.L.lsdo_trackFrameOnPermaref(self.w0, self.h0, _fp(self.pos), _fp(self.colvar), self.n, frame.ptr, _dp(q), C.byref(r))
         return r
 
 

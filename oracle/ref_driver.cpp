@@ -415,6 +415,38 @@ int lsdo_se3_track(lsdo_frame* kf, lsdo_frame* frame, const double frameToRef_in
 }
 
 // ---- Sim3Tracker (Tracking/Sim3Tracker.cpp:149-382) ----
+// one evaluation as trackFrameSim3 runs it per LM step: calcSim3Buffers -> calcSim3WeightsAndResidual -> calcSim3LGS
+int lsdo_sim3_eval(lsdo_frame* ref_kf, lsdo_frame* frame, int level, const double refToFrame_qts[8], float affine_a, float affine_b,
+                   const lsdo_track_settings* s, lsdo_sim3_eval_result* out)
+{
+    std::memset(out, 0, sizeof(*out));
+    Sim3Tracker t(ref_kf->w, ref_kf->h, ref_kf->f->K(0));
+    applyTrackSettings(t.settings, s);
+    TrackingReference ref;
+    ref.importFrame(ref_kf->f.get());
+    ref.makePointCloud(level);
+    t.affineEstimation_a = affine_a; t.affineEstimation_b = affine_b;
+    const Sim3 T = sim3FromQts(refToFrame_qts);
+    LGS7 ls7;
+#if defined(ENABLE_SSE)
+    t.calcSim3BuffersSSE(&ref, frame->f.get(), T, level, false);
+    Sim3ResidualStruct r = t.calcSim3WeightsAndResidualSSE(T);
+    t.calcSim3LGSSSE(ls7);
+#else
+    t.calcSim3Buffers(&ref, frame->f.get(), T, level, false);
+    Sim3ResidualStruct r = t.calcSim3WeightsAndResidual(T);
+    t.calcSim3LGS(ls7);
+#endif
+    for (int i = 0; i < 7; i++) { for (int j = 0; j < 7; j++) out->A[i * 7 + j] = ls7.A(i, j); out->b[i] = ls7.b[i]; }
+    out->num_constraints = (int)ls7.num_constraints;
+    out->sumResD = r.sumResD; out->sumResP = r.sumResP; out->numTermsD = r.numTermsD; out->numTermsP = r.numTermsP;
+    out->mean = r.mean; out->meanD = r.meanD; out->meanP = r.meanP;
+    out->warpedSize = t.buf_warped_size; out->pointUsage = t.pointUsage;
+    out->affine_a_lastIt = t.affineEstimation_a_lastIt; out->affine_b_lastIt = t.affineEstimation_b_lastIt;
+    ref.invalidate();
+    return 0;
+}
+
 int lsdo_sim3_track(lsdo_frame* ref_kf, lsdo_frame* frame, const double frameToRef_init_qts[8], int startLevel, int finalLevel,
                     const lsdo_track_settings* s, lsdo_sim3_result* out)
 {
@@ -447,6 +479,24 @@ int lsdo_frame_setPermaRef(lsdo_frame* kf, float* posData, float* colorAndVarDat
     }
     ref.invalidate();
     return n;
+}
+float lsdo_ref_checkPermaRefOverlap(lsdo_frame* kf, const double refToFrame_qt[7])
+{
+    SE3Tracker t(kf->w, kf->h, kf->f->K(0));
+    return t.checkPermaRefOverlap(kf->f.get(), se3FromQt(refToFrame_qt));
+}
+int lsdo_ref_trackFrameOnPermaref(lsdo_frame* kf, lsdo_frame* frame, const double refToFrame_qt[7], lsdo_track_result* out)
+{
+    std::memset(out, 0, sizeof(*out));
+    SE3Tracker t(kf->w, kf->h, kf->f->K(0));
+    SE3 res = t.trackFrameOnPermaref(kf->f.get(), frame->f.get(), se3FromQt(refToFrame_qt));
+    qtFromSE3(res, out->frameToRef_qt);             // referenceToFrame, as the C restatement returns it
+    out->pointUsage = t.pointUsage; out->lastGoodCount = t.lastGoodCount; out->lastBadCount = t.lastBadCount;
+    out->lastMeanRes = t.lastMeanRes; out->lastResidual = t.lastResidual;
+    out->affineEstimation_a = t.affineEstimation_a; out->affineEstimation_b = t.affineEstimation_b;
+    out->diverged = t.diverged; out->trackingWasGood = t.trackingWasGood;
+    for (int i = 0; i < PYRAMID_LEVELS; i++) out->numCalcResidualCalls[i] = out->numCalcWarpUpdateCalls[i] = -1;   // not counted there
+    return 0;
 }
 
 // ---- DepthMap ----

@@ -4,10 +4,12 @@ checks the results with tests/util.py; the caller chooses the context, the strea
 import numpy as np
 
 from lsd_slam_b200 import abi, synth
-from lsd_slam_b200.stream import GpuStream, GpuStreamGroup
-from tests.util import (IDENT, Pair, check_perma_track, check_se3_eval, check_se3_track, check_sim3_eval, check_sim3_track,
-                        kf_depth_equal, new_depth, observe, oracle_sim3_track, pose_err, se3_inverse, sim3_err, sim3_init,
-                        sim3_inverse, sim3_mul, tracked_pair)
+from lsd_slam_b200.stream import GpuStream, GpuStreamGroup, sim3_mul_qts
+from tests.pin_cases import (AB, MAPPED_FRAMES, MAPPED_KF_EVERY, PERMA_FRAME, POSE_SENSITIVE_DEPTH_RESIDUAL, SIM3_DT, SIM3_SCALE,
+                             adversarial_edit, set_depth)
+from tests.util import (IDENT, Pair, check_perma_overlap, check_perma_track, check_se3_eval, check_se3_track, check_sim3_eval,
+                        check_sim3_track, kf_depth_equal, new_depth, observe, oracle_sim3_track, perma_noise, pose_err, se3_inverse,
+                        sim3_err, sim3_init, sim3_inverse, sim3_mul, tracked_pair)
 
 
 # ---- depth map, bit for bit -------------------------------------------------------------------------------------------------
@@ -323,6 +325,237 @@ def perma_batch(ctx, oracle, seq, trk, prs, fid):
         inits += [gt_inv, IDENT]
     res = trk.trackFrameOnPermaref(ids, fid, np.array(inits))
     return sum(check_perma_track(g, prs[k].track(of, init)) for k, init, g in zip(ids, inits, res))
+
+
+# ---- Sim3 and permaRef on keyframes the device's mapper finished ---------------------------------------------------------------
+def hyp_of_planes(oracle, idepth, var):
+    """hypotheses that Frame::setDepth turns back into these level-0 planes: valid pixels (var > 0) are >= -0.05 there, so
+    setDepth keeps them as they are and turns every other pixel into -1 / -1 again"""
+    hyp = np.zeros(idepth.shape, oracle.HYP_DTYPE)
+    hyp["isValid"] = var > 0
+    hyp["idepth"] = hyp["idepth_smoothed"] = idepth
+    hyp["idepth_var"] = hyp["idepth_var_smoothed"] = var
+    return hyp
+
+
+def mirror(oracle, ctx, seq, kf, img):
+    """an oracle Frame of the same image given the device keyframe's level-0 plane through Frame::setDepth"""
+    f = oracle.Frame(kf, img, seq.K)
+    set_depth(f, hyp_of_planes(oracle, ctx.download(kf, abi.BUF_IDEPTH, 0), ctx.download(kf, abi.BUF_IDEPTH_VAR, 0)))
+    return f
+
+
+def pyramid_mismatches(ctx, kf, of):
+    """(level, plane) pairs whose bits differ between the device keyframe and its oracle Frame"""
+    bad = []
+    for lvl in range(abi.LEVELS):
+        for name, buf, plane in (("idepth", abi.BUF_IDEPTH, of.idepth), ("idepthVar", abi.BUF_IDEPTH_VAR, of.idepthVar)):
+            if not np.array_equal(ctx.download(kf, buf, lvl).view(np.uint32), plane(lvl).view(np.uint32)):
+                bad.append((lvl, name))
+    return bad
+
+
+class MappedRun:
+    """A GpuStream of the seed-1234 sequence of `motion` (tests/motions.py; the default twist by default) with its finished
+    keyframes resident and an oracle mirror of each.  After every keyframe change it compares the pyramids of every resident
+    keyframe with the oracle (`checks`)."""
+
+    def __init__(self, oracle, w, h, motion="default"):
+        from tests import motions
+        self.motion = motion
+        self.seq = seq = motions.sequence(motion, w, h)
+        self.ctx = ctx = abi.Context(w, h, seq.K, max_frames=12)
+        self.gs = gs = GpuStream(ctx, kf_every=MAPPED_KF_EVERY, keep_keyframes=True)
+        self.images = {}
+        img, d = seq.render(0)
+        self.images[0] = img
+        gs.init_gt(0, img, d)
+        self.of, self.checks = {}, []
+        for k in range(1, MAPPED_FRAMES):
+            self.images[k] = seq.render(k)[0]
+            change = gs.next_is_keyframe_change()
+            gs.step(k, self.images[k])
+            if not change:
+                continue
+            for kf in gs.keyframe_ids[:-1]:           # finished: mirrored once, then re-checked after every later change
+                if kf not in self.of:
+                    self.of[kf] = mirror(oracle, ctx, seq, kf, self.images[kf])
+                self.checks.append((k, kf, pyramid_mismatches(ctx, kf, self.of[kf])))
+            active = gs.keyframe_ids[-1]              # the new keyframe as createKeyFrame left it
+            self.checks.append((k, active, pyramid_mismatches(ctx, active, mirror(oracle, ctx, seq, active, self.images[active]))))
+        self.kfs = gs.keyframe_ids[:-1]
+        self.active = gs.keyframe_ids[-1]
+        self.active_hyp = gs.map.current()            # the active keyframe's hypotheses (DepthMap::currentDepthMap)
+
+    def frame_to_ref(self, oracle, ref, fr, perturb=True):
+        """the relative Sim3 SlamSystem starts from: reference->getScaledCamToWorld().inverse() * frame->getScaledCamToWorld()
+        (scale ratio of the two keyframes included), with util.sim3_init's perturbation of translation and scale"""
+        c2w = dict(zip(self.gs.keyframe_ids, self.gs.keyframe_cam_to_world))
+        q = sim3_mul_qts(sim3_inverse(oracle, c2w[ref]), c2w[fr])
+        if perturb:
+            q[4:7] += SIM3_DT
+            q[7] *= SIM3_SCALE
+        return q
+
+    def ref_to_frame(self, oracle, ref, fr, perturb=True):
+        return sim3_inverse(oracle, self.frame_to_ref(oracle, ref, fr, perturb))
+
+    def pairs(self):
+        return [(a, b) for a in self.kfs for b in self.kfs if a != b]
+
+    def close(self):
+        self.ctx.close()
+
+
+def mapped_mirror_bit_exact(mapped):
+    """every resident keyframe's idepth / idepthVar pyramid (levels 0-4) equals the oracle's Frame::setDepth of the same
+    level-0 plane, and a finished keyframe stays so through the later map swaps and createKeyFrame calls of the run"""
+    assert len(mapped.kfs) >= 3
+    assert [kf for _, kf, _ in mapped.checks].count(mapped.kfs[0]) >= 3
+    bad = [(k, kf, m) for k, kf, m in mapped.checks if m]
+    assert not bad, bad
+    ctx = mapped.ctx
+    spread = []
+    for kf in mapped.kfs:                             # what these tests are about: a semi-dense map, no variance shared by all
+        var = ctx.download(kf, abi.BUF_IDEPTH_VAR, 0)
+        v = var[var > 0]
+        assert 0.2 < v.size / var.size < 0.7 and np.unique(v).size > 100, (kf, v.size / var.size, np.unique(v).size)
+        spread.append(v.max() / v.min())
+    assert max(spread) > 30, spread
+    scales = [q[7] for q in mapped.gs.keyframe_cam_to_world]
+    assert max(scales) / min(scales) > 1.2, scales       # createKeyFrame rescales every new keyframe
+
+
+def mapped_sim3_eval(run, oracle):
+    """one Sim3 evaluation per ordered pair, perturbed and not, levels 4..1, two affine estimates"""
+    trk = abi.Sim3Tracker(run.ctx)
+    n_no_depth = 0
+    for ref, fr in run.pairs():
+        for perturb in (True, False):
+            r2f = run.ref_to_frame(oracle, ref, fr, perturb)
+            for lvl in (4, 3, 2, 1):
+                for a, b in AB:
+                    got = trk.eval(ref, fr, lvl, r2f, a, b)
+                    want = oracle.sim3_eval(run.of[ref], run.of[fr], lvl, r2f, a, b)
+                    assert want.warpedSize > 10, (ref, fr, lvl)
+                    check_sim3_eval(got, want)
+                    n_no_depth += want.numTermsD < want.numTermsP      # warped onto frame pixels without depth (sim3.cuh:116-117)
+    assert n_no_depth > 0
+
+
+def mapped_sim3_eval_settings(run, oracle):
+    """var_weight and huber_d other than their defaults (1, 3) reach the kernel's weights"""
+    trk = abi.Sim3Tracker(run.ctx)
+    st = oracle.default_track_settings(main_tracker=False)
+    for s in (trk.settings, st):
+        s.var_weight, s.huber_d = 2.5, 1.5
+    for ref, fr in run.pairs():
+        r2f = run.ref_to_frame(oracle, ref, fr)
+        for lvl in (4, 3, 2, 1):
+            a, b = AB[lvl % 2]
+            check_sim3_eval(trk.eval(ref, fr, lvl, r2f, a, b), oracle.sim3_eval(run.of[ref], run.of[fr], lvl, r2f, a, b, settings=st))
+
+
+def mapped_sim3_track(run, oracle):
+    """trackFrameSim3 per ordered pair over levels 4..1 and 3..2 (lastDepthResidual of pin_cases.POSE_SENSITIVE_DEPTH_RESIDUAL
+    against the exact-sum twin to the reference tolerance)"""
+    trk = abi.Sim3Tracker(run.ctx)
+    n_converged = 0
+    for ref, fr in run.pairs():
+        init = run.frame_to_ref(oracle, ref, fr)
+        for lo, hi in ((4, 1), (3, 2)):
+            est = trk.trackFrameSim3(ref, fr, init, lo, hi)
+            want, exact = oracle_sim3_track(oracle, run.of[ref], run.of[fr], init, lo, hi)
+            check_sim3_track(trk.last, want)
+            sensitive = (run.motion, ref, fr, lo, hi) in POSE_SENSITIVE_DEPTH_RESIDUAL
+            check_sim3_track(trk.last, exact, res_tol=5e-4, depth_res_tol=2e-2 if sensitive else None)
+            assert np.array_equal(est, np.array(trk.last.frameToRef_qts))
+            n_converged += not want.diverged
+    assert n_converged >= len(run.pairs())
+
+
+def mapped_sim3_batch(run, oracle):
+    """every ordered pair in one launch == one by one (bit-identical) == the oracle"""
+    trk = abi.Sim3Tracker(run.ctx)
+    pairs = run.pairs()
+    inits = np.array([run.frame_to_ref(oracle, ref, fr) for ref, fr in pairs])
+    res = trk.trackFrameSim3Batch([p[0] for p in pairs], [p[1] for p in pairs], inits, 4, 1)
+    for (ref, fr), init, r in zip(pairs, inits, res):
+        trk.trackFrameSim3(ref, fr, init, 4, 1)
+        assert bytes(trk.last) == bytes(r)
+        check_sim3_track(r, oracle.sim3_track(run.of[ref], run.of[fr], init, 4, 1))
+
+
+def mapped_perma(run, oracle, noise_aware=False):
+    """setPermaRef of each finished keyframe, the overlap at random poses, trackFrameOnPermaref of PERMA_FRAME from its
+    ground-truth pose (translation in the keyframe's map units: the chain's scale of the keyframe) and from identity.
+    noise_aware: the pose tolerance grows by the reference's own summation noise of each tracking (util.perma_noise)"""
+    ctx, seq = run.ctx, run.seq
+    se3 = abi.SE3Tracker(ctx)
+    prs = {}
+    for k in run.kfs:
+        prs[k] = oracle.PermaRef(run.of[k])
+        assert se3.setPermaRef(k) == prs[k].n > 30
+    want = check_perma_overlap(se3, oracle, prs, np.random.default_rng(3))
+    assert want.min() < 0.9 < want.max()
+    img = seq.render(PERMA_FRAME)[0]
+    ctx.upload(PERMA_FRAME, img)
+    of = oracle.Frame(PERMA_FRAME, img, seq.K)
+    scale = dict(zip(run.gs.keyframe_ids, [q[7] for q in run.gs.keyframe_cam_to_world]))
+    ids, inits = [], []
+    for k in prs:
+        gt = seq.frame_to_ref_qt(PERMA_FRAME, ref=k)
+        gt[4:7] /= scale[k]
+        gt_inv = se3_inverse(oracle, gt)
+        for init in (gt_inv, IDENT):
+            ids.append(k)
+            inits.append(init)
+    res = se3.trackFrameOnPermaref(ids, PERMA_FRAME, np.array(inits))
+    n_good = 0
+    for k, init, g in zip(ids, inits, res):
+        noise = perma_noise(oracle, prs[k], of, init) if noise_aware else (0.0, 0.0)
+        n_good += check_perma_track(g, prs[k].track(of, init), noise)
+    assert n_good >= 2
+    ctx.release(PERMA_FRAME)
+
+
+def mapped_adversarial(run, oracle):
+    """the edited map of the active keyframe (pin_cases.adversarial_edit) loaded on both sides (DepthMap setHypotheses +
+    Frame::setDepth): pyramids, permaRef and Sim3 on it.  Points with negative idepth lie behind the camera and can warp into
+    the image mirrored; the reference has no Wz > 0 test in calcSim3Buffers or checkPermaRefOverlap, and neither have the
+    kernels."""
+    ctx, seq = run.ctx, run.seq
+    kf, other = run.active, run.kfs[-1]
+    hyp = adversarial_edit(run.active_hyp, np.random.default_rng(7))
+    run.gs.map.setHypotheses(kf, hyp, do_set_depth=True)
+    okf = oracle.Frame(kf, run.images[kf], seq.K)
+    set_depth(okf, hyp)
+    assert not pyramid_mismatches(ctx, kf, okf)
+    idepth0, valid0 = okf.idepth(0), okf.idepthVar(0) > 0
+    assert ((idepth0 < 0) & valid0).sum() >= 50 and ((idepth0 == 0) & valid0).sum() >= 32
+    for lvl in range(1, abi.LEVELS):                  # the cancelled blocks reach every level
+        assert ((okf.idepth(lvl) == 0) & (okf.idepthVar(lvl) > 0)).any(), lvl
+
+    se3 = abi.SE3Tracker(ctx)
+    pr = oracle.PermaRef(okf)
+    assert se3.setPermaRef(kf) == pr.n
+    check_perma_overlap(se3, oracle, {kf: pr}, np.random.default_rng(5))
+
+    of = dict(run.of)
+    of[kf] = okf
+    trk = abi.Sim3Tracker(ctx)
+    for ref, fr in ((kf, other), (other, kf)):
+        r2f = run.ref_to_frame(oracle, ref, fr)
+        for lvl in range(abi.LEVELS):
+            for a, b in AB:
+                check_sim3_eval(trk.eval(ref, fr, lvl, r2f, a, b), oracle.sim3_eval(of[ref], of[fr], lvl, r2f, a, b))
+        init = run.frame_to_ref(oracle, ref, fr)
+        trk.trackFrameSim3(ref, fr, init, 4, 1)
+        want, exact = oracle_sim3_track(oracle, of[ref], of[fr], init)
+        assert trk.diverged == bool(want.diverged)
+        if not want.diverged:
+            check_sim3_track(trk.last, want)
+            check_sim3_track(trk.last, exact, res_tol=5e-4)
 
 
 # ---- stream groups ------------------------------------------------------------------------------------------------------------

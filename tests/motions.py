@@ -21,8 +21,11 @@ MOTIONS = {
 }
 
 
+DEFAULT = "default"             # the stream's own twist (synth.DEFAULT_XI), the stream of every other pin
+
+
 def sequence(name, w=320, h=240):
-    return synth.Sequence(w, h, seed=SEED, xi=MOTIONS[name])
+    return synth.Sequence(w, h, seed=SEED, xi=synth.DEFAULT_XI if name == DEFAULT else MOTIONS[name])
 
 
 class Frames:

@@ -4,7 +4,8 @@ and hands its observations to a Pin, which records them (to write a golden file)
 
 tests/test_ref_pin.py runs the cases at the reference's default run-time settings on the default stream,
 tests/test_ref_pin_globals.py under the settings of SETS, tests/test_ref_pin_motions.py under the camera motions of
-tests/motions.py (with two more cases only those reach); tests/golden/make_golden*.py record each of them."""
+tests/motions.py (with two more cases only those reach), tests/test_ref_pin_sim3.py runs the Sim3 tracker and the permaRef
+path on keyframes the mapper finished, under every motion; tests/golden/make_golden*.py record each of them."""
 import contextlib
 import ctypes as C
 import hashlib
@@ -530,3 +531,407 @@ def record_motions():
     for m, c in MOTION_PAIRS:
         out.update(run_under_motion(m, c, None).rec)
     return out
+
+
+# ---- Sim3 and permaRef on keyframes the mapper finished (tests/test_ref_pin_sim3.py) ----------------------------------------
+GOLD_SIM3 = os.path.join(GOLDEN, "ref_pin_sim3_320x240.npz")
+
+MAPPED_KF_EVERY = 5
+MAPPED_FRAMES = 16              # keyframe changes at frames 5, 10 and 15: keyframes 0, 5 and 10 finished, 15 active
+PERMA_FRAME = 12                # a frame that is not a keyframe, for trackFrameOnPermaref
+SIM3_DT, SIM3_SCALE = (0.01, -0.005, 0.004), 1.02       # the perturbation of util.sim3_init
+AB = ((1.0, 0.0), (0.97, 1.5))
+SIM3_SETTINGS = dict(var_weight=2.5, huber_d=1.5)        # the one non-default tracker setting set (class defaults: 1, 3)
+OVERLAP_SIGMA = (0.2, 0.2, 0.3, 0.05, 0.05, 0.05)         # util.check_perma_overlap's random poses
+
+# (motion, reference keyframe, frame keyframe, startLevel, finalLevel) of the trackFrameSim3 calls whose lastDepthResidual is
+# ill-conditioned in the final pose.  Under `vertical`, 0 -> 10 over levels 3..2 rejects every level-2 step, so the reported
+# depth residual is that of the last accepted level-3 step (722 depth terms).  A change of the final translation by 7e-6
+# (relative, a tenth of what tree-ordered sums move the device's pose by elsewhere) moves that residual by up to 4.2e-3 relative
+# with no point changing its pixel or its depth status (other calls: 1e-5 to 4e-5, e.g. the reverse pair or the default
+# motion's 0 -> 10); the device's pose lies 7.2e-6 from the exact-affine-sum twin and its
+# depth residual 4.5e-3.  Pivoting the device's 7x7 solve does not change either.  For these calls lastDepthResidual is held to
+# the reference tolerance (2e-2) against the twin as well; every other field keeps its tolerance.
+POSE_SENSITIVE_DEPTH_RESIDUAL = {("vertical", 0, 10, 3, 2)}
+SENSITIVE_TRANSLATION = 7e-6
+
+
+def depth_residual_sensitivity(m, ref, fr, lo, hi, n=50):
+    """-> (largest relative change of the oracle's level-`lo` meanD, largest change of its depth / warped term counts) when the
+    final translation of the exact-affine-sum trackFrameSim3 moves by SENSITIVE_TRANSLATION (relative) in n seeded directions"""
+    init = m.frame_to_ref(ref, fr)
+    set_globals(False, exactAffineSums=1)
+    try:
+        ex = po.sim3_track(m.of[ref], m.of[fr], init, lo, hi)
+    finally:
+        set_globals(False)
+    a, b = ex.affineEstimation_a, ex.affineEstimation_b
+
+    def ev(q):
+        return po.sim3_eval(m.of[ref], m.of[fr], lo, _qts_op("lsdo_sim3d_inverse", 8, q), a, b)
+    base = ev(np.array(ex.frameToRef_qts))
+    rng = np.random.default_rng(0)
+    dmax, cmax = 0.0, 0
+    for _ in range(n):
+        q = np.array(ex.frameToRef_qts)
+        d = rng.normal(size=3)
+        q[4:7] += d * SENSITIVE_TRANSLATION * np.linalg.norm(q[4:7]) / np.linalg.norm(d)
+        e = ev(q)
+        dmax = max(dmax, abs(e.meanD - base.meanD) / base.meanD)
+        cmax = max(cmax, abs(e.numTermsD - base.numTermsD), abs(e.warpedSize - base.warpedSize))
+    return dmax, cmax
+
+
+def _qts_op(fn, n, *args):
+    out = np.zeros(n, np.float64)
+    arrs = [np.ascontiguousarray(a, np.float64) for a in args]
+    getattr(po.lib(False), fn)(*[po._dp(a) for a in arrs], po._dp(out))
+    return out
+
+
+class Mapped:
+    """oracle/cpu_stream.py's loop on one flavour over frames 0..MAPPED_FRAMES-1 with a keyframe every MAPPED_KF_EVERY frames:
+    the finished keyframes' Frames (`of`: id -> Frame), the active keyframe's id and hypotheses, and each keyframe's
+    camToWorld chained in double by the C restatement's Sophus from the C restatement's thisToParent -- on both flavours, so
+    that both start the Sim3 tracker from the same doubles (each flavour's own thisToParent is pinned by _kf_depth)"""
+
+    def __init__(self, fl, seq, frames):
+        from oracle.cpu_stream import CpuStream
+        set_globals(fl)
+        cs = CpuStream(seq, fl, kf_every=MAPPED_KF_EVERY, keep_keyframes=True)
+        cs.init_gt(0, *frames[0])
+        for k in range(1, MAPPED_FRAMES):
+            cs.step(k, frames[k][0])
+        self.seq, self.frames = seq, frames
+        self.of = {f.id: f for f in cs.finished}
+        self.kfs = list(self.of)
+        self.active, self.active_hyp = cs.kf.id, cs.dm.current().copy()
+        self.thisToParent = {f.id: f.thisToParent() for f in cs.finished + [cs.kf]}
+        if fl is not False:                 # the Sim3 starts are computed once, from the C restatement's chain, for both flavours
+            self.c2w = mapped(False, seq, frames).c2w
+            return
+        self.c2w = {}
+        last = np.array([0, 0, 0, 1, 0, 0, 0, 1], np.float64)
+        for f in cs.finished + [cs.kf]:
+            if f.id:
+                last = _qts_op("lsdo_sim3d_mul", 8, last, self.thisToParent[f.id])
+            self.c2w[f.id] = last
+
+    def frame_to_ref(self, ref, fr, perturb=True):
+        q = _qts_op("lsdo_sim3d_mul", 8, _qts_op("lsdo_sim3d_inverse", 8, self.c2w[ref]), self.c2w[fr])
+        if perturb:
+            q[4:7] += SIM3_DT
+            q[7] *= SIM3_SCALE
+        return q
+
+    def ref_to_frame(self, ref, fr, perturb=True):
+        return _qts_op("lsdo_sim3d_inverse", 8, self.frame_to_ref(ref, fr, perturb))
+
+    def pairs(self):
+        return [(a, b) for a in self.kfs for b in self.kfs if a != b]
+
+
+_mapped: dict = {}
+
+
+def mapped(fl, seq, frames):
+    """the Mapped run of (flavour, sequence), made once per process"""
+    key = (fl, id(seq))
+    if key not in _mapped:
+        _mapped[key] = (seq, Mapped(fl, seq, frames))
+    return _mapped[key][1]
+
+
+def sim3_eval_fields(r):
+    """what a Sim3 evaluation returns, as one float64 row: A (49), b (7), num_constraints, numTermsD, numTermsP, warpedSize,
+    sumResD, sumResP, mean, meanD, meanP, pointUsage, affine_a_lastIt, affine_b_lastIt"""
+    return np.concatenate([np.array(r.A, np.float64), np.array(r.b, np.float64),
+                           [r.num_constraints, r.numTermsD, r.numTermsP, r.warpedSize, r.sumResD, r.sumResP, r.mean, r.meanD,
+                            r.meanP, r.pointUsage, r.affine_a_lastIt, r.affine_b_lastIt]])
+
+
+def sim3_track_fields(r):
+    """what trackFrameSim3 returns that the reference exports: the pose (8 doubles), the Hessian (49), lastResidual,
+    lastDepthResidual, lastPhotometricResidual, pointUsage, affineEstimation_a, affineEstimation_b, diverged"""
+    return np.concatenate([np.array(r.frameToRef_qts), np.array(r.lastSim3Hessian, np.float64),
+                           [r.lastResidual, r.lastDepthResidual, r.lastPhotometricResidual, r.pointUsage,
+                            r.affineEstimation_a, r.affineEstimation_b, r.diverged]])
+
+
+def perma_track_fields(r):
+    """what trackFrameOnPermaref returns that the reference exports: referenceToFrame (7 doubles), pointUsage, lastGoodCount,
+    lastBadCount, lastMeanRes, lastResidual, affineEstimation_a, affineEstimation_b, diverged, trackingWasGood"""
+    return np.concatenate([np.array(r.frameToRef_qt), [r.pointUsage, r.lastGoodCount, r.lastBadCount, r.lastMeanRes,
+                                                         r.lastResidual, r.affineEstimation_a, r.affineEstimation_b,
+                                                         r.diverged, r.trackingWasGood]])
+
+
+def _same_pose(pin, what, x, n):
+    """a pose read back from Sophus' non-unit quaternion (its normalisation differs from the restatement's division in the
+    last bits: 1e-12, as tests/test_oracle_kats.py allows), every other field bit for bit as float32 / float64"""
+    y = pin.value(what, x)
+    assert np.allclose(x[:n], y[:n], rtol=0, atol=1e-12), (what, x[:n] - y[:n])
+    assert np.array_equal(x[n:], y[n:]), (what, np.flatnonzero(x[n:] != y[n:]), x[n:], y[n:])
+
+
+def _kf_depth(pin, m):
+    """each finished keyframe's pyramids and its rescaled thisToParent: the input every Sim3 / permaRef call reads"""
+    for k, f in m.of.items():
+        for lvl in range(po.LEVELS):
+            pin.exact(f"kf{k}/idepth{lvl}", _bits(f.idepth(lvl)))
+            pin.exact(f"kf{k}/idepthVar{lvl}", _bits(f.idepthVar(lvl)))
+        _same_pose(pin, f"kf{k}/thisToParent", m.thisToParent[k], 8)
+
+
+def _eval(pin, what, ref, fr, lvl, r2f, a, b, st):
+    r = po.sim3_eval(ref, fr, lvl, r2f, a, b, settings=st)
+    x = sim3_eval_fields(r)
+    y = pin.value(what, x)
+    assert np.array_equal(x, y), (what, np.flatnonzero(x != y), x[x != y], y[x != y])
+    return r
+
+
+def sim3_eval_mapped(pin, fl, seq, frames):
+    """calcSim3Buffers + calcSim3WeightsAndResidual + calcSim3LGS (Sim3Tracker.cpp:414-607, 748-856, 992-1047) for every ordered
+    pair of finished keyframes, levels 4-1, from the chained pose with and without util.sim3_init's perturbation, at two affine
+    estimates; once more on one pair under SIM3_SETTINGS.  Bit for bit."""
+    m = mapped(fl, seq, frames)
+    set_globals(fl)
+    _kf_depth(pin, m)
+    st = po.default_track_settings(fl, main_tracker=False)
+    for ref, fr in m.pairs():
+        for perturb in (True, False):
+            r2f = m.ref_to_frame(ref, fr, perturb)
+            for lvl in (4, 3, 2, 1):
+                for a, b in AB:
+                    r = _eval(pin, f"{ref}->{fr}/p{int(perturb)}/L{lvl}/a{a}", m.of[ref], m.of[fr], lvl, r2f, a, b, st)
+                    assert r.warpedSize > 10
+    for k, v in SIM3_SETTINGS.items():
+        setattr(st, k, v)
+    ref, fr = m.kfs[0], m.kfs[-1]
+    r2f = m.ref_to_frame(ref, fr)
+    for lvl in (4, 3, 2, 1):
+        a, b = AB[lvl % 2]
+        _eval(pin, f"settings/{ref}->{fr}/L{lvl}", m.of[ref], m.of[fr], lvl, r2f, a, b, st)
+
+
+def sim3_track_mapped(pin, fl, seq, frames):
+    """Sim3Tracker::trackFrameSim3 (Sim3Tracker.cpp:149-382) for every ordered pair of finished keyframes, levels 4..1 and 3..2,
+    from the perturbed chained pose"""
+    m = mapped(fl, seq, frames)
+    set_globals(fl)
+    for ref, fr in m.pairs():
+        init = m.frame_to_ref(ref, fr)
+        for lo, hi in ((4, 1), (3, 2)):
+            r = po.sim3_track(m.of[ref], m.of[fr], init, lo, hi)
+            _same_pose(pin, f"{ref}->{fr}/{lo}{hi}", sim3_track_fields(r), 8)
+
+
+def overlap_poses(kfs):
+    """util.check_perma_overlap's five random refToFrame poses per keyframe (seed 3)"""
+    rng = np.random.default_rng(3)
+    return {k: [_qts_op("lsdo_se3d_exp", 7, rng.normal(0, OVERLAP_SIGMA)) for _ in range(5)] for k in kfs}
+
+
+def perma_gt(m, k, frame):
+    """refToFrame of `frame` on keyframe k from ground truth, the translation in the keyframe's map units"""
+    gt = m.seq.frame_to_ref_qt(frame, ref=k)
+    gt[4:7] /= m.c2w[k][7]
+    return _qts_op("lsdo_se3d_inverse", 7, gt)
+
+
+def _perma(pin, fl, m, prs, tag=""):
+    """checkPermaRefOverlap (SE3Tracker.cpp:121-157) at overlap_poses and at the ground-truth pose of PERMA_FRAME, and
+    trackFrameOnPermaref (:162-272) of PERMA_FRAME from ground truth and from identity, on each snapshot of prs"""
+    f = po.Frame(PERMA_FRAME, m.frames[PERMA_FRAME][0], m.seq.K, fast=fl)
+    poses = overlap_poses(prs)
+    for k, pr in prs.items():
+        gt = perma_gt(m, k, PERMA_FRAME)
+        ov = np.array([pr.overlap(q) for q in poses[k] + [gt]], np.float32)
+        pin.exact(f"{tag}kf{k}/overlap", _bits(ov))
+        pin.value(f"{tag}kf{k}/overlap_values", ov)
+        for name, init in (("gt", gt), ("identity", IDENT)):
+            _same_pose(pin, f"{tag}kf{k}/track_{name}", perma_track_fields(pr.track(f, init)), 7)
+
+
+def perma_mapped(pin, fl, seq, frames):
+    """Frame::setPermaRef of each finished keyframe (the snapshot bit for bit), then the overlap check and the tracking on it"""
+    m = mapped(fl, seq, frames)
+    set_globals(fl)
+    prs = {}
+    for k, f in m.of.items():
+        prs[k] = pr = po.PermaRef(f)
+        assert pr.n > 30
+        pin.exact(f"kf{k}/snapshot_pos", _bits(pr.pos[:pr.n]))
+        pin.exact(f"kf{k}/snapshot_colvar", _bits(pr.colvar[:pr.n]))
+    _perma(pin, fl, m, prs)
+
+
+def adversarial_edit(hyp, rng):
+    """A real map with a few hundred pixels edited to the value edges of Frame::setDepth, the idepth pyramid and
+    makePointCloud:
+      * for every pyramid level L = 1..4, aligned 2^L x 2^L blocks whose left half holds +a and right half -a with one
+        variance: the level-(L-1) pixels of the block are exact negatives of each other, so the inverse-variance weighted
+        sum is exactly 0 at level L and the pyramid gives 1 / (ivarSum / 0) = 0 there (Frame.cpp:862-864); in a third
+        block per level the negative side is one ulp larger, which leaves a tiny idepth (a point very far away);
+      * idepths in [-0.05, 0) (kept by the gate of Frame.cpp:219; the floats at and below -0.05 are dropped by it);
+      * idepth exactly 0.0 and -0.0 with a valid variance (skipped as points, TrackingReference.cpp:133);
+      * runs of five neighbouring pixels with variances 1e-7, 1e-5, 1e-3, 1e-1, 1e1.
+    Only valid pixels are read or written, so the uninitialised fields of the reference's invalid pixels do not matter."""
+    hyp = hyp.copy()
+    h, w = hyp.shape
+    free = np.zeros((h, w), bool)                    # interior pixels no edit has touched yet
+    free[2:-2, 2:-2] = True
+    typical = np.float32(np.median(hyp["idepth_smoothed"][hyp["isValid"] > 0]))
+
+    def put(ys, xs, idepth, var=None):
+        hyp["isValid"][ys, xs] = 1
+        hyp["blacklisted"][ys, xs] = 0
+        for f in ("idepth", "idepth_smoothed"):
+            hyp[f][ys, xs] = idepth
+        if var is not None:
+            for f in ("idepth_var", "idepth_var_smoothed"):
+                hyp[f][ys, xs] = var
+        free[ys, xs] = False
+
+    for lvl in range(po.LEVELS - 1, 0, -1):
+        s = 1 << lvl
+        by, bx = h // s, w // s
+        ok = free[:by * s, :bx * s].reshape(by, s, bx, s).all(axis=(1, 3)).ravel()
+        for j, i in enumerate(rng.choice(np.flatnonzero(ok), 3, replace=False)):
+            y0, x0 = (int(i) // bx) * s, (int(i) % bx) * s
+            a = np.float32(rng.uniform(0.005, 0.05))
+            b = -a if j < 2 else -np.nextafter(a, np.float32(1))
+            var = np.float32(10.0 ** rng.uniform(-4, -1))
+            put(slice(y0, y0 + s), slice(x0, x0 + s // 2), a, var)
+            put(slice(y0, y0 + s), slice(x0 + s // 2, x0 + s), b, var)
+
+    def pick(n):
+        ys, xs = np.nonzero(free & (hyp["isValid"] > 0))
+        i = rng.choice(ys.size, n, replace=False)
+        return ys[i], xs[i]
+
+    ys, xs = pick(64)
+    neg = rng.uniform(-0.0499, -1e-4, 64).astype(np.float32)
+    neg[:4] = [np.nextafter(np.float32(-0.05), np.float32(0)), np.float32(-1e-6), np.float32(-0.05), np.float32(-0.06)]
+    put(ys, xs, neg)
+    ys, xs = pick(32)
+    put(ys, xs, np.where(np.arange(32) % 2 == 0, np.float32(0.0), np.float32(-0.0)).astype(np.float32))
+    runs = 0
+    for y, x in zip(*pick(80)):
+        x = min(max(x - x % 2, 2), w - 8)
+        if runs < 40 and free[y, x:x + 5].all():
+            put(y, slice(x, x + 5), typical, np.float32([1e-7, 1e-5, 1e-3, 1e-1, 1e1]))
+            runs += 1
+    assert runs == 40
+    return hyp
+
+
+def set_depth(frame, hyp):
+    """Frame::setDepth (Frame.cpp:199-243) of a hypothesis map"""
+    h = np.ascontiguousarray(hyp, po.HYP_DTYPE)
+    frame.L.lsdo_frame_setDepth(frame.ptr, h.ctypes.data_as(C.POINTER(po.Hyp)))
+
+
+def adversarial_keyframe(fl, m):
+    """the active keyframe's image with adversarial_edit (seed 7) of its hypotheses loaded through Frame::setDepth"""
+    hyp = adversarial_edit(m.active_hyp, np.random.default_rng(7))
+    f = po.Frame(m.active, m.frames[m.active][0], m.seq.K, fast=fl)
+    set_depth(f, hyp)
+    return f, hyp
+
+
+def adversarial_map(pin, fl, seq, frames):
+    """adversarial_keyframe: its pyramids, then permaRef and Sim3 on it (both directions against the last finished keyframe, the
+    active keyframe's chained pose).  Points with negative idepth lie behind the camera and can warp into the image mirrored;
+    the reference has no Wz > 0 test in calcSim3Buffers or checkPermaRefOverlap."""
+    m = mapped(fl, seq, frames)
+    set_globals(fl)
+    okf, _ = adversarial_keyframe(fl, m)
+    for lvl in range(po.LEVELS):
+        pin.exact(f"idepth{lvl}", _bits(okf.idepth(lvl)))
+        pin.exact(f"idepthVar{lvl}", _bits(okf.idepthVar(lvl)))
+    idepth0, valid0 = okf.idepth(0), okf.idepthVar(0) > 0
+    assert ((idepth0 < 0) & valid0).sum() >= 50 and ((idepth0 == 0) & valid0).sum() >= 32
+    for lvl in range(1, po.LEVELS):                  # the cancelled blocks reach every level
+        assert ((okf.idepth(lvl) == 0) & (okf.idepthVar(lvl) > 0)).any(), lvl
+    pr = po.PermaRef(okf)
+    pin.exact("snapshot_pos", _bits(pr.pos[:pr.n]))
+    pin.exact("snapshot_colvar", _bits(pr.colvar[:pr.n]))
+    _perma(pin, fl, m, {m.active: pr})
+    of = dict(m.of)
+    of[m.active] = okf
+    other = m.kfs[-1]
+    st = po.default_track_settings(fl, main_tracker=False)
+    for ref, fr in ((m.active, other), (other, m.active)):
+        r2f = m.ref_to_frame(ref, fr)
+        for lvl in range(po.LEVELS):
+            for a, b in AB:
+                _eval(pin, f"{ref}->{fr}/L{lvl}/a{a}", of[ref], of[fr], lvl, r2f, a, b, st)
+        r = po.sim3_track(of[ref], of[fr], m.frame_to_ref(ref, fr), 4, 1)
+        _same_pose(pin, f"{ref}->{fr}/track", sim3_track_fields(r), 8)
+
+
+# case -> (function, C-restatement flavour, reference-compiled flavour), as CASES
+SIM3_CASES = {
+    "sim3_eval_mapped": (sim3_eval_mapped, False, "ref"),
+    "sim3_track_mapped": (sim3_track_mapped, False, "ref"),
+    "perma_mapped": (perma_mapped, False, "ref"),
+    "adversarial_map": (adversarial_map, False, "ref"),
+}
+SIM3_ONLY = {"adversarial_map": (motions.DEFAULT, "forward")}
+SIM3_MOTIONS = (motions.DEFAULT,) + tuple(motions.MOTIONS)
+SIM3_PAIRS = [(m, c) for m in SIM3_MOTIONS for c in SIM3_CASES if m in SIM3_ONLY.get(c, (m,))]
+
+
+def run_sim3(motion, case, gold):
+    """runs one case under one motion on the C restatement (gold = the record) or on the reference-compiled library
+    (gold = None); returns the case's Pin"""
+    fn, fl, ref_fl = SIM3_CASES[case]
+    fl = ref_fl if gold is None else fl
+    seq, frames = motions.stream(motion)
+    p = Pin(f"{motion}/{case}", gold)
+    try:
+        fn(p, fl, seq, frames)
+    finally:
+        po.set_globals(fl)
+    return p
+
+
+def record_sim3():
+    """every (motion, case) on the reference-compiled library (needs oracle/_ref): the arrays of ref_pin_sim3_320x240.npz"""
+    out = {}
+    for m, c in SIM3_PAIRS:
+        out.update(run_sim3(m, c, None).rec)
+    return out
+
+
+def sim3_eval_result(row) -> po.Sim3EvalResult:
+    """the recorded sim3_eval_fields row as the struct the checks of tests/util.py read"""
+    r = po.Sim3EvalResult()
+    r.A[:], r.b[:] = [float(x) for x in row[:49]], [float(x) for x in row[49:56]]
+    (r.num_constraints, r.numTermsD, r.numTermsP, r.warpedSize) = (int(x) for x in row[56:60])
+    (r.sumResD, r.sumResP, r.mean, r.meanD, r.meanP, r.pointUsage, r.affine_a_lastIt, r.affine_b_lastIt) = row[60:68]
+    return r
+
+
+def sim3_track_result(row, calls) -> po.Sim3Result:
+    """the recorded sim3_track_fields row as a Sim3Result, with the LM call counters (locals in the reference) of `calls`"""
+    r = po.Sim3Result()
+    r.frameToRef_qts[:], r.lastSim3Hessian[:] = [float(x) for x in row[:8]], [float(x) for x in row[8:57]]
+    (r.lastResidual, r.lastDepthResidual, r.lastPhotometricResidual, r.pointUsage, r.affineEstimation_a,
+     r.affineEstimation_b) = row[57:63]
+    r.diverged = int(row[63])
+    r.numCalcResidualCalls[:], r.numCalcWarpUpdateCalls[:] = list(calls.numCalcResidualCalls), list(calls.numCalcWarpUpdateCalls)
+    return r
+
+
+def perma_track_result(row, calls) -> po.TrackResult:
+    """the recorded perma_track_fields row as a TrackResult, with the LM call counters (not counted in the reference) of `calls`"""
+    r = po.TrackResult()
+    r.frameToRef_qt[:] = [float(x) for x in row[:7]]
+    (r.pointUsage, r.lastGoodCount, r.lastBadCount, r.lastMeanRes, r.lastResidual, r.affineEstimation_a,
+     r.affineEstimation_b) = row[7:14]
+    r.diverged, r.trackingWasGood = int(row[14]), int(row[15])
+    r.numCalcResidualCalls[:], r.numCalcWarpUpdateCalls[:] = list(calls.numCalcResidualCalls), list(calls.numCalcWarpUpdateCalls)
+    return r

@@ -237,9 +237,9 @@ def check_sim3_eval(got, want):
     assert abs(got.affine_b_lastIt - want.affine_b_lastIt) <= 2e-2
 
 
-def check_sim3_track(got, want, res_tol=2e-2):
+def check_sim3_track(got, want, res_tol=2e-2, depth_res_tol=None):
     """Sim3Tracker::trackFrameSim3: outcome and LM call counters exactly, pose and scale to POSE_TOL, the Hessian, the residuals
-    to `res_tol` and the affine estimate in proportion"""
+    to `res_tol` (lastDepthResidual to `depth_res_tol` where the caller gives one) and the affine estimate in proportion"""
     assert got.diverged == want.diverged
     assert list(got.numCalcResidualCalls) == list(want.numCalcResidualCalls)
     assert list(got.numCalcWarpUpdateCalls) == list(want.numCalcWarpUpdateCalls)
@@ -248,7 +248,8 @@ def check_sim3_track(got, want, res_tol=2e-2):
     H, Hw = np.array(got.lastSim3Hessian), np.array(want.lastSim3Hessian)
     assert np.abs(H - Hw).max() <= 1e-3 * np.abs(Hw).max()
     for f in ("lastResidual", "lastDepthResidual", "lastPhotometricResidual"):
-        assert abs(getattr(got, f) - getattr(want, f)) <= res_tol * abs(getattr(want, f)) + 1e-7, f
+        tol = depth_res_tol if f == "lastDepthResidual" and depth_res_tol is not None else res_tol
+        assert abs(getattr(got, f) - getattr(want, f)) <= tol * abs(getattr(want, f)) + 1e-7, f
     assert abs(got.pointUsage - want.pointUsage) <= 1e-3 * want.pointUsage
     assert abs(got.affineEstimation_a - want.affineEstimation_a) <= 0.25 * res_tol
     assert abs(got.affineEstimation_b - want.affineEstimation_b) <= 25 * res_tol
@@ -272,14 +273,15 @@ def oracle_sim3_track(oracle, ref, fr, init, lo=4, hi=1, g=None):
 
 
 # ---- permaRef -----------------------------------------------------------------------------------------------------------------
-def check_perma_track(g, o):
-    """one trackFrameOnPermaref result against the oracle's: the outcome; unless diverged the pose, the LM call counters, the
-    residual, trackingWasGood and the point usage.  -> whether the oracle's tracking was good"""
+def check_perma_track(g, o, noise=(0.0, 0.0)):
+    """one trackFrameOnPermaref result against the oracle's: the outcome; unless diverged the pose (to POSE_TOL and PERMA_ANG_TOL
+    plus the caller's (translation, rotation) `noise`), the LM call counters, the residual, trackingWasGood and the point usage.
+    -> whether the oracle's tracking was good"""
     assert bool(g.diverged) == bool(o.diverged)
     if o.diverged:
         return False
     dt, ang = pose_err(np.array(g.frameToRef_qt), np.array(o.frameToRef_qt))
-    assert dt <= POSE_TOL and ang <= PERMA_ANG_TOL, (dt, ang)
+    assert dt <= POSE_TOL + noise[0] and ang <= PERMA_ANG_TOL + noise[1], (dt, ang, noise)
     assert list(g.numCalcResidualCalls) == list(o.numCalcResidualCalls)
     assert list(g.numCalcWarpUpdateCalls) == list(o.numCalcWarpUpdateCalls)
     assert abs(g.lastResidual - o.lastResidual) <= 1e-3 * abs(o.lastResidual) + 1e-6
@@ -300,6 +302,19 @@ def check_perma_overlap(se3, oracle, prs, rng):
     want = np.array([prs[k].overlap(q) for k, q in zip(ids, poses)], np.float32)
     assert np.allclose(got, want, rtol=OVERLAP_RTOL, atol=OVERLAP_ATOL), np.abs(got - want).max()
     return want
+
+
+def perma_noise(oracle, pr, frame, init):
+    """the reference's own summation noise in one trackFrameOnPermaref: (translation, rotation) pose_err between its sequential
+    fp32 sums and the same tracking with exact sums (lsdo_globals.exactTrackingSums).  On mapped keyframes under camera motion
+    it reaches 8e-6 rad, four times PERMA_ANG_TOL"""
+    a = pr.track(frame, init)
+    oracle.set_globals(exactTrackingSums=1)
+    try:
+        b = pr.track(frame, init)
+    finally:
+        oracle.set_globals()
+    return pose_err(np.array(a.frameToRef_qt), np.array(b.frameToRef_qt))
 
 
 # ---- closed loops replayed on the oracle (oracle/replay.py) ----------------------------------------------------------------
