@@ -249,7 +249,7 @@ void lsdo_depthmap_propagateDepth(lsdo_depthmap* d, lsdo_frame* new_kf);
 void lsdo_ref_prepareForStereoWith(lsdo_frame* frame, lsdo_frame* kf, const double thisToOther_qts[8], const float K[9], float out[30]);
 /* per-stage EMA timers of the reference (DepthMap.cpp:1126-1162), ms of the last call */
 void lsdo_depthmap_last_timings(const lsdo_depthmap* d, float out_ms[8]);
-/* diagnostic branch counters of doLineStereo and propagateDepth, summed over every depth map of the process (C restatement only:
+/* diagnostic branch counters of doLineStereo, observeDepth and propagateDepth, summed over every depth map of the process (C restatement only:
  * they show which branches a test reaches; no float is read or written by them) */
 enum {
     LSDO_BR_DEPTH_X,          /* x-dominant depth formula, DepthMap.cpp:1876-1886 */
@@ -264,6 +264,15 @@ enum {
     LSDO_BR_PROP_INVALIDATE,  /* propagateDepth: target replaced by a nearer source, :600 */
     LSDO_BR_PROP_MERGE,       /* propagateDepth: source merged into a consistent target, :619-631 */
     LSDO_BR_PROP_MERGE_CAP,   /* propagateDepth: merged validity capped, :626-627 */
+    LSDO_BR_STEREO_ERR_SEARCH,  /* doLineStereo -3: best match error of the search above 4 MAX_ERROR_STEREO, :1750-1754 */
+    LSDO_BR_STEREO_ERR_INTERP,  /* doLineStereo -3: interpolated error above the gradient-dependent bound, :1861-1865 */
+    LSDO_BR_STEREO_UNCLEAR,     /* doLineStereo -2: no clear winner, :1758-1762 */
+    LSDO_BR_STEREO_NEGATIVE,    /* doLineStereo -2: negative idepth with allowNegativeIdepths off, :1903-1908 */
+    LSDO_BR_UPDATE_FAIL_INVALIDATE,  /* observeDepthUpdate on -2: variance inflated above MAX_VAR, invalidated, :381-385 */
+    LSDO_BR_UPDATE_INCONSISTENT,     /* observeDepthUpdate: inconsistent observation, variance inflated, :410-417 */
+    LSDO_BR_CREATE_BLACKLIST,   /* observeDepthCreate: blacklisted-- on -3 or -2, :269-273 */
+    LSDO_BR_PROP_MASK,          /* propagateDepth: source dropped by the tracking mask, :550-555 */
+    LSDO_BR_PROP_COLOR,         /* propagateDepth without a mask: source dropped by the colour difference, :559-569 */
     LSDO_BR_COUNT
 };
 void lsdo_depth_branch_counts(int64_t out[LSDO_BR_COUNT]);

@@ -233,11 +233,14 @@ def default_track_settings(fast=False, main_tracker: bool = True) -> TrackSettin
 # the diagnostic branch counters of the C restatement's depth map, in the order of lsd_oracle.h's LSDO_BR_* enum
 BRANCHES = ("depth_x", "depth_y", "firstx_gate", "rescale_gate", "near_clamp", "epl_crop",
             "clip_left", "clip_right", "clip_top", "clip_bottom", "subpixel_pre", "subpixel_post", "subpixel_none",
-            "prop_skip", "prop_invalidate", "prop_merge", "prop_merge_cap")
+            "prop_skip", "prop_invalidate", "prop_merge", "prop_merge_cap",
+            "stereo_err_search", "stereo_err_interp", "stereo_unclear", "stereo_negative",
+            "update_fail_invalidate", "update_inconsistent", "create_blacklist", "prop_mask", "prop_color")
 
 
 def branch_counts(fast=False) -> dict:
-    """how often each branch of doLineStereo and propagateDepth ran since the last reset, over every depth map of the process"""
+    """how often each branch of doLineStereo, observeDepth and propagateDepth ran since the last reset, over every depth map of
+    the process"""
     out = np.zeros(len(BRANCHES), np.int64)
     lib(fast).lsdo_depth_branch_counts(out.ctypes.data_as(C.POINTER(C.c_int64)))
     return dict(zip(BRANCHES, out.tolist()))

@@ -78,6 +78,59 @@ def update_keyframe_sequence(ctx, oracle, seq, frames):
         kf_depth_equal(ctx, p.okf, 0)
 
 
+def fill_holes_and_regularize_observed(ctx, oracle, seq, frames):
+    """the passes of depthmap_individual_passes, on the map one observeDepth of the stream left"""
+    p = Pair(ctx, oracle, seq, frames, "gt")
+    ofs = [p.add_frame(k) for k in (2, 3)]
+    p.sync_counters()
+    p.odm.observeDepth(ofs)
+    p.gdm.observeDepth([2, 3])
+    assert p.compare(exact=True)["n_valid"] > 10000
+    p.odm.regularizeFillHoles()
+    p.gdm.regularizeFillHoles()
+    p.compare(exact=True)
+    assert np.array_equal(p.gdm.integral(), p.odm.integral())
+    for occl in (False, True):
+        p.odm.regularize(occl, 24)
+        p.gdm.regularize(occl, 24)
+        p.compare(exact=True)
+
+
+def propagate_and_create_keyframe_device_mask(ctx, oracle, seq, frames):
+    """propagate_and_create_keyframe with the tracking mask, from identical inputs: each frame is tracked on the device and its
+    good mask is handed to the oracle, as oracle/replay.py does.  propagate_and_create_keyframe's with-mask variant lets each
+    side use its own tracker's mask; the two masks differ on up to 1e-3 of the pixels (test_gpu_track.py), and under the backward
+    and roll motions those pixels move the regularised depth of their neighbours after createKeyFrame by up to 1.1e-3, beyond
+    the 2e-5 it allows.  With the same mask on both sides every step is bit for bit."""
+    p = tracked_pair(ctx, oracle, seq, frames, [2, 5, 9])
+    trk = abi.SE3Tracker(ctx, mode=0)
+    for k in (2, 5, 9):
+        of = p.oframes[k]
+        oracle.lib().lsdo_frame_set_depthHasBeenUpdatedFlag(p.okf.ptr, 0)
+        ctx.L.lsdgpu_ref_import(ctx.ptr, 0)
+        trk.trackFrame(0, k, IDENT if k == 2 else of.thisToParent()[:7])        # writes the device's mask; the pose is restored
+        ctx.set_pose(k, of.thisToParent(), 0, oracle.lib().lsdo_frame_initialTrackedResidual(of.ptr))
+        mask = ctx.download(k, abi.BUF_GOODMASK)
+        assert mask.mean() > 0.05
+        of.refPixelWasGood(create=True)[:] = mask
+        p.sync_counters()
+        p.odm.updateKeyframe([of])
+        p.gdm.updateKeyframe([k])
+        p.compare(exact=True)
+    before = p.odm.current().copy()
+    p.odm.propagateDepth(p.oframes[9])
+    p.gdm.propagateDepth(9)
+    assert p.compare(exact=True)["n_valid"] > 5000
+    p.odm.set_current(before)
+    p.gdm.setHypotheses(0, before, do_set_depth=False)
+    p.odm.createKeyFrame(p.oframes[9])
+    q = p.gdm.createKeyFrame(9)
+    assert np.allclose(q[:7], p.oframes[9].thisToParent()[:7], atol=1e-12)
+    assert np.float32(q[7]).tobytes() == np.float32(p.oframes[9].thisToParent()[7]).tobytes()
+    p.compare(exact=True)
+    assert np.array_equal(ctx.download(9, abi.BUF_IDEPTH, 0), p.oframes[9].idepth(0))
+
+
 def finalize_create_and_refs(ctx, oracle, seq, frames_in):
     """finalizeKeyFrame + createKeyFrame (propagation, rescale) and then update_keyframe_refs with frames tracked on the previous
     keyframe -- the scene at mean inverse depth 1 on keyframe 0, as in the pin's create_keyframe_and_finalize"""
@@ -215,14 +268,16 @@ def se3_eval_each_level(ctx, oracle, seq, frames, mask_tol=1e-4, sum_noise=False
                 assert (ctx.download(3, abi.BUF_GOODMASK) != of.refPixelWasGood()).mean() < mask_tol
 
 
-def se3_track(ctx, oracle, seq, frames, mode, k, sum_noise=False, diverges=False):
-    """trackFrame of frame k on keyframe 0 from identity, checked by check_se3_track.  sum_noise: the pose may also differ by the
-    reference's own summation noise, its distance to the same tracking with exact sums"""
+def se3_track(ctx, oracle, seq, frames, mode, k, sum_noise=False, diverges=False, usage_points=0):
+    """trackFrame of frame k on keyframe 0 from identity, checked by check_se3_track.  sum_noise: the pose and the point usage may
+    also differ by the reference's own summation noise, their distance to the same tracking with exact sums (the point usage also
+    by how much it moves between the oracle's final pose and the device's); usage_points: the point usage may also differ by that
+    many level-1 points' worth (1 / refNum each)"""
     okf, of = se3_setup(ctx, oracle, seq, frames, k)
     trk = abi.SE3Tracker(ctx, mode=mode)
     pose_g = trk.trackFrame(0, k, IDENT)
     r = oracle.se3_track(okf, of, IDENT)
-    noise = (0.0, 0.0)
+    noise, usage_noise = (0.0, 0.0), 0.0
     if sum_noise:
         g = ctx.get_globals()
         oracle.set_globals(exactTrackingSums=1, **g)
@@ -233,7 +288,18 @@ def se3_track(ctx, oracle, seq, frames, mode, k, sum_noise=False, diverges=False
         finally:
             oracle.set_globals(**g)
         noise = pose_err(np.array(r.frameToRef_qt), np.array(rx.frameToRef_qt))
-    check_se3_track(ctx, trk, k, pose_g, r, of, diverges=diverges, noise=noise)
+        # the point usage at the device's pose against the oracle's, both at the oracle's (a, b): how far it moves over the pose gap
+        fk = oracle.Frame(k, frames[k][0], seq.K)
+        at = [oracle.se3_eval(okf, fk, 1, se3_inverse(oracle, q).astype(np.float32), r.affineEstimation_a,
+                              r.affineEstimation_b).pointUsage for q in (pose_g, np.array(r.frameToRef_qt))]
+        usage_noise = abs(r.pointUsage - rx.pointUsage) + abs(at[0] - at[1])
+    if usage_points:
+        # the reported point usage is that of the LAST evaluated pose, a rejected candidate whenever level 1 ends on a step below
+        # stepSizeMin (SE3Tracker.cpp:432-441); that candidate is the final pose plus a step solved from each side's own sums,
+        # so a point at the image border can be inside for one side and outside for the other.  Each such point moves the usage
+        # by up to 1 / refNum, as it moves the good / bad counts check_se3_track holds to 2.
+        usage_noise += usage_points / len(okf.point_cloud(1)[0])
+    check_se3_track(ctx, trk, k, pose_g, r, of, diverges=diverges, noise=noise, usage_noise=usage_noise)
 
 
 # ---- Sim3 tracker -------------------------------------------------------------------------------------------------------------
@@ -563,26 +629,27 @@ GROUP_KF_EVERY = 20
 _group_frames = {}
 
 
-def _group_sequence(w, h, s, n):
-    """stream s: its own synthetic sequence (seed 1234 + 1000 s, as scripts/bench_streams.py)"""
-    key = (w, h, s)
+def _group_sequence(w, h, s, n, make=None):
+    """stream s: its own synthetic sequence (seed 1234 + 1000 s, as scripts/bench_streams.py), or make(w, h) if given"""
+    key = (w, h, s, make)
     seq, fr = _group_frames.get(key, (None, []))
     if seq is None:
-        seq = synth.Sequence(w, h, seed=1234 + 1000 * s)
+        seq = make(w, h) if make else synth.Sequence(w, h, seed=1234 + 1000 * s)
     while len(fr) < n:
         fr.append(seq.render(len(fr)))
     _group_frames[key] = (seq, fr)
     return seq, fr
 
 
-def run_streams(w, h, phases, n_steps, grouped, before_step=None):
+def run_streams(w, h, phases, n_steps, grouped, before_step=None, sequences=None):
     """one GpuStream per phase (keyframe every GROUP_KF_EVERY frames, shifted by its phase), stepped n_steps times.
+    sequences: per stream a function (w, h) -> sequence to use instead of its own seeded one.
     grouped(k): step k is one group call (True) or one single call per stream (False).  before_step(k, streams) may change
     the streams' state first.  Returns per step and stream what util.observe saw, whether the step diverged and whether it
     changed keyframe."""
     streams, frames = [], []
     for s, ph in enumerate(phases):
-        seq, fr = _group_sequence(w, h, s, n_steps + 1)
+        seq, fr = _group_sequence(w, h, s, n_steps + 1, sequences[s] if sequences else None)
         ctx = abi.Context(w, h, seq.K, max_frames=8)
         gs = GpuStream(ctx, mode=1, kf_every=GROUP_KF_EVERY, kf_phase=ph)
         gs.init_gt(0, fr[0][0], fr[0][1])

@@ -5,7 +5,8 @@ and hands its observations to a Pin, which records them (to write a golden file)
 tests/test_ref_pin.py runs the cases at the reference's default run-time settings on the default stream,
 tests/test_ref_pin_globals.py under the settings of SETS, tests/test_ref_pin_motions.py under the camera motions of
 tests/motions.py (with two more cases only those reach), tests/test_ref_pin_sim3.py runs the Sim3 tracker and the permaRef
-path on keyframes the mapper finished, under every motion; tests/golden/make_golden*.py record each of them."""
+path on keyframes the mapper finished, under every motion, tests/test_ref_pin_photometry.py runs cases under the exposure
+schedules of tests/photometry.py; tests/golden/make_golden*.py record each of them."""
 import contextlib
 import ctypes as C
 import hashlib
@@ -14,7 +15,7 @@ import os
 import numpy as np
 
 from oracle import pyoracle as po
-from tests import motions
+from tests import motions, photometry
 from tests.util import IDENT, pose_err
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -286,9 +287,10 @@ def create_keyframe_and_finalize(pin, fl, seq, frames_in):
     pin.hyp("updateKeyframe with mixed tracking parents", s.dm.current())
 
 
-def se3_single_evaluation(pin, fl, seq, frames):
+def se3_single_evaluation(pin, fl, seq, frames, affines=((1.0, 0.0),)):
     """calcResidualAndBuffers + calcWeightsAndResidual + calculateWarpUpdate (SE3Tracker.cpp:885-1029, 749-790,
-    1258-1299, LGSX.h:184-402), the reference's private members called directly"""
+    1258-1299, LGSX.h:184-402), the reference's private members called directly, at the ground-truth pose of frame 3 and each
+    affine estimate (a, b) of `affines` (the first one's observations carry no prefix)"""
     set_globals(fl)
     kf = po.Frame(0, frames[0][0], seq.K, fast=fl)
     kf.setDepthFromGroundTruth(frames[0][1])
@@ -297,22 +299,27 @@ def se3_single_evaluation(pin, fl, seq, frames):
     g = np.ascontiguousarray(seq.frame_to_ref_qt(3), np.float64)
     po.lib(False).lsdo_se3d_inverse(g.ctypes.data_as(C.POINTER(C.c_double)), inv.ctypes.data_as(C.POINTER(C.c_double)))
     pose = inv.astype(np.float32)
+    for i, (a, b) in enumerate(affines):
+        _se3_eval_levels(pin, fl, kf, f, pose, a, b, "" if i == 0 else f"a{a:g}_b{b:g}/")
+
+
+def _se3_eval_levels(pin, fl, kf, f, pose, a, b, tag):
     names = ("meanUnweightedRes", "meanWeightedRes", "lsError", "meanRes", "affine_a_lastIt", "affine_b_lastIt")
     for lvl in (4, 3, 2, 1):
-        ra = po.se3_eval(kf, f, lvl, pose, 1.0, 0.0, po.default_track_settings(fl), write_mask=(lvl == 1))
+        ra = po.se3_eval(kf, f, lvl, pose, a, b, po.default_track_settings(fl), write_mask=(lvl == 1))
         counts = np.array([ra.warpedSize, ra.goodCount, ra.badCount, ra.pointUsage], np.float64)
-        cb = pin.value(f"L{lvl}/counts", counts)
+        cb = pin.value(f"{tag}L{lvl}/counts", counts)
         assert counts[0] == cb[0] > 50
         assert np.array_equal(counts[1:], cb[1:]), (lvl, counts, cb)
         x = np.array([getattr(ra, n) for n in names], np.float64)
-        y = pin.value(f"L{lvl}/scalars", x)
-        for n, xi, yi in zip(names, x, y):
-            assert abs(xi - yi) <= 2e-6 * max(abs(yi), 1.0), (lvl, n, xi, yi)
-        A, B = np.array(ra.A), pin.value(f"L{lvl}/A", np.array(ra.A))
+        y = pin.value(f"{tag}L{lvl}/scalars", x)
+        for n, xi, yi in zip(names, x, y):       # no good point: the mean over the good points is 0/0 on both sides
+            assert abs(xi - yi) <= 2e-6 * max(abs(yi), 1.0) or (np.isnan(xi) and np.isnan(yi)), (lvl, n, xi, yi)
+        A, B = np.array(ra.A), pin.value(f"{tag}L{lvl}/A", np.array(ra.A))
         assert np.abs(A - B).max() <= 2e-6 * np.abs(B).max(), lvl
-        b, bb = np.array(ra.b), pin.value(f"L{lvl}/b", np.array(ra.b))
-        assert np.abs(b - bb).max() <= 2e-6 * np.abs(bb).max() + 1e-9, lvl
-    pin.exact("mask", f.refPixelWasGood(create=False) != 0)
+        bv, bb = np.array(ra.b), pin.value(f"{tag}L{lvl}/b", np.array(ra.b))
+        assert np.abs(bv - bb).max() <= 2e-6 * np.abs(bb).max() + 1e-9, lvl
+    pin.exact(f"{tag}mask", f.refPixelWasGood(create=False) != 0)
 
 
 def _se3_track_sequence(pin, fl, seq, frames, exact):
@@ -935,3 +942,68 @@ def perma_track_result(row, calls) -> po.TrackResult:
     r.diverged, r.trackingWasGood = int(row[14]), int(row[15])
     r.numCalcResidualCalls[:], r.numCalcWarpUpdateCalls[:] = list(calls.numCalcResidualCalls), list(calls.numCalcWarpUpdateCalls)
     return r
+
+
+# ---- exposure changes (tests/photometry.py) -----------------------------------------------------------------------------------
+GOLD_PHOTOMETRY = os.path.join(GOLDEN, "ref_pin_photometry_320x240.npz")
+
+FAR_AFFINE = (1.4, -20.0)       # an affine estimate far from every schedule's truth at frame 3
+
+
+def eval_affines(seq):
+    """se3_single_evaluation's affine estimates under an exposure schedule: the identity, frame 3's true (a, b), FAR_AFFINE"""
+    return ((1.0, 0.0), tuple(round(float(x), 6) for x in seq.affine(3)), FAR_AFFINE)
+
+
+def se3_eval_exposure(pin, fl, seq, frames):
+    """se3_single_evaluation at the affine estimates of eval_affines: counts, statistics, normal equations and the level-1 mask"""
+    se3_single_evaluation(pin, fl, seq, frames, affines=eval_affines(seq))
+
+
+def propagation_exposure(pin, fl, seq, frames):
+    """propagateDepth of the ground-truth map to frame PROPAGATION_FRAME at its true pose, without a tracking mask (the colour
+    check of DepthMap.cpp:559-569 compares raw intensities, so a change of exposure drops sources) and with one (:550-555)"""
+    k = PROPAGATION_FRAME
+    mask = (np.random.default_rng(8).random((seq.h // 2, seq.w // 2)) > 0.15).astype(np.uint8)
+    for what, m in (("no mask", None), ("mask", mask)):
+        s = Side(seq, frames, fl, "gt")
+        s.add_frame(k, _gt_qts(seq, k), mask=m)
+        s.dm.propagateDepth(s.fr[k])
+        assert pin.hyp(f"propagateDepth[{k}] {what}", s.dm.current()) > 5000
+
+
+# case -> (function, C-restatement flavour, reference-compiled flavour), as CASES
+PHOTOMETRY_CASES = {c: CASES[c] for c in DEPTH}
+PHOTOMETRY_CASES["propagation_exposure"] = (propagation_exposure, False, "ref")
+PHOTOMETRY_CASES["se3_eval_exposure"] = (se3_eval_exposure, False, "ref")
+PHOTOMETRY_CASES["se3_track_scalar"] = CASES["se3_track_scalar"]
+PHOTOMETRY_CASES["bench_loop_with_keyframe_changes"] = CASES["bench_loop_with_keyframe_changes"]
+for _c in ("sim3_eval_mapped", "sim3_track_mapped", "perma_mapped"):
+    PHOTOMETRY_CASES[_c] = SIM3_CASES[_c]
+PHOTOMETRY_PAIRS = [(s, c) for s in photometry.SCHEDULES for c in PHOTOMETRY_CASES]
+# the depth-map counters (pyoracle.BRANCHES) that no depth-map case of tests/test_ref_pin.py reaches on the default stream at the
+# default settings: the colour check of propagateDepth needs two frames that disagree in brightness, the negative-idepth -2 of
+# doLineStereo needs allowNegativeIdepths = 0
+UNREACHED_BY_DEFAULT_PHOTOMETRIC = ("stereo_negative", "prop_color")
+
+
+def run_under_exposure(schedule, case, gold):
+    """runs one case under one exposure schedule on the C restatement (gold = the record) or on the reference-compiled library
+    (gold = None); returns the case's Pin"""
+    fn, fl, ref_fl = PHOTOMETRY_CASES[case]
+    fl = ref_fl if gold is None else fl
+    seq, frames = photometry.stream(schedule)
+    p = Pin(f"{schedule}/{case}", gold)
+    try:
+        fn(p, fl, seq, frames)
+    finally:
+        po.set_globals(fl)
+    return p
+
+
+def record_photometry():
+    """every (schedule, case) on the reference-compiled library (needs oracle/_ref): the arrays of ref_pin_photometry_320x240.npz"""
+    out = {}
+    for s, c in PHOTOMETRY_PAIRS:
+        out.update(run_under_exposure(s, c, None).rec)
+    return out

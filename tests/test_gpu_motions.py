@@ -21,7 +21,7 @@ from oracle import replay
 from tests import device_cases as cases
 from tests import motions
 from tests.pin_cases import ONLY, PROPAGATION_FRAME, WIDE_BASELINE_FRAME
-from tests.util import IDENT, Pair, assert_step_ok, kf_depth_equal, new_depth, se3_inverse, tracked_pair
+from tests.util import Pair, assert_step_ok, kf_depth_equal, new_depth, se3_inverse
 
 pytestmark = pytest.mark.gpu
 
@@ -64,22 +64,7 @@ def test_random_init_observe_and_update_bit_exact(ctx, oracle, stream):
 
 
 def test_fill_holes_and_regularize_on_the_observed_map_bit_exact(ctx, oracle, stream):
-    """the passes of depthmap_individual_passes, on the map one observeDepth under the motion left"""
-    seq, frames = stream
-    p = Pair(ctx, oracle, seq, frames, "gt")
-    ofs = [p.add_frame(k) for k in (2, 3)]
-    p.sync_counters()
-    p.odm.observeDepth(ofs)
-    p.gdm.observeDepth([2, 3])
-    assert p.compare(exact=True)["n_valid"] > 10000
-    p.odm.regularizeFillHoles()
-    p.gdm.regularizeFillHoles()
-    p.compare(exact=True)
-    assert np.array_equal(p.gdm.integral(), p.odm.integral())
-    for occl in (False, True):
-        p.odm.regularize(occl, 24)
-        p.gdm.regularize(occl, 24)
-        p.compare(exact=True)
+    cases.fill_holes_and_regularize_observed(ctx, oracle, *stream)
 
 
 def test_propagate_and_create_keyframe(ctx, oracle, stream):
@@ -87,39 +72,7 @@ def test_propagate_and_create_keyframe(ctx, oracle, stream):
 
 
 def test_propagate_and_create_keyframe_with_tracking_mask_bit_exact(ctx, oracle, stream):
-    """device_cases.propagate_and_create_keyframe with the tracking mask, from identical inputs: each frame is tracked on
-    the device and its good mask is handed to the oracle, as oracle/replay.py does.  That test's own with-mask variant lets each
-    side use its own tracker's mask; the two masks differ on up to 1e-3 of the pixels (test_gpu_track.py), and under the backward
-    and roll motions those pixels move the regularised depth of their neighbours after createKeyFrame by up to 1.1e-3, beyond
-    the 2e-5 it allows.  With the same mask on both sides every step is bit for bit."""
-    seq, frames = stream
-    p = tracked_pair(ctx, oracle, seq, frames, [2, 5, 9])
-    trk = abi.SE3Tracker(ctx, mode=0)
-    for k in (2, 5, 9):
-        of = p.oframes[k]
-        oracle.lib().lsdo_frame_set_depthHasBeenUpdatedFlag(p.okf.ptr, 0)
-        ctx.L.lsdgpu_ref_import(ctx.ptr, 0)
-        trk.trackFrame(0, k, IDENT if k == 2 else of.thisToParent()[:7])        # writes the device's mask; the pose is restored
-        ctx.set_pose(k, of.thisToParent(), 0, oracle.lib().lsdo_frame_initialTrackedResidual(of.ptr))
-        mask = ctx.download(k, abi.BUF_GOODMASK)
-        assert mask.mean() > 0.05                      # all ones under forward: every pixel tracked well
-        of.refPixelWasGood(create=True)[:] = mask
-        p.sync_counters()
-        p.odm.updateKeyframe([of])
-        p.gdm.updateKeyframe([k])
-        p.compare(exact=True)
-    before = p.odm.current().copy()
-    p.odm.propagateDepth(p.oframes[9])
-    p.gdm.propagateDepth(9)
-    assert p.compare(exact=True)["n_valid"] > 5000
-    p.odm.set_current(before)
-    p.gdm.setHypotheses(0, before, do_set_depth=False)
-    p.odm.createKeyFrame(p.oframes[9])
-    q = p.gdm.createKeyFrame(9)
-    assert np.allclose(q[:7], p.oframes[9].thisToParent()[:7], atol=1e-12)
-    assert np.float32(q[7]).tobytes() == np.float32(p.oframes[9].thisToParent()[7]).tobytes()
-    p.compare(exact=True)
-    assert np.array_equal(ctx.download(9, abi.BUF_IDEPTH, 0), p.oframes[9].idepth(0))
+    cases.propagate_and_create_keyframe_device_mask(ctx, oracle, *stream)
 
 
 def test_finalize_create_keyframe_and_refs_bit_exact(ctx, oracle, stream):

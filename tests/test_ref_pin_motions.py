@@ -156,4 +156,7 @@ def test_default_cases_leave_those_branches_unreached(seq_small, frames_small):
         fn(pin.Pin(c), fl, seq_small, frames_small)
     got = po.branch_counts()
     assert all(got[b] == 0 for b in UNREACHED_BY_DEFAULT), {b: got[b] for b in UNREACHED_BY_DEFAULT}
+    # reached by tests/test_ref_pin_photometry.py (exposure changes) and the allowNegativeIdepths=0 set of the settings pin
+    unreached = pin.UNREACHED_BY_DEFAULT_PHOTOMETRIC
+    assert all(got[b] == 0 for b in unreached), {b: got[b] for b in unreached}
     assert got["depth_x"] > 100000 and got["clip_left"] > 0 and got["clip_top"] > 0
