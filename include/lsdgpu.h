@@ -154,6 +154,25 @@ int lsdgpu_frame_get_depth_stats(lsdgpu_ctx* ctx, int frame_id, float* meanIdept
 /* Frame::clear_refPixelWasGood (SlamSystem.cpp:573) */
 int lsdgpu_frame_clear_good_mask(lsdgpu_ctx* ctx, int frame_id);
 
+/* ---- frame memory: minimized frames (DataStructures/FrameMemory.cpp) ------------------------------------------------------------
+ * Found by symbol lookup (dlsym), like lsdgpu_track_and_map_group; LSDGPU_ABI_VERSION is unchanged.  A minimized frame gives its
+ * slot back and keeps, in a record allocated in stream order from a memory pool of the context, what Frame::minimizeInMemory keeps:
+ * image, idepth and idepthVar of level 0 (fp32), the reactivation data, the permaRef and all host-side metadata (pose, parent,
+ * initialTrackedResidual, counters, depth statistics, flags).  Its refPixelWasGood mask is cleared.  On a minimized frame these read
+ * the record in place: lsdgpu_frame_get_pose / _set_pose / _get_counters / _set_counters / _get_depth_stats,
+ * lsdgpu_frame_download_reactivation_data, lsdgpu_frame_download of IMAGE, IDEPTH and IDEPTH_VAR at level 0, the keyframe side of
+ * lsdgpu_perma_overlap_batch / lsdgpu_perma_track_batch, lsdgpu_map_export_pointcloud at level 0, and lsdgpu_frame_release (which
+ * frees the record).  Every other entry point that names a minimized frame fails with a message naming it and changes nothing.
+ * Neither call waits for the device.
+ * Frame::minimizeInMemory, Frame.cpp:377-395: one kernel.  Already minimized: nothing to do (0).  The depth map's active keyframe is
+ * refused, as by lsdgpu_frame_release. */
+int lsdgpu_frame_minimize(lsdgpu_ctx* ctx, int frame_id);
+/* FrameMemory::activateFrame (FrameMemory.cpp:129-137) + Frame::require (Frame.cpp:319-338): takes a free slot, restores the record
+ * and rebuilds image levels 1..4, the gradients and maxGradients from level 0 (3 kernels); the idepth pyramid is rebuilt on first
+ * use.  The frame is byte-identical to the frame before lsdgpu_frame_minimize, except that its refPixelWasGood mask is cleared.
+ * Already active: nothing to do (0).  No free slot: an error, and the frame stays minimized. */
+int lsdgpu_frame_activate(lsdgpu_ctx* ctx, int frame_id);
+
 /* ---- Tracking: Tracking/TrackingReference.cpp + Tracking/SE3Tracker.cpp -------------------------- */
 /* TrackingReference::importFrame :71-87 (+ the depthHasBeenUpdatedFlag=false of SlamSystem.cpp:907-912):
  * (re)builds the keyframe's idepth pyramids (Frame::buildIDepthAndIDepthVar, Frame.cpp:775-877) that

@@ -162,6 +162,8 @@ SYMBOLS = [
     ("lsdgpu_frame_set_counters", C.c_int, [_vp, C.c_int, C.c_int, C.c_int]),
     ("lsdgpu_frame_get_depth_stats", C.c_int, [_vp, C.c_int, _fp, _ip, _ip]),
     ("lsdgpu_frame_clear_good_mask", C.c_int, [_vp, C.c_int]),
+    ("lsdgpu_frame_minimize", C.c_int, [_vp, C.c_int]),
+    ("lsdgpu_frame_activate", C.c_int, [_vp, C.c_int]),
     ("lsdgpu_ref_import", C.c_int, [_vp, C.c_int]),
     ("lsdgpu_se3_eval", C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _fp, C.c_float, C.c_float, C.POINTER(TrackSettings), C.c_int, C.POINTER(EvalResult)]),
     ("lsdgpu_se3_track", C.c_int, [_vp, C.c_int, C.c_int, _dp, C.POINTER(TrackSettings), C.c_int, C.POINTER(TrackResult)]),
@@ -403,6 +405,15 @@ class Context:
 
     def release(self, fid: int):
         self._ck(self.L.lsdgpu_frame_release(self.ptr, fid))
+
+    def minimize(self, fid: int):
+        """Frame::minimizeInMemory (lsdgpu_frame_minimize): the frame gives its slot back and keeps level 0, the reactivation
+        data, the permaRef and its metadata in a record; its good mask is cleared"""
+        self._ck(self.L.lsdgpu_frame_minimize(self.ptr, fid))
+
+    def activate(self, fid: int):
+        """FrameMemory::activateFrame + Frame::require (lsdgpu_frame_activate): a minimized frame takes a free slot again"""
+        self._ck(self.L.lsdgpu_frame_activate(self.ptr, fid))
 
     def download(self, fid: int, what: int, level: int = 0) -> np.ndarray:
         w, h = self.w >> level, self.h >> level

@@ -13,7 +13,7 @@ extern "C" int lsdgpu_frame_set_perma_ref(lsdgpu_ctx* ctx, int kf_id, int* num_p
 { LSD_LOCK(ctx);   // Frame::setPermaRef -> reference->makePointCloud(QUICK_KF_CHECK_LVL) + copy (Frame.cpp:149-174, TrackingReference.cpp:96-147)
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* kf = findSlot(ctx, kf_id);
-    if (!kf) return lsd_fail(ctx, "unknown keyframe id");
+    if (!kf) return failMissing(ctx, kf_id, "unknown keyframe id");
     int r = ensureIdepthPyramid(ctx, kf);
     if (r) return r;
     const LevelCam& c = ctx->cam[QUICK_KF_CHECK_LVL];
@@ -48,7 +48,7 @@ static int fillPermaItems(lsdgpu_ctx* ctx, int n, const int* kf_ids, const doubl
     if (n <= 0 || n > LSD_MAX_PERMA_BATCH) return lsd_fail(ctx, "bad candidate count");
     items.resize(n);
     for (int i = 0; i < n; i++) {
-        FrameSlot* kf = findSlot(ctx, kf_ids[i]);
+        FrameSlot* kf = findFrame(ctx, kf_ids[i]);           // a minimized keyframe's permaRef is read from its record
         if (!kf) return lsd_fail(ctx, "unknown keyframe id");
         if (kf->permaNumPts <= 0) return lsd_fail(ctx, "keyframe has no permaRef (call lsdgpu_frame_set_perma_ref)");
         lsd::SE3<double> T;
@@ -84,7 +84,7 @@ extern "C" int lsdgpu_perma_track_batch(lsdgpu_ctx* ctx, int n, const int* kf_id
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* fr = findSlot(ctx, frame_id);
-    if (!fr) return lsd_fail(ctx, "unknown frame id");
+    if (!fr) return failMissing(ctx, frame_id, "unknown frame id");
     std::vector<PermaItem> items;
     int r = fillPermaItems(ctx, n, kf_ids, refToFrame_init_qt, items);
     if (r) return r;
@@ -146,7 +146,7 @@ static int sim3Launch(lsdgpu_ctx* ctx, int n, const int* ref_ids, const int* fra
     for (int i = 0; i < n; i++) {
         FrameSlot* kf = findSlot(ctx, ref_ids[i]);
         FrameSlot* fr = findSlot(ctx, frame_ids[i]);
-        if (!kf || !fr) return lsd_fail(ctx, "unknown frame id");
+        if (!kf || !fr) return failMissing(ctx, kf ? frame_ids[i] : ref_ids[i], "unknown frame id");
         int r = ensureIdepthPyramid(ctx, kf);       // reference->makePointCloud(lvl), Sim3Tracker.cpp:174
         if (r) return r;
         r = ensureIdepthPyramid(ctx, fr);           // frame->idepth(level) / idepthVar(level), :467-468

@@ -168,6 +168,8 @@ extern "C" void lsdgpu_destroy(lsdgpu_ctx* ctx)
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     peerCloseAll(ctx);
     cloudRelease(ctx);
+    for (auto& m : ctx->minimized) cudaFreeAsync(m.record, ctx->stream);
+    if (ctx->recordPool) { cudaStreamSynchronize(ctx->stream); cudaMemPoolDestroy(ctx->recordPool); }
     cudaFree(ctx->arena);
     if (ctx->stageRing) cudaFree(ctx->stageRing);
     if (ctx->dRemapX) cudaFree(ctx->dRemapX);

@@ -58,7 +58,7 @@ extern "C" int lsdgpu_depth_init_from_gt(lsdgpu_ctx* ctx, int kf_id)
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* kf = findSlot(ctx, kf_id);
-    if (!kf) return lsd_fail(ctx, "unknown keyframe id");
+    if (!kf) return failMissing(ctx, kf_id, "unknown keyframe id");
     if (!kf->hasDepth) return lsd_fail(ctx, "initializeFromGTDepth: frame has no idepth (call lsdgpu_frame_set_depth_gt)");
     const int n = ctx->w * ctx->h;
     ctx->activeKf = kf_id; ctx->activeKfReactivated = false;
@@ -124,7 +124,7 @@ extern "C" int lsdgpu_depth_set_hypotheses(lsdgpu_ctx* ctx, int kf_id, const lsd
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* kf = findSlot(ctx, kf_id);
-    if (!kf) return lsd_fail(ctx, "unknown keyframe id");
+    if (!kf) return failMissing(ctx, kf_id, "unknown keyframe id");
     const int n = ctx->w * ctx->h;
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
     memcpy(ctx->hStageF, aos, (size_t)n * 32);
@@ -180,7 +180,7 @@ static int setupObserve(lsdgpu_ctx* ctx, const lsdgpu_ref_desc* refs, int n_refs
     OP.byIdSize = 0;
     for (int k = 0; k < n_refs; k++) {
         FrameSlot* fr = findSlot(ctx, refs[k].frame_id);
-        if (!fr) return lsd_fail(ctx, "unknown reference frame id");
+        if (!fr) return failMissing(ctx, refs[k].frame_id, "unknown reference frame id");
         RefConst& rc = OP.refs[k];
         if (refs[k].tracked_on_kf) {
             // :1096-1097 refToKf = frame->pose->thisToParent_raw
@@ -324,7 +324,7 @@ extern "C" int lsdgpu_depth_propagate(lsdgpu_ctx* ctx, int new_kf_id)
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* kf = findSlot(ctx, ctx->activeKf);
     FrameSlot* nk = findSlot(ctx, new_kf_id);
-    if (!kf || !nk) return lsd_fail(ctx, "propagateDepth: unknown keyframe");
+    if (!kf || !nk) return failMissing(ctx, new_kf_id, "propagateDepth: unknown keyframe");
     return runPropagate(ctx, kf, nk);
 }
 
@@ -334,7 +334,7 @@ extern "C" int lsdgpu_depth_create_keyframe(lsdgpu_ctx* ctx, int new_kf_id, doub
     FrameSlot* kf = findSlot(ctx, ctx->activeKf);
     FrameSlot* nk = findSlot(ctx, new_kf_id);
     if (!kf) return lsd_fail(ctx, "createKeyFrame: depth map is not valid");
-    if (!nk) return lsd_fail(ctx, "createKeyFrame: unknown new keyframe");
+    if (!nk) return failMissing(ctx, new_kf_id, "createKeyFrame: unknown new keyframe");
     if (nk->parentId < 0) return lsd_fail(ctx, "createKeyFrame: new keyframe has no tracking parent");
     lsd::SE3<double> tp;
     for (int i = 0; i < 4; i++) tp.q[i] = nk->thisToParent[i];
@@ -450,7 +450,7 @@ extern "C" int lsdgpu_frame_take_reactivation_data(lsdgpu_ctx* ctx, int kf_id)
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* kf = findSlot(ctx, kf_id);
-    if (!kf) return lsd_fail(ctx, "unknown keyframe id");
+    if (!kf) return failMissing(ctx, kf_id, "unknown keyframe id");
     if (ctx->activeKf != kf_id) return lsd_fail(ctx, "takeReActivationData: the keyframe is not the active one");
     return takeReactivationData(ctx, kf);
 }
@@ -458,7 +458,7 @@ extern "C" int lsdgpu_frame_take_reactivation_data(lsdgpu_ctx* ctx, int kf_id)
 extern "C" int lsdgpu_frame_download_reactivation_data(lsdgpu_ctx* ctx, int kf_id, float* idepth_reAct, float* idepthVar_reAct, uint8_t* validity_reAct)
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
-    FrameSlot* kf = findSlot(ctx, kf_id);
+    FrameSlot* kf = findFrame(ctx, kf_id);                                 // a minimized keyframe: from its record
     if (!kf) return lsd_fail(ctx, "unknown keyframe id");
     if (!kf->reactValid) return lsd_fail(ctx, "keyframe has no reactivation data");
     const size_t n = (size_t)ctx->w * ctx->h;
@@ -473,7 +473,7 @@ extern "C" int lsdgpu_depth_set_from_existing_kf(lsdgpu_ctx* ctx, int kf_id)
 { LSD_LOCK(ctx);   // DepthMap::setFromExistingKF :920-962
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* kf = findSlot(ctx, kf_id);
-    if (!kf) return lsd_fail(ctx, "unknown keyframe id");
+    if (!kf) return failMissing(ctx, kf_id, "unknown keyframe id");
     if (!kf->hasDepth) return lsd_fail(ctx, "setFromExistingKF: keyframe has no depth");          // assert(kf->hasIDepthBeenSet()), :922
     if (!kf->reactValid) return lsd_fail(ctx, "setFromExistingKF: keyframe has no reactivation data");
     const int n = ctx->w * ctx->h;

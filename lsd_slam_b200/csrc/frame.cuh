@@ -49,8 +49,9 @@ __device__ __forceinline__ unsigned char remapPixelOpenCV(const uint8_t* __restr
     const int v = p00 * ((32 - fx) * (32 - fy) * 32) + p01 * (fx * (32 - fy) * 32) + p10 * ((32 - fx) * fy * 32) + p11 * (fx * fy * 32);
     return (unsigned char)((v + (1 << 14)) >> 15);
 }
-// source of level 0 of k_image_pyramid: the u8 image itself, or a raw image through UndistorterPTAM's / UndistorterOpenCV's tables
-enum { PYR_U8 = 0, PYR_PTAM = 1, PYR_OPENCV = 2 };
+// source of level 0 of k_image_pyramid: the u8 image itself, or a raw image through UndistorterPTAM's / UndistorterOpenCV's tables,
+// or (PYR_F32) the fp32 level 0 kept in a minimized frame's record (Frame::require after minimizeInMemory, Frame.cpp:319-338)
+enum { PYR_U8 = 0, PYR_PTAM = 1, PYR_OPENCV = 2, PYR_F32 = 3 };
 template <int SRC>
 __global__ void __launch_bounds__(256) k_image_pyramid(const uint8_t* __restrict__ src, PyrPtrs p, int w, int h,
                                                        const float* __restrict__ remapX = nullptr, const float* __restrict__ remapY = nullptr,
@@ -63,7 +64,9 @@ __global__ void __launch_bounds__(256) k_image_pyramid(const uint8_t* __restrict
     const int bx = blockIdx.x, by = blockIdx.y;
     const int x = bx * 16 + tx, y = by * 16 + ty;
     float v;
-    if (SRC != PYR_U8) {
+    if (SRC == PYR_F32)
+        v = reinterpret_cast<const float*>(src)[y * w + x];
+    else if (SRC != PYR_U8) {
         const unsigned char u = SRC == PYR_PTAM ? undistortPixel(src, in_w, __ldg(remapX + y * w + x), __ldg(remapY + y * w + x))
                                                 : remapPixelOpenCV(src, in_w, in_h, map1[y * w + x], __ldg(map2 + y * w + x));
         if (undist) undist[y * w + x] = u;
@@ -269,4 +272,25 @@ __global__ void __launch_bounds__(256) k_undistort_opencv(const uint8_t* __restr
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = remapPixelOpenCV(raw, in_w, in_h, map1[i], __ldg(map2 + i));
+}
+
+// The copies of lsdgpu_frame_minimize (slot -> record) and lsdgpu_frame_activate (record -> slot): up to REC_MAX_SEGS buffers of
+// a frame in one launch, 16 bytes per thread and step.  Every buffer starts 256-byte aligned and its length is rounded up to 16
+// bytes (each one lies in an allocation padded to 256 bytes).
+#define REC_MAX_SEGS 10
+struct RecordCopy {
+    const uint4* src[REC_MAX_SEGS];
+    uint4* dst[REC_MAX_SEGS];
+    long long end[REC_MAX_SEGS];         // cumulative length in uint4 units
+    int n;
+};
+__global__ void __launch_bounds__(256) k_record_copy(const __grid_constant__ RecordCopy c)
+{
+    const long long total = c.end[c.n - 1];
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        int k = 0;
+        while (i >= c.end[k]) k++;
+        const long long o = i - (k ? c.end[k - 1] : 0);
+        c.dst[k][o] = __ldg(c.src[k] + o);
+    }
 }

@@ -12,6 +12,7 @@ static FrameSlot* acquireSlot(lsdgpu_ctx* ctx, int id)
 {
     FrameSlot* s = findSlot(ctx, id);
     if (s) return s;
+    if (findMinimized(ctx, id)) return nullptr;      // a minimized frame keeps its id until it is activated or released
     for (auto& c : ctx->slots)
         if (!c.used) {
             FrameSlot fresh = c;          // keep the pointers
@@ -37,7 +38,7 @@ extern "C" int lsdgpu_frame_upload_u8(lsdgpu_ctx* ctx, int frame_id, const uint8
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* s = acquireSlot(ctx, frame_id);
-    if (!s) return lsd_fail(ctx, "no free frame slot (release frames or raise max_frames)");
+    if (!s) return failMissing(ctx, frame_id, "no free frame slot (release frames or raise max_frames)");
     const size_t n0 = (size_t)ctx->w * ctx->h;
     // double-buffered staging: only wait for the upload issued two frames ago.  A caller buffer that is already
     // page-locked (cudaHostAlloc / cudaHostRegister, e.g. a camera DMA buffer) is copied from directly -- it must then
@@ -80,7 +81,7 @@ extern "C" int lsdgpu_frame_from_stage(lsdgpu_ctx* ctx, int frame_id, int index)
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     if (index < 0 || index >= ctx->stageEntries) return lsd_fail(ctx, "bad ring index");
     FrameSlot* s = acquireSlot(ctx, frame_id);
-    if (!s) return lsd_fail(ctx, "no free frame slot (release frames or raise max_frames)");
+    if (!s) return failMissing(ctx, frame_id, "no free frame slot (release frames or raise max_frames)");
     return buildFrameFromDeviceU8(ctx, s, ctx->stageRing + (size_t)index * ctx->w * ctx->h);
 }
 
@@ -109,9 +110,159 @@ static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* 
 extern "C" int lsdgpu_frame_release(lsdgpu_ctx* ctx, int frame_id)
 { LSD_LOCK(ctx);
     FrameSlot* s = findSlot(ctx, frame_id);
-    if (!s) return lsd_fail(ctx, "unknown frame id");
+    if (!s) {
+        for (size_t i = 0; i < ctx->minimized.size(); i++)
+            if (ctx->minimized[i].id == frame_id) {
+                LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+                LSD_CHECK(ctx, cudaFreeAsync(ctx->minimized[i].record, ctx->stream));
+                ctx->minimized.erase(ctx->minimized.begin() + i);
+                // the pool keeps freed records for later minimizes (see lsdgpu_frame_minimize); a released frame's memory goes back
+                // to the device, down to what the records still alive need
+                size_t live = 0;
+                for (const auto& m : ctx->minimized) live += m.recordBytes;
+                LSD_CHECK(ctx, cudaMemPoolTrimTo(ctx->recordPool, live));
+                return 0;
+            }
+        return lsd_fail(ctx, "unknown frame id");
+    }
     if (ctx->activeKf == frame_id) return lsd_fail(ctx, "frame is the active keyframe of the depth map");
     s->used = false; s->id = -1;
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------------
+// frame memory: Frame::minimizeInMemory and FrameMemory::activateFrame + Frame::require (DESIGN.md section 3)
+// ------------------------------------------------------------------------------------------------------
+// The buffers of a frame that a minimized record keeps, in record order: dStats, image / idepth / idepthVar of level 0, the
+// reactivation data, the permaRef.  Buffers the frame does not have are null.
+struct RecordPart { char** ptr; size_t bytes; };
+static int recordParts(const lsdgpu_ctx* ctx, FrameSlot& s, RecordPart* p)
+{
+    const size_t n0 = (size_t)ctx->w * ctx->h;
+    int k = 0;
+    p[k++] = { (char**)&s.dStats, 3 * sizeof(double) };
+    p[k++] = { (char**)&s.image[0], n0 * 4 };
+    p[k++] = { (char**)&s.idepth[0], s.hasDepth ? n0 * 4 : 0 };
+    p[k++] = { (char**)&s.idepthVar[0], s.hasDepth ? n0 * 4 : 0 };
+    p[k++] = { (char**)&s.reactIdepth, s.reactValid ? n0 * 4 : 0 };
+    p[k++] = { (char**)&s.reactVar, s.reactValid ? n0 * 4 : 0 };
+    p[k++] = { (char**)&s.reactValidity, s.reactValid ? n0 : 0 };
+    p[k++] = { (char**)&s.permaPC, (size_t)s.permaNumPts * 16 };
+    p[k++] = { (char**)&s.permaVar, (size_t)s.permaNumPts * 4 };
+    return k;
+}
+static void addCopy(RecordCopy& c, const void* src, void* dst, size_t bytes)
+{
+    if (!bytes) return;
+    c.src[c.n] = (const uint4*)src; c.dst[c.n] = (uint4*)dst;
+    c.end[c.n] = (c.n ? c.end[c.n - 1] : 0) + (long long)(alignUp(bytes, 16) / 16);
+    c.n++;
+}
+static int launchRecordCopy(lsdgpu_ctx* ctx, const RecordCopy& c)
+{
+    const long long total = c.end[c.n - 1];
+    const int grid = (int)std::min<long long>((total + 255) / 256, (long long)ctx->smCount * 8);
+    k_record_copy<<<grid, 256, 0, ctx->stream>>>(c);
+    LAUNCH(ctx);
+    LSD_CHECK(ctx, cudaGetLastError());
+    return 0;
+}
+
+extern "C" int lsdgpu_frame_minimize(lsdgpu_ctx* ctx, int frame_id)
+{ LSD_LOCK(ctx);
+    if (findMinimized(ctx, frame_id)) return 0;
+    FrameSlot* s = findSlot(ctx, frame_id);
+    if (!s) return lsd_fail(ctx, "unknown frame id");
+    if (ctx->activeKf == frame_id) return lsd_fail(ctx, "frame is the active keyframe of the depth map");
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    if (!ctx->recordPool) {
+        cudaMemPoolProps pp;
+        memset(&pp, 0, sizeof(pp));
+        pp.allocType = cudaMemAllocationTypePinned;
+        pp.location.type = cudaMemLocationTypeDevice; pp.location.id = ctx->device;
+        LSD_CHECK(ctx, cudaMemPoolCreate(&ctx->recordPool, &pp));
+        // freed records stay mapped for the next minimize instead of going back to the device at each synchronisation (which
+        // made every allocation map fresh memory on the stream); the context's destruction returns them
+        uint64_t keep = UINT64_MAX;
+        LSD_CHECK(ctx, cudaMemPoolSetAttribute(ctx->recordPool, cudaMemPoolAttrReleaseThreshold, &keep));
+    }
+    FrameSlot m = *s;
+    RecordPart from[REC_MAX_SEGS], to[REC_MAX_SEGS];
+    const int np = recordParts(ctx, *s, from);
+    recordParts(ctx, m, to);
+    size_t bytes = 0;
+    for (int k = 0; k < np; k++) bytes += alignUp(from[k].bytes, 256);
+    char* rec = nullptr;
+    LSD_CHECK(ctx, cudaMallocFromPoolAsync((void**)&rec, bytes, ctx->recordPool, ctx->stream));
+    RecordCopy c;
+    memset(&c, 0, sizeof(c));
+    size_t off = 0;
+    for (int k = 0; k < np; k++) {
+        *to[k].ptr = from[k].bytes ? rec + off : nullptr;
+        addCopy(c, *from[k].ptr, *to[k].ptr, from[k].bytes);
+        off += alignUp(from[k].bytes, 256);
+    }
+    const int r = launchRecordCopy(ctx, c);
+    if (r) { cudaFreeAsync(rec, ctx->stream); return r; }
+    for (int l = 0; l < LSD_LEVELS; l++) {
+        m.grad[l] = nullptr;
+        if (l) m.image[l] = m.idepth[l] = m.idepthVar[l] = nullptr;
+    }
+    m.maxgrad = nullptr; m.goodMask = nullptr;
+    m.record = rec; m.recordBytes = bytes;
+    m.idepthPyrValid = false;
+    m.hasGoodMask = false;                                          // clear_refPixelWasGood, Frame.cpp:388
+    ctx->minimized.push_back(m);
+    s->used = false; s->id = -1;
+    return 0;
+}
+
+extern "C" int lsdgpu_frame_activate(lsdgpu_ctx* ctx, int frame_id)
+{ LSD_LOCK(ctx);
+    if (findSlot(ctx, frame_id)) return 0;
+    FrameSlot* m = findMinimized(ctx, frame_id);
+    if (!m) return lsd_fail(ctx, "unknown frame id");
+    FrameSlot* c = nullptr;
+    for (auto& f : ctx->slots)
+        if (!f.used) { c = &f; break; }
+    if (!c) {
+        ctx->err = "no free frame slot to activate frame " + std::to_string(frame_id) + " (minimize or release frames, or raise max_frames); it stays minimized";
+        return -2;
+    }
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    FrameSlot a = *m;
+    RecordPart from[REC_MAX_SEGS], to[REC_MAX_SEGS];
+    const int np = recordParts(ctx, *m, from);
+    for (int l = 0; l < LSD_LEVELS; l++) {                         // the slot's buffers
+        a.image[l] = c->image[l]; a.grad[l] = c->grad[l]; a.idepth[l] = c->idepth[l]; a.idepthVar[l] = c->idepthVar[l];
+    }
+    a.maxgrad = c->maxgrad; a.goodMask = c->goodMask; a.dStats = c->dStats;
+    a.permaPC = c->permaPC; a.permaVar = c->permaVar;
+    a.reactIdepth = c->reactIdepth; a.reactVar = c->reactVar; a.reactValidity = c->reactValidity;
+    recordParts(ctx, a, to);
+    RecordCopy cp;
+    memset(&cp, 0, sizeof(cp));
+    for (int k = 0; k < np; k++)
+        if (from[k].ptr != (char**)&m->image[0]) addCopy(cp, *from[k].ptr, *to[k].ptr, from[k].bytes);   // level 0 of the image: below
+    int r = launchRecordCopy(ctx, cp);
+    if (r) return r;
+    PyrPtrs pp;
+    for (int l = 0; l < LSD_LEVELS; l++) pp.l[l] = a.image[l];
+    k_image_pyramid<PYR_F32><<<dim3(ctx->w / 16, ctx->h / 16), 256, 0, ctx->stream>>>((const uint8_t*)m->image[0], pp, ctx->w, ctx->h);
+    LAUNCH(ctx);
+    GradPtrs gp;
+    for (int l = 0; l < LSD_LEVELS; l++) { gp.img[l] = a.image[l]; gp.grad[l] = a.grad[l]; gp.w[l] = ctx->w >> l; gp.h[l] = ctx->h >> l; }
+    gp.maxgrad0 = a.maxgrad;
+    LSD_CHECK(ctx, launchPDL(k_gradients, dim3(divUp(ctx->w, GR_TW) * divUp(ctx->h, GR_TH), LSD_LEVELS), dim3(256), 0, ctx->stream, gp));
+    LAUNCH(ctx);
+    LSD_CHECK(ctx, cudaGetLastError());
+    LSD_CHECK(ctx, cudaFreeAsync(m->record, ctx->stream));
+    a.record = nullptr; a.recordBytes = 0;
+    a.used = true;
+    a.idepthPyrValid = false;                                       // ensureIdepthPyramid rebuilds levels 1..4 on first use
+    a.reactAllocated = a.reactValid;
+    *c = a;
+    ctx->minimized.erase(ctx->minimized.begin() + (m - ctx->minimized.data()));
     return 0;
 }
 
@@ -131,9 +282,13 @@ int ensureIdepthPyramid(lsdgpu_ctx* ctx, FrameSlot* s)
 extern "C" int lsdgpu_frame_download(lsdgpu_ctx* ctx, int frame_id, int what, int level, void* out)
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
-    FrameSlot* s = findSlot(ctx, frame_id);
+    FrameSlot* s = findFrame(ctx, frame_id);
     if (!s) return lsd_fail(ctx, "unknown frame id");
     if (level < 0 || level >= LSD_LEVELS) return lsd_fail(ctx, "bad level");
+    if (s->record && !(level == 0 && (what == LSDGPU_BUF_IMAGE || what == LSDGPU_BUF_IDEPTH || what == LSDGPU_BUF_IDEPTH_VAR))) {
+        ctx->err = "frame " + std::to_string(frame_id) + " is minimized: only image, idepth and idepthVar of level 0 are kept (lsdgpu_frame_activate it first)";
+        return -2;
+    }
     const size_t n = ((size_t)ctx->w * ctx->h) >> (2 * level);
     const void* src = nullptr;
     size_t bytes = 0;
@@ -160,7 +315,7 @@ extern "C" int lsdgpu_frame_set_depth_gt(lsdgpu_ctx* ctx, int frame_id, const fl
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* s = findSlot(ctx, frame_id);
-    if (!s) return lsd_fail(ctx, "unknown frame id");
+    if (!s) return failMissing(ctx, frame_id, "unknown frame id");
     const int n = ctx->w * ctx->h;
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
     memcpy(ctx->hStageF, depth, (size_t)n * 4);
@@ -177,7 +332,7 @@ extern "C" int lsdgpu_frame_set_idepth(lsdgpu_ctx* ctx, int frame_id, const floa
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* s = findSlot(ctx, frame_id);
-    if (!s) return lsd_fail(ctx, "unknown frame id");
+    if (!s) return failMissing(ctx, frame_id, "unknown frame id");
     const size_t n = (size_t)ctx->w * ctx->h;
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
     memcpy(ctx->hStageF, idepth, n * 4);
@@ -190,7 +345,7 @@ extern "C" int lsdgpu_frame_set_idepth(lsdgpu_ctx* ctx, int frame_id, const floa
 
 extern "C" int lsdgpu_frame_set_pose(lsdgpu_ctx* ctx, int frame_id, const double qts[8], int parent_id, float itr)
 { LSD_LOCK(ctx);
-    FrameSlot* s = findSlot(ctx, frame_id);
+    FrameSlot* s = findFrame(ctx, frame_id);
     if (!s) return lsd_fail(ctx, "unknown frame id");
     memcpy(s->thisToParent, qts, sizeof(s->thisToParent));
     s->parentId = parent_id; s->initialTrackedResidual = itr;
@@ -198,7 +353,7 @@ extern "C" int lsdgpu_frame_set_pose(lsdgpu_ctx* ctx, int frame_id, const double
 }
 extern "C" int lsdgpu_frame_get_pose(lsdgpu_ctx* ctx, int frame_id, double qts[8], int* parent_id, float* itr)
 { LSD_LOCK(ctx);
-    FrameSlot* s = findSlot(ctx, frame_id);
+    FrameSlot* s = findFrame(ctx, frame_id);
     if (!s) return lsd_fail(ctx, "unknown frame id");
     if (qts) memcpy(qts, s->thisToParent, sizeof(s->thisToParent));
     if (parent_id) *parent_id = s->parentId;
@@ -207,7 +362,7 @@ extern "C" int lsdgpu_frame_get_pose(lsdgpu_ctx* ctx, int frame_id, double qts[8
 }
 extern "C" int lsdgpu_frame_get_counters(lsdgpu_ctx* ctx, int frame_id, int* tracked, int* mapped)
 { LSD_LOCK(ctx);
-    FrameSlot* s = findSlot(ctx, frame_id);
+    FrameSlot* s = findFrame(ctx, frame_id);
     if (!s) return lsd_fail(ctx, "unknown frame id");
     if (tracked) *tracked = s->numFramesTrackedOnThis;
     if (mapped) *mapped = s->numMappedOnThis;
@@ -215,14 +370,14 @@ extern "C" int lsdgpu_frame_get_counters(lsdgpu_ctx* ctx, int frame_id, int* tra
 }
 extern "C" int lsdgpu_frame_set_counters(lsdgpu_ctx* ctx, int frame_id, int tracked, int mapped)
 { LSD_LOCK(ctx);
-    FrameSlot* s = findSlot(ctx, frame_id);
+    FrameSlot* s = findFrame(ctx, frame_id);
     if (!s) return lsd_fail(ctx, "unknown frame id");
     s->numFramesTrackedOnThis = tracked; s->numMappedOnThis = mapped;
     return 0;
 }
 extern "C" int lsdgpu_frame_get_depth_stats(lsdgpu_ctx* ctx, int frame_id, float* meanIdepth, int* numPoints, int* flag)
 { LSD_LOCK(ctx);
-    FrameSlot* s = findSlot(ctx, frame_id);
+    FrameSlot* s = findFrame(ctx, frame_id);
     if (!s) return lsd_fail(ctx, "unknown frame id");
     if ((meanIdepth || numPoints) && s->statsPending) {      // fetched lazily: keeps updateKeyframe free of host syncs
         LSD_CHECK(ctx, cudaSetDevice(ctx->device));
@@ -240,7 +395,7 @@ extern "C" int lsdgpu_frame_get_depth_stats(lsdgpu_ctx* ctx, int frame_id, float
 extern "C" int lsdgpu_frame_clear_good_mask(lsdgpu_ctx* ctx, int frame_id)
 { LSD_LOCK(ctx);
     FrameSlot* s = findSlot(ctx, frame_id);
-    if (!s) return lsd_fail(ctx, "unknown frame id");
+    if (!s) return failMissing(ctx, frame_id, "unknown frame id");
     s->hasGoodMask = false;
     return 0;
 }
@@ -249,7 +404,7 @@ extern "C" int lsdgpu_ref_import(lsdgpu_ctx* ctx, int kf_id)
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* kf = findSlot(ctx, kf_id);
-    if (!kf) return lsd_fail(ctx, "unknown keyframe id");
+    if (!kf) return failMissing(ctx, kf_id, "unknown keyframe id");
     int r = ensureIdepthPyramid(ctx, kf);
     if (r) return r;
     kf->depthHasBeenUpdatedFlag = false;       // SlamSystem.cpp:907-912
@@ -419,7 +574,7 @@ extern "C" int lsdgpu_frame_upload_distorted_u8(lsdgpu_ctx* ctx, int frame_id, c
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* s = acquireSlot(ctx, frame_id);
-    if (!s) return lsd_fail(ctx, "no free frame slot (release frames or raise max_frames)");
+    if (!s) return failMissing(ctx, frame_id, "no free frame slot (release frames or raise max_frames)");
     int r = uploadRaw(ctx, raw);
     if (r) return r;
     return buildFrameFromDeviceU8(ctx, s, ctx->dRaw, ctx->dCvMap1 ? PYR_OPENCV : ctx->dRemapX ? PYR_PTAM : PYR_U8);

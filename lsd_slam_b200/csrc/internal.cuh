@@ -60,6 +60,8 @@ struct FrameSlot {
     int parentId = -1;
     float initialTrackedResidual = 0.f;
     int numFramesTrackedOnThis = 0, numMappedOnThis = 0;
+    char* record = nullptr;              // minimized frame (lsdgpu_frame_minimize): its record, which the pointers above point into
+    size_t recordBytes = 0;
 };
 
 struct PyrPtrs {
@@ -120,6 +122,11 @@ struct lsdgpu_ctx {
     char* arena = nullptr;
     size_t arenaBytes = 0;
     std::vector<FrameSlot> slots;
+    // minimized frames (Frame::minimizeInMemory): the frame's metadata, with image / idepth / idepthVar of level 0, the
+    // reactivation data, the permaRef and dStats pointing into its record and every other device pointer null.  Records come
+    // in stream order from recordPool (DESIGN.md section 3).
+    std::vector<FrameSlot> minimized;
+    cudaMemPool_t recordPool = nullptr;
 
     // depth map
     HypField cur, oth;
@@ -256,6 +263,26 @@ static inline FrameSlot* findSlot(lsdgpu_ctx* ctx, int id)
     for (auto& s : ctx->slots)
         if (s.used && s.id == id) return &s;
     return nullptr;
+}
+
+static inline FrameSlot* findMinimized(lsdgpu_ctx* ctx, int id)
+{
+    for (auto& s : ctx->minimized)
+        if (s.id == id) return &s;
+    return nullptr;
+}
+// a frame in a slot or minimized: the entry points that read a minimized frame's record in place
+static inline FrameSlot* findFrame(lsdgpu_ctx* ctx, int id)
+{
+    FrameSlot* s = findSlot(ctx, id);
+    return s ? s : findMinimized(ctx, id);
+}
+// the error of an entry point that needs frame `id` in a slot: `msg` when the id is unknown, or that the frame is minimized
+static inline int failMissing(lsdgpu_ctx* ctx, int id, const char* msg)
+{
+    if (!findMinimized(ctx, id)) return lsd_fail(ctx, msg);
+    ctx->err = "frame " + std::to_string(id) + " is minimized (lsdgpu_frame_activate it first)";
+    return -2;
 }
 
 static inline int divUp(int a, int b) { return (a + b - 1) / b; }

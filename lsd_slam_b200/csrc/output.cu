@@ -14,7 +14,7 @@ extern "C" int lsdgpu_keyframe_pack_pointcloud(lsdgpu_ctx* ctx, int kf_id, int p
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* kf = findSlot(ctx, kf_id);
-    if (!kf) return lsd_fail(ctx, "unknown keyframe id");
+    if (!kf) return failMissing(ctx, kf_id, "unknown keyframe id");
     if (publish_level < 0 || publish_level >= LSD_LEVELS) return lsd_fail(ctx, "bad level");
     int r = ensureIdepthPyramid(ctx, kf);                      // f->idepth(publishLvl), ROSOutput3DWrapper.cpp:96-97
     if (r) return r;
@@ -136,7 +136,11 @@ extern "C" int lsdgpu_map_export_pointcloud(lsdgpu_ctx* ctx, int n, const int* k
     if (ctx->cloudMaxKf == 0) return lsd_fail(ctx, "map_export_pointcloud: no reservation (call lsdgpu_cloud_reserve first)");
     std::vector<FrameSlot*> kfs(n);
     for (int i = 0; i < n; i++) {
-        kfs[i] = findSlot(ctx, kf_ids[i]);
+        kfs[i] = level == 0 ? findFrame(ctx, kf_ids[i]) : findSlot(ctx, kf_ids[i]);   // level 0 of a minimized keyframe: its record
+        if (!kfs[i] && level > 0 && findMinimized(ctx, kf_ids[i])) {
+            snprintf(msg, sizeof(msg), "map_export_pointcloud: keyframe %d (kf_ids[%d]) is minimized: only level 0 is kept", kf_ids[i], i);
+            return lsd_fail(ctx, msg);
+        }
         if (!kfs[i] || !kfs[i]->hasDepth) {
             snprintf(msg, sizeof(msg), "map_export_pointcloud: keyframe %d (kf_ids[%d]) %s", kf_ids[i], i,
                      kfs[i] ? "has no depth" : "is unknown");

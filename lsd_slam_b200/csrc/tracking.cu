@@ -418,7 +418,7 @@ extern "C" int lsdgpu_se3_eval(lsdgpu_ctx* ctx, int kf_id, int frame_id, int lev
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* kf = findSlot(ctx, kf_id);
     FrameSlot* fr = findSlot(ctx, frame_id);
-    if (!kf || !fr) return lsd_fail(ctx, "unknown frame id");
+    if (!kf || !fr) return failMissing(ctx, kf ? frame_id : kf_id, "unknown frame id");
     if (level < 0 || level >= LSD_LEVELS) return lsd_fail(ctx, "bad level");
     int r = ensureIdepthPyramid(ctx, kf);
     if (r) return r;
@@ -540,7 +540,7 @@ extern "C" int lsdgpu_se3_track(lsdgpu_ctx* ctx, int kf_id, int frame_id, const 
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* kf = findSlot(ctx, kf_id);
     FrameSlot* fr = findSlot(ctx, frame_id);
-    if (!kf || !fr) return lsd_fail(ctx, "unknown frame id");
+    if (!kf || !fr) return failMissing(ctx, kf ? frame_id : kf_id, "unknown frame id");
     int r = ensureIdepthPyramid(ctx, kf);      // reference->makePointCloud(lvl), SE3Tracker.cpp:321
     if (r) return r;
     lsdgpu_track_settings ds;
@@ -561,7 +561,7 @@ extern "C" int lsdgpu_se3_track_sharded(lsdgpu_ctx* ctx, int kf_id, int frame_id
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     FrameSlot* kf = findSlot(ctx, kf_id);
     FrameSlot* fr = findSlot(ctx, frame_id);
-    if (!kf || !fr) return lsd_fail(ctx, "unknown frame id");
+    if (!kf || !fr) return failMissing(ctx, kf ? frame_id : kf_id, "unknown frame id");
     if (n_shards < 1 || shard < 0 || shard >= n_shards) return lsd_fail(ctx, "bad shard");
     if (n_shards > 1 && !allreduce) return lsd_fail(ctx, "sharded tracking needs an all-reduce callback");
     int r = ensureIdepthPyramid(ctx, kf);
@@ -588,6 +588,7 @@ extern "C" int lsdgpu_track_and_map(lsdgpu_ctx* ctx, int kf_id, int frame_id, co
                                     const double init_qt[7], const lsdgpu_track_settings* s, int mode,
                                     int keyframe_change, lsdgpu_track_result* out, double new_qts[8])
 { LSD_LOCK(ctx);
+    if (findMinimized(ctx, kf_id)) return failMissing(ctx, kf_id, "unknown keyframe id");      // before the frame is built
     int r = gray ? lsdgpu_frame_upload_u8(ctx, frame_id, gray) : lsdgpu_frame_from_stage(ctx, frame_id, stage_index);
     if (r) return r;
     FrameSlot* kf = findSlot(ctx, kf_id);
@@ -649,7 +650,11 @@ extern "C" int lsdgpu_track_and_map_group(int n, const lsdgpu_group_step* steps,
         if (c->device != c0->device) return groupFail(n, steps, i, "context is on another device than step 0's");
         if (c->w != c0->w || c->h != c0->h) return groupFail(n, steps, i, "context size differs from step 0's");
         if (c->nRanks > 1) return groupFail(n, steps, i, "context is peer-attached (a sharded stream cannot be grouped)");
-        if (!findSlot(steps[i].ctx, steps[i].kf_id)) return groupFail(n, steps, i, "unknown frame id (keyframe)");
+        if (!findSlot(steps[i].ctx, steps[i].kf_id)) {
+            if (findMinimized(steps[i].ctx, steps[i].kf_id)) return groupFail(n, steps, i, ("keyframe " + std::to_string(steps[i].kf_id) + " is minimized").c_str());
+            return groupFail(n, steps, i, "unknown frame id (keyframe)");
+        }
+        if (findMinimized(steps[i].ctx, steps[i].frame_id)) return groupFail(n, steps, i, ("frame " + std::to_string(steps[i].frame_id) + " is minimized").c_str());
     }
     if (cudaSetDevice(c0->device) != cudaSuccess) return groupFail(n, steps, -1, "cudaSetDevice failed", -1);
 

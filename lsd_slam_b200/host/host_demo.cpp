@@ -15,7 +15,7 @@ using namespace lsd_slam;
 int main(int argc, char** argv)
 {
     if (argc < 2) {
-        std::fprintf(stderr, "usage: host_demo <frames.bin> [kf_every] | host_demo --undistorter <calib.cfg> <tables.bin>"
+        std::fprintf(stderr, "usage: host_demo <frames.bin> [kf_every [late | prune <max_frames> <max_active>]] | host_demo --undistorter <calib.cfg> <tables.bin>"
                              " | host_demo --undistorter-any <calib.cfg> <tables.bin>\n");
         return 2;
     }
@@ -64,6 +64,10 @@ int main(int argc, char** argv)
     // in unmappedTrackedFrames are (SlamSystem.cpp:559-575 -> DepthMap.cpp:1085-1099).  The first frame of the old keyframe is
     // used: the last one is too close to the new keyframe for the epipolar-length gate (DepthMap.cpp:203).
     const bool lateMapping = argc > 3 && std::string(argv[3]) == "late";
+    // "prune <max_frames> <max_active>": a context with few frame slots that keeps every keyframe; after each keyframe change
+    // FrameMemory::pruneActiveFrames (SlamSystem.cpp:327) minimizes all but the max_active most recently activated frames
+    const bool prune = argc > 5 && std::string(argv[3]) == "prune";
+    const int maxFrames = prune ? std::atoi(argv[4]) : 8;
     FILE* f = std::fopen(argv[1], "rb");
     if (!f) { std::perror("open"); return 2; }
     int w, h, n;
@@ -73,7 +77,8 @@ int main(int argc, char** argv)
     if (std::fread(depth.data(), 4, depth.size(), f) != depth.size()) return 2;
     std::vector<unsigned char> img((size_t)w * h);
     try {
-        DeviceContext dev(0, w, h, K, 8);
+        DeviceContext dev(0, w, h, K, maxFrames);
+        if (prune) dev.frameMemory().setMaxActiveFrames(std::atoi(argv[5]));
         SE3Tracker tracker(dev, w, h, K);
         tracker.settings.maxItsPerLvl[4] = 0;                              // SlamSystem.cpp:80-81
         DepthMap map(dev, w, h, K);
@@ -106,6 +111,7 @@ int main(int argc, char** argv)
                 prev.reset();
                 early.reset();
                 last = SE3();
+                if (prune) dev.frameMemory().pruneActiveFrames();
             } else {
                 std::deque<std::shared_ptr<Frame>> refs{ fr };
                 map.updateKeyframe(refs);                                  // :571

@@ -1,8 +1,10 @@
 // lsd_host.cpp -- implementation of lsd_host.h over the C ABI.  See the header for the reference citations.
 #include "lsd_host.h"
 
+#include <algorithm>
 #include <cstdio>
 #include <fstream>
+#include <iterator>
 #include <string>
 
 #include <cmath>
@@ -81,8 +83,9 @@ Sim3 FramePoseStruct::getCamToWorld(int recursionDepth) const
     return trackingParent->getCamToWorld(recursionDepth + 1) * thisToParent_raw;
 }
 
-DeviceContext::DeviceContext(int device, int w, int h, const Matrix3f& K, int maxFrames) : w_(w), h_(h)
+DeviceContext::DeviceContext(int device, int w, int h, const Matrix3f& K, int maxFrames) : w_(w), h_(h), maxFrames_(maxFrames)
 {
+    memory_.reset(new FrameMemory(*this, 10 + 20));       // maxLoopClosureCandidates + 20, settings.cpp:97 / FrameMemory.cpp:153
     int rc = lsdgpu_create(device, w, h, K.m, maxFrames, &ctx_);
     if (rc != 0) {
         std::string msg = ctx_ ? lsdgpu_last_error(ctx_) : "lsdgpu_create failed (bad size: width and height must be multiples of 16)";
@@ -97,23 +100,113 @@ void DeviceContext::check(int rc, const char* where) const
     if (rc != 0) throw LsdGpuError(std::string(where) + ": " + lsdgpu_last_error(ctx_));
 }
 
+FrameMemory::FrameMemory(DeviceContext& dev, int maxActive) : dev_(dev), maxActive_(maxActive) {}
+
+void FrameMemory::minimizeLeastRecent()
+{
+    const int activeKf = lsdgpu_depth_active_keyframe(dev_.raw());
+    for (auto it = activeFrames.rbegin(); it != activeFrames.rend(); ++it) {
+        Frame* f = *it;
+        if (f->id() == activeKf || std::find(held_.begin(), held_.end(), f) != held_.end()) continue;
+        activeFrames.erase(std::next(it).base());
+        f->minimizeOnDevice();
+        f->isActive = false;
+        return;
+    }
+    throw LsdGpuError("FrameMemory: no frame slot can be freed: every active frame is the active keyframe or in use by this call "
+                      "(raise max_frames)");
+}
+void FrameMemory::makeRoom()
+{
+    std::lock_guard<std::recursive_mutex> l(mu_);
+    while ((int)activeFrames.size() >= dev_.maxFrames()) minimizeLeastRecent();
+}
+void FrameMemory::activateFrame(Frame* frame)
+{
+    std::lock_guard<std::recursive_mutex> l(mu_);
+    if (frame->isActive) {
+        activeFrames.remove(frame);
+    } else {
+        makeRoom();
+        dev_.check(lsdgpu_frame_activate(dev_.raw(), frame->id()), "FrameMemory::activateFrame");
+        frame->isActive = true;
+    }
+    activeFrames.push_front(frame);
+}
+void FrameMemory::deactivateFrame(Frame* frame)
+{
+    std::lock_guard<std::recursive_mutex> l(mu_);
+    if (!frame->isActive) return;
+    activeFrames.remove(frame);
+    frame->minimizeOnDevice();
+    frame->isActive = false;
+}
+void FrameMemory::pruneActiveFrames()
+{
+    std::lock_guard<std::recursive_mutex> l(mu_);
+    while ((int)activeFrames.size() > maxActive_) minimizeLeastRecent();
+}
+
+ActiveFrames::ActiveFrames(FrameMemory& memory, std::initializer_list<Frame*> frames)
+    : ActiveFrames(memory, std::vector<Frame*>(frames)) {}
+ActiveFrames::ActiveFrames(FrameMemory& memory, const std::vector<Frame*>& frames) : memory_(memory)
+{
+    std::lock_guard<std::recursive_mutex> l(memory_.mu_);
+    try {
+        for (Frame* f : frames) {
+            memory_.activateFrame(f);
+            memory_.held_.push_back(f);
+            n_++;
+        }
+    } catch (...) {
+        memory_.held_.resize(memory_.held_.size() - n_);
+        throw;
+    }
+}
+ActiveFrames::~ActiveFrames()
+{
+    std::lock_guard<std::recursive_mutex> l(memory_.mu_);
+    memory_.held_.resize(memory_.held_.size() - n_);
+}
+
 Frame::Frame(DeviceContext& dev, int id, int width, int height, const Matrix3f&, double timestamp, const unsigned char* image, bool distorted)
     : dev_(dev), id_(id), w_(width), h_(height), timestamp_(timestamp)
 {
     pose = new FramePoseStruct();
     pose->frameID = id;
+    FrameMemory& m = dev_.frameMemory();
+    std::lock_guard<std::recursive_mutex> l(m.mu_);
+    m.makeRoom();
     dev_.check(distorted ? lsdgpu_frame_upload_distorted_u8(dev_.raw(), id, image) : lsdgpu_frame_upload_u8(dev_.raw(), id, image), "Frame::Frame");
+    m.activeFrames.push_front(this);                    // Frame.cpp:35-54 leaves a new frame active
 }
 Frame::~Frame()
 {
+    {
+        FrameMemory& m = dev_.frameMemory();
+        std::lock_guard<std::recursive_mutex> l(m.mu_);
+        if (isActive) m.activeFrames.remove(this);
+    }
     lsdgpu_frame_release(dev_.raw(), id_);      // may fail for the active keyframe: DepthMap::invalidate() first
     delete pose;
 }
+void Frame::minimizeOnDevice() { dev_.check(lsdgpu_frame_minimize(dev_.raw(), id_), "Frame::minimizeInMemory"); }
+bool Frame::minimizeInMemory()
+{
+    dev_.frameMemory().deactivateFrame(this);
+    return true;
+}
+void Frame::getActiveLock() { dev_.frameMemory().activateFrame(this); }
 void Frame::setDepthFromGroundTruth(const float* depth, float cov_scale)
 {
+    getActiveLock();                                                    // Frame.cpp:247
     dev_.check(lsdgpu_frame_set_depth_gt(dev_.raw(), id_, depth, cov_scale), "Frame::setDepthFromGroundTruth");
 }
-void Frame::clear_refPixelWasGood() { dev_.check(lsdgpu_frame_clear_good_mask(dev_.raw(), id_), "Frame::clear_refPixelWasGood"); }
+void Frame::clear_refPixelWasGood()
+{
+    if (!isActive) return;                                              // minimizeInMemory cleared it, Frame.cpp:388
+    dev_.check(lsdgpu_frame_clear_good_mask(dev_.raw(), id_), "Frame::clear_refPixelWasGood");
+}
 float Frame::meanIdepth()
 {
     float m = 1; int n = 0, f = 0;
@@ -134,6 +227,7 @@ bool Frame::depthHasBeenUpdatedFlag() const
 }
 void Frame::downloadIdepth(int level, std::vector<float>& idepth, std::vector<float>& idepthVar)
 {
+    if (level > 0) getActiveLock();                                     // levels 1..4 are rebuilt on activation (Frame::require)
     size_t n = (size_t)width(level) * height(level);
     idepth.resize(n); idepthVar.resize(n);
     dev_.check(lsdgpu_frame_download(dev_.raw(), id_, LSDGPU_BUF_IDEPTH, level, idepth.data()), "Frame::idepth");
@@ -141,12 +235,14 @@ void Frame::downloadIdepth(int level, std::vector<float>& idepth, std::vector<fl
 }
 void Frame::downloadRefPixelWasGood(std::vector<unsigned char>& mask)
 {
+    getActiveLock();
     mask.resize((size_t)width(1) * height(1));
     dev_.check(lsdgpu_frame_download(dev_.raw(), id_, LSDGPU_BUF_GOODMASK, 1, mask.data()), "Frame::refPixelWasGood");
 }
 
 void TrackingReference::importFrame(Frame* sourceKF)
 {
+    sourceKF->getActiveLock();                                          // TrackingReference.cpp:74
     keyframe = sourceKF;
     frameID = sourceKF->id();
     sourceKF->dev().check(lsdgpu_ref_import(sourceKF->dev().raw(), frameID), "TrackingReference::importFrame");
@@ -162,6 +258,7 @@ SE3 SE3Tracker::trackFrame(TrackingReference* reference, Frame* frame, const SE3
     double init[7];
     for (int i = 0; i < 4; i++) init[i] = frameToReference_initialEstimate.q[i];
     for (int i = 0; i < 3; i++) init[4 + i] = frameToReference_initialEstimate.t[i];
+    ActiveFrames held(dev_.frameMemory(), { reference->keyframe, frame });   // SE3Tracker.cpp:286; the keyframe's levels live in its slot
     lsdgpu_track_result r;
     dev_.check(lsdgpu_se3_track(dev_.raw(), reference->keyframe->id(), frame->id(), init, &settings, mode, &r), "SE3Tracker::trackFrame");
     pointUsage = r.pointUsage; lastGoodCount = r.lastGoodCount; lastBadCount = r.lastBadCount;
@@ -216,6 +313,7 @@ Sim3 Sim3Tracker::trackFrameSim3(TrackingReference* reference, Frame* frame, con
 {
     double init[8];
     sim3ToQts(frameToReference_initialEstimate, init);
+    ActiveFrames held(dev_.frameMemory(), { reference->keyframe, frame });   // Sim3Tracker.cpp:155
     lsdgpu_sim3_result r;
     dev_.check(lsdgpu_sim3_track(dev_.raw(), reference->keyframe->id(), frame->id(), init, startLevel, finalLevel, &settings, &r),
                "Sim3Tracker::trackFrameSim3");
@@ -230,6 +328,9 @@ void Sim3Tracker::trackFrameSim3Batch(const std::vector<TrackingReference*>& ref
     if (frames.size() != n || inits.size() != n) throw LsdGpuError("Sim3Tracker::trackFrameSim3Batch: list lengths differ");
     std::vector<int> refIds(n), frIds(n);
     std::vector<double> q(8 * n);
+    std::vector<Frame*> used;
+    for (size_t i = 0; i < n; i++) { used.push_back(references[i]->keyframe); used.push_back(frames[i]); }
+    ActiveFrames held(dev_.frameMemory(), used);
     for (size_t i = 0; i < n; i++) {
         refIds[i] = references[i]->keyframe->id(); frIds[i] = frames[i]->id();
         sim3ToQts(inits[i], &q[8 * i]);
@@ -351,11 +452,13 @@ void DepthMap::invalidate()
 }
 void DepthMap::initializeFromGTDepth(Frame* new_frame)
 {
+    new_frame->getActiveLock();                                         // DepthMap.cpp:969
     dev_.check(lsdgpu_depth_init_from_gt(dev_.raw(), new_frame->id()), "DepthMap::initializeFromGTDepth");
     activeKeyFrame = new_frame;
 }
 void DepthMap::initializeRandomly(Frame* new_frame)
 {   // DepthMap.cpp:883-916: the rand() draws stay on the host, the hypotheses are uploaded
+    new_frame->getActiveLock();                                         // DepthMap.cpp:885
     std::vector<float> maxGrad((size_t)width_ * height_);
     dev_.check(lsdgpu_frame_download(dev_.raw(), new_frame->id(), LSDGPU_BUF_MAXGRAD, 0, maxGrad.data()), "DepthMap::initializeRandomly");
     lsdgpu_globals g;
@@ -380,6 +483,7 @@ void DepthMap::initializeRandomly(Frame* new_frame)
 }
 void DepthMap::setFromExistingKF(Frame* kf, const float* idepth, const float* idepthVar, const unsigned char* validity)
 {   // DepthMap.cpp:920-962
+    kf->getActiveLock();                                                // DepthMap.cpp:924
     std::vector<lsdgpu_hyp> hyp((size_t)width_ * height_);
     std::memset(hyp.data(), 0, hyp.size() * sizeof(lsdgpu_hyp));
     for (size_t i = 0; i < hyp.size(); i++) {
@@ -399,6 +503,9 @@ void DepthMap::setFromExistingKF(Frame* kf, const float* idepth, const float* id
 void DepthMap::updateKeyframe(std::deque<std::shared_ptr<Frame>> referenceFrames)
 {
     if (!isValid()) throw LsdGpuError("DepthMap::updateKeyframe: assert(isValid())");
+    std::vector<Frame*> used{ activeKeyFrame };
+    for (auto& f : referenceFrames) used.push_back(f.get());            // the device reads their images and masks
+    ActiveFrames held(dev_.frameMemory(), used);
     std::vector<lsdgpu_ref_desc> refs;
     for (auto& f : referenceFrames) {
         if (!f->hasTrackingParent()) throw LsdGpuError("DepthMap::updateKeyframe: assert(frame->hasTrackingParent())");   // :1085
@@ -426,6 +533,7 @@ void DepthMap::createKeyFrame(Frame* new_keyframe)
 {
     if (!isValid()) throw LsdGpuError("DepthMap::createKeyFrame: assert(isValid())");
     if (!new_keyframe || !new_keyframe->hasTrackingParent()) throw LsdGpuError("DepthMap::createKeyFrame: new keyframe has no tracking parent");
+    ActiveFrames held(dev_.frameMemory(), { activeKeyFrame, new_keyframe });   // DepthMap.cpp:1256, :1229
     double qts[8];
     dev_.check(lsdgpu_depth_create_keyframe(dev_.raw(), new_keyframe->id(), qts), "DepthMap::createKeyFrame");
     Sim3 s;
@@ -438,6 +546,7 @@ void DepthMap::createKeyFrame(Frame* new_keyframe)
 void DepthMap::finalizeKeyFrame()
 {
     if (!isValid()) throw LsdGpuError("DepthMap::finalizeKeyFrame: assert(isValid())");
+    activeKeyFrame->getActiveLock();
     dev_.check(lsdgpu_depth_finalize_keyframe(dev_.raw()), "DepthMap::finalizeKeyFrame");
 }
 void DepthMap::download(std::vector<lsdgpu_hyp>& out)

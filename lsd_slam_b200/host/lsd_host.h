@@ -12,7 +12,10 @@
 #pragma once
 
 #include <deque>
+#include <initializer_list>
+#include <list>
 #include <memory>
+#include <mutex>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -62,6 +65,48 @@ public:
     explicit LsdGpuError(const std::string& what) : std::runtime_error(what) {}
 };
 
+class Frame;
+class DeviceContext;
+
+// DataStructures/FrameMemory.h: the active-frame list of FrameMemory (FrameMemory.cpp:129-166), one per DeviceContext.  The
+// reference's heap is unbounded; a context has max_frames slots, so activating a frame (or constructing one) with every slot
+// taken first minimizes the least recently activated frame that is neither the depth map's active keyframe nor held by a call
+// in progress (ActiveFrames).  A call that needs more frames than that leaves free throws LsdGpuError.
+class FrameMemory {
+public:
+    FrameMemory(DeviceContext& dev, int maxActive);
+    void activateFrame(Frame* frame);                   // FrameMemory.cpp:129-137 + Frame::require (lsdgpu_frame_activate)
+    void deactivateFrame(Frame* frame);                 // FrameMemory.cpp:138-147
+    void pruneActiveFrames();                           // FrameMemory.cpp:149-166: at most maxActive frames stay active
+    int maxActiveFrames() const { return maxActive_; }
+    void setMaxActiveFrames(int n) { maxActive_ = n; }
+
+private:
+    friend class Frame;
+    friend class ActiveFrames;
+    void makeRoom();                                    // a free slot for one more active frame
+    void minimizeLeastRecent();
+    DeviceContext& dev_;
+    int maxActive_;
+    std::list<Frame*> activeFrames;                     // most recently activated first
+    std::vector<Frame*> held_;                          // frames of the calls in progress (ActiveFrames)
+    std::recursive_mutex mu_;                           // FrameMemory::activeFramesMutex (tracking and mapping threads)
+};
+
+// The frames one device call reads, activated and kept in their slots until the call returns (the shared active locks the
+// reference holds for the duration of trackFrame, updateKeyframe, ..., Frame.h:138-141)
+class ActiveFrames {
+public:
+    ActiveFrames(FrameMemory& memory, std::initializer_list<Frame*> frames);
+    ActiveFrames(FrameMemory& memory, const std::vector<Frame*>& frames);
+    ~ActiveFrames();
+    ActiveFrames(const ActiveFrames&) = delete;
+
+private:
+    FrameMemory& memory_;
+    size_t n_ = 0;
+};
+
 // One device context per SlamSystem (SlamSystem owns one SE3Tracker + one DepthMap, SlamSystem.h:126,131)
 class DeviceContext {
 public:
@@ -73,10 +118,14 @@ public:
     void check(int rc, const char* where) const;
     int width() const { return w_; }
     int height() const { return h_; }
+    int maxFrames() const { return maxFrames_; }
+    // bound of pruneActiveFrames: maxLoopClosureCandidates + 20 (util/settings.cpp:97)
+    FrameMemory& frameMemory() { return *memory_; }
 
 private:
     lsdgpu_ctx* ctx_ = nullptr;
-    int w_, h_;
+    int w_, h_, maxFrames_;
+    std::unique_ptr<FrameMemory> memory_;
 };
 
 // FramePoseStruct, DataStructures/FramePoseStruct.h (the two members the path touches)
@@ -112,14 +161,22 @@ public:
     // buffers for callers that still need host copies (e.g. Output3DWrapper): explicit downloads
     void downloadIdepth(int level, std::vector<float>& idepth, std::vector<float>& idepthVar);
     void downloadRefPixelWasGood(std::vector<unsigned char>& mask);
+    // Frame.cpp:377-395: frees the slot; level 0, the reactivation data and the permaRef stay (lsdgpu_frame_minimize).  Goes
+    // through FrameMemory::deactivateFrame so that the next getActiveLock activates the frame again.
+    bool minimizeInMemory();
+    // Frame.h:138-141: makes the frame active (FrameMemory::activateFrame); the device's calls need the frame in a slot
+    void getActiveLock();
 
     FramePoseStruct* pose;
+    bool isActive = true;
     float initialTrackedResidual = 0;
     int numFramesTrackedOnThis = 0, numMappedOnThis = 0, numMappedOnThisTotal = 0;
 
     DeviceContext& dev() const { return dev_; }
 
 private:
+    friend class FrameMemory;
+    void minimizeOnDevice();
     DeviceContext& dev_;
     int id_, w_, h_;
     double timestamp_;

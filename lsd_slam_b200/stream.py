@@ -13,7 +13,9 @@ times and what the full-loop parity tests run.  ``fused_call=True`` issues the w
 
 The stream keeps the ids of its keyframes and their camToWorld, chained from the thisToParent Sim3 that createKeyFrame returns
 (odometry: no pose graph), so that ``ctx.export_pointcloud(stream.keyframe_ids, stream.keyframe_cam_to_world_f7())`` is the
-viewer's map of the run.  With ``keep_keyframes=True`` finished keyframes stay resident (the context needs a frame slot for each).
+viewer's map of the run.  With ``keep_keyframes=True`` finished keyframes stay resident (the context needs a frame slot for each);
+adding ``max_active_keyframes=k`` keeps only the newest k finished keyframes in frame slots and minimizes the older ones after each
+keyframe change (``Context.minimize``, FrameMemory::pruneActiveFrames, FrameMemory.cpp:149-166), so the map can outgrow max_frames.
 
 ``GpuStreamGroup`` steps K such streams (one context each, same GPU) with ONE call per frame
 (``lsdgpu_track_and_map_group``): the trackings of the K frames share one launch, each stream on its own slice of the SMs.
@@ -62,9 +64,12 @@ def qts_to_sim3f(qts) -> np.ndarray:
 
 class GpuStream:
     def __init__(self, ctx: abi.Context, mode: int = 1, kf_every: int = 20, fused_call: bool = True, kf_phase: int = 0,
-                 keep_keyframes: bool = False):
+                 keep_keyframes: bool = False, max_active_keyframes: int | None = None):
+        if max_active_keyframes is not None and (not keep_keyframes or max_active_keyframes < 0):
+            raise ValueError("max_active_keyframes needs keep_keyframes=True and a count >= 0")
         self.ctx = ctx
         self.keep_keyframes = keep_keyframes
+        self.max_active_keyframes = max_active_keyframes
         self.keyframe_ids: list[int] = []          # every keyframe of the run, oldest first
         self.keyframe_cam_to_world: list[np.ndarray] = []   # their camToWorld as qts[8], the first keyframe at the origin
         self.kf_phase = kf_phase          # shifts the forced keyframe changes: frame n changes keyframe when (n + kf_phase) % kf_every == 0
@@ -157,6 +162,10 @@ class GpuStream:
             for i in self.prev_ids + ([] if self.keep_keyframes else [old_kf]):
                 ctx.release(i)
             self.prev_ids = []
+            if self.max_active_keyframes is not None:
+                finished = self.keyframe_ids[:-1]
+                for i in finished[:max(0, len(finished) - self.max_active_keyframes)]:
+                    ctx.minimize(i)             # a no-op for a keyframe that is minimized already; one the caller re-activated goes again
         else:
             self.last_pose = pose
             self.prev_ids.append(fid)
