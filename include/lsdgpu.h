@@ -10,7 +10,7 @@
  * adapter classes in lsd_slam_b200/host/ keep the reference's method names on top of this ABI;
  * INTEGRATION.md shows the binding a maintainer adds to lsd_slam_core.
  *
- * Conventions: extern "C", POD only, caller-owned HOST buffers, opaque context, int return
+ * Conventions: extern "C", POD only, caller-owned HOST buffers (DEVICE buffers for the *_device entry points), opaque context, int return
  * (0 = ok, negative = error, text via lsdgpu_last_error), never throws.  One context owns one CUDA
  * stream and all device state of one SlamSystem (one tracker + one depth map); contexts are independent
  * and thread-compatible (SlamSystem runs tracking and mapping on different threads: calls into ONE
@@ -306,6 +306,44 @@ int lsdgpu_map_export_pointcloud(lsdgpu_ctx* ctx, int n, const int* kf_ids, cons
 /* device time (CUDA events, ms) from the start of the first kernel of the last lsdgpu_map_export_pointcloud call to the end of its
  * last kernel (the copies of a batched call run between them); for benchmarks, KeyFrameDisplay.cpp:106-222 */
 int lsdgpu_cloud_last_kernel_ms(lsdgpu_ctx* ctx, float* ms);
+/* ---- device-resident input and output, ordered on the caller's CUDA stream ------------------------------------------------
+ * Found by symbol lookup (dlsym), like lsdgpu_track_and_map_group; LSDGPU_ABI_VERSION is unchanged.  Each *_device entry point
+ * below does what its host twin does, with the same errors, but takes its image from or writes its result to DEVICE memory, so
+ * that a frame decoded on the GPU (e.g. the luma plane of a video decoder) and a GPU consumer of the results (a CUDA-registered
+ * vertex buffer, a tensor) never pass through host memory.
+ *   stream   the caller's cudaStream_t; NULL = the legacy default stream.  The call behaves as if its device work ran on
+ *            `stream`: it starts after everything the caller enqueued on `stream` before the call, and work the caller enqueues on
+ *            `stream` after the call returns starts after the call has read its inputs and written its outputs.  (The context
+ *            records an event on `stream` that its own stream waits on, and after its work an event on its own stream that
+ *            `stream` waits on.)  The host does not wait for the device, except lsdgpu_map_export_pointcloud_device for the
+ *            point count it returns.
+ *   pointers d_* must be device or managed memory of the context's device (checked with cudaPointerGetAttributes).  Images have
+ *            a row pitch in bytes >= their width (any value, odd included); an image must stay valid and unchanged until the
+ *            call's work on `stream` is done.  Outputs have an explicit capacity and an alignment (below).  Frame ids,
+ *            keyframe lists, camToWorld, filters and counts stay HOST memory.
+ *   errors   every argument is checked before anything is changed: a rejected call acquires no frame slot, writes no byte
+ *            and leaves a message in lsdgpu_last_error.
+ * Frame::Frame(id,w,h,K,ts,const uchar*) Frame.cpp:35-54 + buildImage / buildGradients / buildMaxGradients, as lsdgpu_frame_upload_u8,
+ * from a device image of w x h bytes with row pitch pitch_bytes */
+int lsdgpu_frame_upload_device_u8(lsdgpu_ctx* ctx, int frame_id, const uint8_t* d_gray, size_t pitch_bytes, void* stream);
+/* UndistorterPTAM::undistort (util/Undistorter.cpp:355-411) or UndistorterOpenCV::undistort (:564-567) + Frame::Frame, as
+ * lsdgpu_frame_upload_distorted_u8, from a device raw image of the installed undistorter's in_width x in_height bytes */
+int lsdgpu_frame_upload_distorted_device_u8(lsdgpu_ctx* ctx, int frame_id, const uint8_t* d_raw, size_t pitch_bytes, void* stream);
+/* the prefetch ring's lsdgpu_stage_put (raw frames ahead of Frame::Frame, Frame.cpp:35-54) from a device image; unlike
+ * lsdgpu_stage_put it does not wait for the device.  lsdgpu_frame_from_stage, lsdgpu_track_and_map and lsdgpu_track_and_map_group
+ * take the entry through stage_index as before. */
+int lsdgpu_stage_put_device(lsdgpu_ctx* ctx, int index, const uint8_t* d_gray, size_t pitch_bytes, void* stream);
+/* lsdgpu_frame_download (Frame::image / gradients / maxGradients / idepth / idepthVar / refPixelWasGood, Frame.h:102-114) into
+ * device memory: a device-to-device copy of the same plane.  capacity_bytes >= the plane's size; d_out aligned to its element
+ * (4 bytes, 16 for LSDGPU_BUF_GRADIENTS). */
+int lsdgpu_frame_download_device(lsdgpu_ctx* ctx, int frame_id, int what, int level, void* d_out, size_t capacity_bytes, void* stream);
+/* lsdgpu_map_export_pointcloud (KeyFrameDisplay::refreshPC + flushPC, KeyFrameDisplay.cpp:106-222, :269-339) written straight into
+ * d_out (16-byte aligned, capacity_points records; NULL to only count) by one launch over all n keyframes.  Needs no
+ * lsdgpu_cloud_reserve: its descriptors and scratch come from a memory pool of the context in stream order.  Waits for the device
+ * to return *n_points_out and counts; leaves lsdgpu_cloud_last_kernel_ms unchanged. */
+int lsdgpu_map_export_pointcloud_device(lsdgpu_ctx* ctx, int n, const int* kf_ids, const float* camToWorld, int level,
+                                        const lsdgpu_cloud_filter* f, int layout, void* d_out, int64_t capacity_points,
+                                        int64_t* n_points_out, int32_t* counts, void* stream);
 /* Frame::takeReActivationData(currentDepthMap), DataStructures/Frame.cpp:107-145: snapshot of the ACTIVE depth map into the
  * keyframe's idepth_reAct / idepthVar_reAct / validity_reAct -- kept on the device.  lsdgpu_depth_finalize_keyframe calls it
  * (DepthMap.cpp:1387); exposed for re-activation bookkeeping outside finalize. */

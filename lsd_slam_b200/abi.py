@@ -183,6 +183,12 @@ SYMBOLS = [
     ("lsdgpu_map_export_pointcloud", C.c_int, [_vp, C.c_int, _ip, _fp, C.c_int, C.c_void_p, C.c_int, _vp, C.c_int64,
                                                C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     ("lsdgpu_cloud_last_kernel_ms", C.c_int, [_vp, _fp]),
+    ("lsdgpu_frame_upload_device_u8", C.c_int, [_vp, C.c_int, _vp, C.c_size_t, _vp]),
+    ("lsdgpu_frame_upload_distorted_device_u8", C.c_int, [_vp, C.c_int, _vp, C.c_size_t, _vp]),
+    ("lsdgpu_stage_put_device", C.c_int, [_vp, C.c_int, _vp, C.c_size_t, _vp]),
+    ("lsdgpu_frame_download_device", C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, _vp]),
+    ("lsdgpu_map_export_pointcloud_device", C.c_int, [_vp, C.c_int, _ip, _fp, C.c_int, C.c_void_p, C.c_int, _vp, C.c_int64,
+                                                      C.POINTER(C.c_int64), C.POINTER(C.c_int32), _vp]),
     ("lsdgpu_frame_take_reactivation_data", C.c_int, [_vp, C.c_int]),
     ("lsdgpu_frame_download_reactivation_data", C.c_int, [_vp, C.c_int, _fp, _fp, C.POINTER(C.c_uint8)]),
     ("lsdgpu_depth_set_from_existing_kf", C.c_int, [_vp, C.c_int]),
@@ -242,6 +248,38 @@ class LsdGpuError(RuntimeError):
     pass
 
 
+def _is_tensor(x) -> bool:
+    """x is a torch.Tensor; decided without importing torch, so that numpy callers never load it"""
+    return type(x).__module__.split(".")[0] == "torch"
+
+
+def _tensor_dtype(t, dtype: str, what: str):
+    import torch
+    if t.dtype != getattr(torch, dtype):
+        raise ValueError(f"{what}: needs torch.{dtype}, not {t.dtype}")
+
+
+def _cuda_stream(t, device: int, what: str) -> int:
+    """checks that t is a CUDA tensor on the context's device -> the handle of that device's current stream (0 = the legacy default
+    stream), on which the *_device entry points order their work"""
+    import torch
+    if not t.is_cuda:
+        raise ValueError(f"{what}: needs a CUDA tensor, not one on {t.device}")
+    if t.device.index != device:
+        raise ValueError(f"{what}: the tensor is on {t.device}, the context on cuda:{device}")
+    return torch.cuda.current_stream(t.device).cuda_stream
+
+
+def _device_image(t, device: int, w: int, h: int, what: str):
+    """a 2-D uint8 CUDA tensor of h x w whose rows are contiguous -> (pointer, row pitch in bytes, stream)"""
+    _tensor_dtype(t, "uint8", what)
+    if t.dim() != 2 or tuple(t.shape) != (h, w):
+        raise ValueError(f"{what}: needs shape ({h}, {w}), not {tuple(t.shape)}")
+    if t.stride(1) != 1 or t.stride(0) < w:
+        raise ValueError(f"{what}: needs contiguous rows (stride(1) == 1, stride(0) >= {w}), not strides {t.stride()}")
+    return t.data_ptr(), t.stride(0), _cuda_stream(t, device, what)
+
+
 class UndistorterPTAM:
     """Mirror of lsd_slam::UndistorterPTAM (util/Undistorter.h:96-160) with the calibration file's lines already parsed.
     out_calib: "crop", "full" or (fx, fy, cx, cy, 0).  Host-only; `install(ctx)` puts the tables on the device."""
@@ -274,6 +312,7 @@ class UndistorterPTAM:
             ctx._ck(ctx.L.lsdgpu_set_undistorter(ctx.ptr, self.in_w, self.in_h, None, None))
         else:
             ctx._ck(ctx.L.lsdgpu_set_undistorter(ctx.ptr, self.in_w, self.in_h, self.remapX.ctypes.data_as(_fp), self.remapY.ctypes.data_as(_fp)))
+        ctx.raw_size = (self.in_w, self.in_h)
 
 
 class UndistorterOpenCV:
@@ -310,6 +349,7 @@ class UndistorterOpenCV:
         assert (ctx.w, ctx.h) == (self.out_w, self.out_h)
         ctx._ck(ctx.L.lsdgpu_set_undistorter_opencv(ctx.ptr, self.in_w, self.in_h, self.map1.ctypes.data_as(C.POINTER(C.c_int16)),
                                                     self.map2.ctypes.data_as(C.POINTER(C.c_uint16))))
+        ctx.raw_size = (self.in_w, self.in_h)
 
 
 def default_track_settings(main_tracker: bool = True) -> TrackSettings:
@@ -327,6 +367,8 @@ class Context:
     def __init__(self, w: int, h: int, K: np.ndarray, device: int = 0, max_frames: int = 8, **globals_kw):
         self.L = load()
         self.w, self.h = w, h
+        self.device = device
+        self.raw_size = None                  # (in_width, in_height) of the installed undistorter
         self.K = np.ascontiguousarray(K, np.float32).reshape(3, 3)
         p = _vp()
         rc = self.L.lsdgpu_create(device, w, h, self.K.ctypes.data_as(_fp), max_frames, C.byref(p))
@@ -388,7 +430,13 @@ class Context:
         return ms.value, n.value, b.value
 
     # ---- Frame ----
-    def upload(self, fid: int, image_u8: np.ndarray):
+    def upload(self, fid: int, image_u8):
+        """Frame::Frame from a host image (numpy), or from a 2-D uint8 CUDA tensor with contiguous rows (its row stride is the
+        pitch), ordered on the tensor's current stream (lsdgpu_frame_upload_device_u8)"""
+        if _is_tensor(image_u8):
+            ptr, pitch, stream = _device_image(image_u8, self.device, self.w, self.h, "upload")
+            self._ck(self.L.lsdgpu_frame_upload_device_u8(self.ptr, fid, ptr, pitch, stream))
+            return
         img = np.ascontiguousarray(image_u8, np.uint8)
         assert img.shape == (self.h, self.w)
         self._ck(self.L.lsdgpu_frame_upload_u8(self.ptr, fid, img.ctypes.data_as(_u8p)))
@@ -396,7 +444,13 @@ class Context:
     def stage_reserve(self, n: int):
         self._ck(self.L.lsdgpu_stage_reserve(self.ptr, n))
 
-    def stage_put(self, index: int, image_u8: np.ndarray):
+    def stage_put(self, index: int, image_u8):
+        """one frame into prefetch-ring entry `index`: a host image (numpy), or a CUDA tensor as `upload` takes it
+        (lsdgpu_stage_put_device, which does not wait for the device)"""
+        if _is_tensor(image_u8):
+            ptr, pitch, stream = _device_image(image_u8, self.device, self.w, self.h, "stage_put")
+            self._ck(self.L.lsdgpu_stage_put_device(self.ptr, index, ptr, pitch, stream))
+            return
         img = np.ascontiguousarray(image_u8, np.uint8)
         self._ck(self.L.lsdgpu_stage_put(self.ptr, index, img.ctypes.data_as(_u8p)))
 
@@ -415,14 +469,26 @@ class Context:
         """FrameMemory::activateFrame + Frame::require (lsdgpu_frame_activate): a minimized frame takes a free slot again"""
         self._ck(self.L.lsdgpu_frame_activate(self.ptr, fid))
 
-    def download(self, fid: int, what: int, level: int = 0) -> np.ndarray:
+    def download(self, fid: int, what: int, level: int = 0, out=None):
+        """one plane of a frame as a numpy array, or -- out = a contiguous CUDA tensor (float32; uint8 for BUF_GOODMASK) of at
+        least the plane's size -- copied on the device into out, ordered on its current stream; returns a view of out
+        (lsdgpu_frame_download_device)"""
         w, h = self.w >> level, self.h >> level
         if what == BUF_GRADIENTS:
-            out = np.empty((h, w, 4), np.float32)
+            shape, dtype = (h, w, 4), np.float32
         elif what == BUF_GOODMASK:
-            out = np.empty((self.h >> 1, self.w >> 1), np.uint8)
+            shape, dtype = (self.h >> 1, self.w >> 1), np.uint8
         else:
-            out = np.empty((h, w), np.float32)
+            shape, dtype = (h, w), np.float32
+        if out is not None:
+            _tensor_dtype(out, "uint8" if dtype == np.uint8 else "float32", "download(out=)")
+            n = int(np.prod(shape))
+            if not out.is_contiguous() or out.numel() < n:
+                raise ValueError(f"download(out=): needs a contiguous tensor of at least {n} elements")
+            stream = _cuda_stream(out, self.device, "download(out=)")
+            self._ck(self.L.lsdgpu_frame_download_device(self.ptr, fid, what, level, out.data_ptr(), out.numel() * out.element_size(), stream))
+            return out.reshape(-1)[:n].view(shape)
+        out = np.empty(shape, dtype)
         self._ck(self.L.lsdgpu_frame_download(self.ptr, fid, what, level, out.ctypes.data_as(_vp)))
         return out
 
@@ -496,8 +562,15 @@ class Context:
         self._ck(self.L.lsdgpu_undistort_u8(self.ptr, raw.ctypes.data_as(C.POINTER(C.c_uint8)), out.ctypes.data_as(C.POINTER(C.c_uint8))))
         return out
 
-    def upload_distorted(self, fid: int, raw_u8: np.ndarray):
-        """undistort (either model) + Frame construction fused (one H2D copy of the raw image, remap feeds the pyramid kernel)"""
+    def upload_distorted(self, fid: int, raw_u8):
+        """undistort (either model) + Frame construction fused (one H2D copy of the raw image, remap feeds the pyramid kernel).
+        raw_u8 may be a CUDA tensor as `upload` takes it, of the undistorter's input size (lsdgpu_frame_upload_distorted_device_u8)"""
+        if _is_tensor(raw_u8):
+            if self.raw_size is None:
+                raise ValueError("upload_distorted: no undistorter installed")
+            ptr, pitch, stream = _device_image(raw_u8, self.device, *self.raw_size, "upload_distorted")
+            self._ck(self.L.lsdgpu_frame_upload_distorted_device_u8(self.ptr, fid, ptr, pitch, stream))
+            return
         raw = np.ascontiguousarray(raw_u8, np.uint8)
         self._ck(self.L.lsdgpu_frame_upload_distorted_u8(self.ptr, fid, raw.ctypes.data_as(C.POINTER(C.c_uint8))))
 
@@ -518,12 +591,25 @@ class Context:
         filter: CloudFilter, dict of its fields, or None (the viewer's defaults).  Returns (points, counts): points in keyframe
         order (CLOUD_PLY_DTYPE world points + intensity, or CLOUD_VERTEX_DTYPE camera points + colour), counts = (n, 2) int32
         totalPoints, displayedPoints.  Needs cloud_reserve first.  capacity=None sizes the output for every interior pixel;
-        out = a caller's array of the layout's dtype to fill instead (its length is the capacity; the points are a view of it)."""
+        out = a caller's array of the layout's dtype to fill instead (its length is the capacity; the points are a view of it).
+        out = a contiguous float32 CUDA tensor of shape (capacity, 4): the points are written there on the device, ordered on its
+        current stream, in one launch and without a reservation (lsdgpu_map_export_pointcloud_device); points = a view of out."""
         ids = np.ascontiguousarray(kf_ids, np.int32).reshape(-1)
         n = len(ids)
         c2w = np.ascontiguousarray(camToWorld, np.float32).reshape(n, 7)
         if filter is None or isinstance(filter, dict):
             filter = default_cloud_filter(**(filter or {}))
+        if out is not None and _is_tensor(out):
+            _tensor_dtype(out, "float32", "export_pointcloud(out=)")
+            if out.dim() != 2 or out.shape[1] != 4 or not out.is_contiguous():
+                raise ValueError(f"export_pointcloud(out=): needs a contiguous (capacity, 4) tensor, not {tuple(out.shape)}")
+            stream = _cuda_stream(out, self.device, "export_pointcloud(out=)")
+            counts = np.zeros((n, 2), np.int32)
+            npts = C.c_int64(0)
+            self._ck(self.L.lsdgpu_map_export_pointcloud_device(self.ptr, n, ids.ctypes.data_as(_ip), c2w.ctypes.data_as(_fp), level,
+                                                                C.byref(filter), layout, out.data_ptr(), out.shape[0], C.byref(npts),
+                                                                counts.ctypes.data_as(C.POINTER(C.c_int32)), stream))
+            return out[:npts.value], counts
         wl, hl = self.w >> level, self.h >> level
         if out is None:
             if capacity is None:

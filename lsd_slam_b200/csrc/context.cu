@@ -140,6 +140,8 @@ extern "C" int lsdgpu_create(int device, int width, int height, const float K[9]
     LSD_CHECK(ctx, cudaHostAlloc((void**)&ctx->hScalars, 64, cudaHostAllocDefault));
     LSD_CHECK(ctx, cudaHostAlloc(&ctx->hGroupSegs, TP_MAX_GROUP * sizeof(TrackGroupSeg), cudaHostAllocDefault));
     LSD_CHECK(ctx, cudaEventCreateWithFlags(&ctx->groupEvent, cudaEventDisableTiming));
+    LSD_CHECK(ctx, cudaEventCreateWithFlags(&ctx->callerIn, cudaEventDisableTiming));
+    LSD_CHECK(ctx, cudaEventCreateWithFlags(&ctx->callerOut, cudaEventDisableTiming));
     // the tracker writes its result block straight into mapped pinned memory (no D2H copy on the path)
     LSD_CHECK(ctx, cudaHostAlloc((void**)&ctx->hTrackState, sizeof(TrackState), cudaHostAllocMapped));
     // cudaHostAlloc does not clear: a recycled block may still hold the result of a destroyed context, whose doneSeq would satisfy
@@ -183,6 +185,8 @@ extern "C" void lsdgpu_destroy(lsdgpu_ctx* ctx)
     cudaFreeHost(ctx->hScalars); cudaFreeHost(ctx->hTrackState);
     if (ctx->hGroupSegs) cudaFreeHost(ctx->hGroupSegs);
     if (ctx->groupEvent) cudaEventDestroy(ctx->groupEvent);
+    if (ctx->callerIn) cudaEventDestroy(ctx->callerIn);
+    if (ctx->callerOut) cudaEventDestroy(ctx->callerOut);
     for (int i = 0; i < 8; i++) { if (ctx->tBegin[i]) cudaEventDestroy(ctx->tBegin[i]); if (ctx->tEnd[i]) cudaEventDestroy(ctx->tEnd[i]); }
     if (ctx->kBegin) cudaEventDestroy(ctx->kBegin);
     if (ctx->kEnd) cudaEventDestroy(ctx->kEnd);

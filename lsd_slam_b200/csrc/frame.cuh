@@ -17,19 +17,21 @@
 // SlamSystem.cpp:55).  The 2x2 box sum is exact in fp32 for u8-origin data (SURVEY App. A-11) and is
 // associated like the scalar loop (Frame.cpp:621-624).
 // SRC = PYR_PTAM fuses UndistorterPTAM::undistort (util/Undistorter.cpp:380-410) in front: level 0 is gathered bilinearly from
-// the RAW (distorted, in_w wide) image through the remap tables, truncated to 8 bits exactly as the reference's
+// the RAW (distorted) image through the remap tables, truncated to 8 bits exactly as the reference's
 // `data[idx] = float expression` does, and converted to float as Frame::Frame does (Frame.cpp:44-52) -- the undistorted u8 image
 // never exists in memory unless `undist` is given (parity hook / host consumers).  SRC = PYR_OPENCV does the same with
 // UndistorterOpenCV's fixed-point remap (remapPixelOpenCV, maps map1 / map2, raw image in_w x in_h).
-__device__ __forceinline__ unsigned char undistortPixel(const uint8_t* __restrict__ raw, int in_w, float xx, float yy)
+// `pitch` is the row stride of the source image in bytes: its width for the library's own staging copies, any value >= the
+// width for a caller's device image (lsdgpu_frame_upload_device_u8 and its siblings; it may be odd, so loads are bytewise).
+__device__ __forceinline__ unsigned char undistortPixel(const uint8_t* __restrict__ raw, int pitch, float xx, float yy)
 {
     if (xx < 0) return 0;
     const int xxi = (int)xx, yyi = (int)yy;
     xx -= xxi;
     yy -= yyi;
     const float xxyy = xx * yy;
-    const uint8_t* src = raw + xxi + yyi * in_w;
-    const float v = xxyy * src[1 + in_w] + (yy - xxyy) * src[in_w] + (xx - xxyy) * src[1] + (1 - xx - yy + xxyy) * src[0];
+    const uint8_t* src = raw + xxi + yyi * pitch;
+    const float v = xxyy * src[1 + pitch] + (yy - xxyy) * src[pitch] + (xx - xxyy) * src[1] + (1 - xx - yy + xxyy) * src[0];
     return (unsigned char)v;
 }
 // UndistorterOpenCV::undistort (util/Undistorter.cpp:564-567) = cv::remap(image, result, map1, map2, INTER_LINEAR) with the default
@@ -37,23 +39,25 @@ __device__ __forceinline__ unsigned char undistortPixel(const uint8_t* __restric
 // The 2x2 weights are OpenCV's 15-bit fixed-point bilinear table, (32 - fx) * (32 - fy) * 32 ... (exact, they sum to 32768); a
 // tap outside the in_w x in_h image contributes 0; the sum is rounded as OpenCV's fixed-point cast, (sum + 2^14) >> 15.  Every
 // tap is bounds-checked, so any pair of maps is safe to install.
-__device__ __forceinline__ unsigned char remapPixelOpenCV(const uint8_t* __restrict__ raw, int in_w, int in_h, short2 m1, unsigned int m2)
+__device__ __forceinline__ unsigned char remapPixelOpenCV(const uint8_t* __restrict__ raw, int in_w, int in_h, int pitch, short2 m1,
+                                                          unsigned int m2)
 {
     const int sx = m1.x, sy = m1.y;
     const int fx = m2 & 31, fy = (m2 >> 5) & 31;          // cv::remap reads map2 & (INTER_TAB_SIZE2 - 1)
     const bool x0 = sx >= 0 && sx < in_w, x1 = sx + 1 >= 0 && sx + 1 < in_w;
     const bool y0 = sy >= 0 && sy < in_h, y1 = sy + 1 >= 0 && sy + 1 < in_h;
-    const uint8_t* s = raw + (ptrdiff_t)sy * in_w + sx;
+    const uint8_t* s = raw + (ptrdiff_t)sy * pitch + sx;
     const int p00 = (x0 && y0) ? __ldg(s) : 0, p01 = (x1 && y0) ? __ldg(s + 1) : 0;
-    const int p10 = (x0 && y1) ? __ldg(s + in_w) : 0, p11 = (x1 && y1) ? __ldg(s + in_w + 1) : 0;
+    const int p10 = (x0 && y1) ? __ldg(s + pitch) : 0, p11 = (x1 && y1) ? __ldg(s + pitch + 1) : 0;
     const int v = p00 * ((32 - fx) * (32 - fy) * 32) + p01 * (fx * (32 - fy) * 32) + p10 * ((32 - fx) * fy * 32) + p11 * (fx * fy * 32);
     return (unsigned char)((v + (1 << 14)) >> 15);
 }
 // source of level 0 of k_image_pyramid: the u8 image itself, or a raw image through UndistorterPTAM's / UndistorterOpenCV's tables,
 // or (PYR_F32) the fp32 level 0 kept in a minimized frame's record (Frame::require after minimizeInMemory, Frame.cpp:319-338)
 enum { PYR_U8 = 0, PYR_PTAM = 1, PYR_OPENCV = 2, PYR_F32 = 3 };
+// src_pitch = the row stride in bytes of src (PYR_U8, PYR_PTAM, PYR_OPENCV); PYR_F32 reads w floats per row.
 template <int SRC>
-__global__ void __launch_bounds__(256) k_image_pyramid(const uint8_t* __restrict__ src, PyrPtrs p, int w, int h,
+__global__ void __launch_bounds__(256) k_image_pyramid(const uint8_t* __restrict__ src, int src_pitch, PyrPtrs p, int w, int h,
                                                        const float* __restrict__ remapX = nullptr, const float* __restrict__ remapY = nullptr,
                                                        int in_w = 0, uint8_t* __restrict__ undist = nullptr,
                                                        const short2* __restrict__ map1 = nullptr, const uint16_t* __restrict__ map2 = nullptr,
@@ -67,12 +71,12 @@ __global__ void __launch_bounds__(256) k_image_pyramid(const uint8_t* __restrict
     if (SRC == PYR_F32)
         v = reinterpret_cast<const float*>(src)[y * w + x];
     else if (SRC != PYR_U8) {
-        const unsigned char u = SRC == PYR_PTAM ? undistortPixel(src, in_w, __ldg(remapX + y * w + x), __ldg(remapY + y * w + x))
-                                                : remapPixelOpenCV(src, in_w, in_h, map1[y * w + x], __ldg(map2 + y * w + x));
+        const unsigned char u = SRC == PYR_PTAM ? undistortPixel(src, src_pitch, __ldg(remapX + y * w + x), __ldg(remapY + y * w + x))
+                                                : remapPixelOpenCV(src, in_w, in_h, src_pitch, map1[y * w + x], __ldg(map2 + y * w + x));
         if (undist) undist[y * w + x] = u;
         v = (float)u;
     } else
-        v = (float)src[y * w + x];
+        v = (float)src[y * src_pitch + x];
     p.l[0][y * w + x] = v;
     s0[ty][tx] = v;
     __syncthreads();
@@ -271,7 +275,7 @@ __global__ void __launch_bounds__(256) k_undistort_opencv(const uint8_t* __restr
                                                           const uint16_t* __restrict__ map2, int n, uint8_t* __restrict__ out)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = remapPixelOpenCV(raw, in_w, in_h, map1[i], __ldg(map2 + i));
+    if (i < n) out[i] = remapPixelOpenCV(raw, in_w, in_h, in_w, map1[i], __ldg(map2 + i));
 }
 
 // The copies of lsdgpu_frame_minimize (slot -> record) and lsdgpu_frame_activate (record -> slot): up to REC_MAX_SEGS buffers of

@@ -32,7 +32,7 @@ static FrameSlot* acquireSlot(lsdgpu_ctx* ctx, int id)
     return nullptr;
 }
 
-static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int src = PYR_U8);
+static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int pitch, int src = PYR_U8);
 
 extern "C" int lsdgpu_frame_upload_u8(lsdgpu_ctx* ctx, int frame_id, const uint8_t* gray)
 { LSD_LOCK(ctx);
@@ -50,7 +50,7 @@ extern "C" int lsdgpu_frame_upload_u8(lsdgpu_ctx* ctx, int frame_id, const uint8
     const bool pinned = cudaPointerGetAttributes(&pa, gray) == cudaSuccess && pa.type == cudaMemoryTypeHost;
     if (!pinned) { cudaGetLastError(); memcpy(ctx->hStage[b], gray, n0); }
     LSD_CHECK(ctx, cudaMemcpyAsync(ctx->dStageU8[b], pinned ? gray : ctx->hStage[b], n0, cudaMemcpyHostToDevice, ctx->stream));
-    int r = buildFrameFromDeviceU8(ctx, s, ctx->dStageU8[b]);
+    int r = buildFrameFromDeviceU8(ctx, s, ctx->dStageU8[b], ctx->w);
     LSD_CHECK(ctx, cudaEventRecord(ctx->stageDone[b], ctx->stream));
     return r;
 }
@@ -82,19 +82,45 @@ extern "C" int lsdgpu_frame_from_stage(lsdgpu_ctx* ctx, int frame_id, int index)
     if (index < 0 || index >= ctx->stageEntries) return lsd_fail(ctx, "bad ring index");
     FrameSlot* s = acquireSlot(ctx, frame_id);
     if (!s) return failMissing(ctx, frame_id, "no free frame slot (release frames or raise max_frames)");
-    return buildFrameFromDeviceU8(ctx, s, ctx->stageRing + (size_t)index * ctx->w * ctx->h);
+    return buildFrameFromDeviceU8(ctx, s, ctx->stageRing + (size_t)index * ctx->w * ctx->h, ctx->w);
 }
 
-static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int src)
+extern "C" int lsdgpu_frame_upload_device_u8(lsdgpu_ctx* ctx, int frame_id, const uint8_t* d_gray, size_t pitch, void* stream)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    int r = checkDeviceImage(ctx, "frame_upload_device_u8", d_gray, pitch, ctx->w, ctx->h);
+    if (r) return r;
+    FrameSlot* s = acquireSlot(ctx, frame_id);
+    if (!s) return failMissing(ctx, frame_id, "no free frame slot (release frames or raise max_frames)");
+    LSD_CHECK(ctx, afterCallerStream(ctx, stream));
+    if ((r = buildFrameFromDeviceU8(ctx, s, d_gray, (int)pitch))) return r;
+    LSD_CHECK(ctx, beforeCallerStream(ctx, stream));
+    return 0;
+}
+extern "C" int lsdgpu_stage_put_device(lsdgpu_ctx* ctx, int index, const uint8_t* d_gray, size_t pitch, void* stream)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    if (index < 0 || index >= ctx->stageEntries) return lsd_fail(ctx, "bad ring index");
+    int r = checkDeviceImage(ctx, "stage_put_device", d_gray, pitch, ctx->w, ctx->h);
+    if (r) return r;
+    LSD_CHECK(ctx, afterCallerStream(ctx, stream));
+    LSD_CHECK(ctx, cudaMemcpy2DAsync(ctx->stageRing + (size_t)index * ctx->w * ctx->h, ctx->w, d_gray, pitch, ctx->w, ctx->h,
+                                     cudaMemcpyDefault, ctx->stream));
+    LSD_CHECK(ctx, beforeCallerStream(ctx, stream));
+    return 0;
+}
+
+// dsrc: the u8 image (PYR_U8) or the raw image (PYR_PTAM, PYR_OPENCV), `pitch` bytes per row
+static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int pitch, int src)
 {
     const int w = ctx->w, h = ctx->h;
     PyrPtrs pp;
     for (int l = 0; l < LSD_LEVELS; l++) pp.l[l] = s->image[l];
-    if (src == PYR_PTAM) k_image_pyramid<PYR_PTAM><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pp, w, h, ctx->dRemapX, ctx->dRemapY, ctx->rawW, nullptr);
+    if (src == PYR_PTAM) k_image_pyramid<PYR_PTAM><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h, ctx->dRemapX, ctx->dRemapY, ctx->rawW, nullptr);
     else if (src == PYR_OPENCV)
-        k_image_pyramid<PYR_OPENCV><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pp, w, h, nullptr, nullptr, ctx->rawW, nullptr,
-                                                                                   ctx->dCvMap1, ctx->dCvMap2, ctx->rawH);
-    else k_image_pyramid<PYR_U8><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pp, w, h);
+        k_image_pyramid<PYR_OPENCV><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h, nullptr, nullptr, ctx->rawW,
+                                                                                   nullptr, ctx->dCvMap1, ctx->dCvMap2, ctx->rawH);
+    else k_image_pyramid<PYR_U8><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h);
     LAUNCH(ctx);
     GradPtrs gp;
     for (int l = 0; l < LSD_LEVELS; l++) { gp.img[l] = s->image[l]; gp.grad[l] = s->grad[l]; gp.w[l] = w >> l; gp.h[l] = h >> l; }
@@ -151,6 +177,20 @@ static int recordParts(const lsdgpu_ctx* ctx, FrameSlot& s, RecordPart* p)
     p[k++] = { (char**)&s.permaVar, (size_t)s.permaNumPts * 4 };
     return k;
 }
+cudaError_t ensureRecordPool(lsdgpu_ctx* ctx)
+{
+    if (ctx->recordPool) return cudaSuccess;
+    cudaMemPoolProps pp;
+    memset(&pp, 0, sizeof(pp));
+    pp.allocType = cudaMemAllocationTypePinned;
+    pp.location.type = cudaMemLocationTypeDevice; pp.location.id = ctx->device;
+    cudaError_t e = cudaMemPoolCreate(&ctx->recordPool, &pp);
+    if (e != cudaSuccess) { ctx->recordPool = nullptr; return e; }
+    // freed blocks stay mapped for the next allocation instead of going back to the device at each synchronisation (which
+    // made every allocation map fresh memory on the stream); the context's destruction returns them
+    uint64_t keep = UINT64_MAX;
+    return cudaMemPoolSetAttribute(ctx->recordPool, cudaMemPoolAttrReleaseThreshold, &keep);
+}
 static void addCopy(RecordCopy& c, const void* src, void* dst, size_t bytes)
 {
     if (!bytes) return;
@@ -175,17 +215,7 @@ extern "C" int lsdgpu_frame_minimize(lsdgpu_ctx* ctx, int frame_id)
     if (!s) return lsd_fail(ctx, "unknown frame id");
     if (ctx->activeKf == frame_id) return lsd_fail(ctx, "frame is the active keyframe of the depth map");
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
-    if (!ctx->recordPool) {
-        cudaMemPoolProps pp;
-        memset(&pp, 0, sizeof(pp));
-        pp.allocType = cudaMemAllocationTypePinned;
-        pp.location.type = cudaMemLocationTypeDevice; pp.location.id = ctx->device;
-        LSD_CHECK(ctx, cudaMemPoolCreate(&ctx->recordPool, &pp));
-        // freed records stay mapped for the next minimize instead of going back to the device at each synchronisation (which
-        // made every allocation map fresh memory on the stream); the context's destruction returns them
-        uint64_t keep = UINT64_MAX;
-        LSD_CHECK(ctx, cudaMemPoolSetAttribute(ctx->recordPool, cudaMemPoolAttrReleaseThreshold, &keep));
-    }
+    LSD_CHECK(ctx, ensureRecordPool(ctx));
     FrameSlot m = *s;
     RecordPart from[REC_MAX_SEGS], to[REC_MAX_SEGS];
     const int np = recordParts(ctx, *s, from);
@@ -248,7 +278,8 @@ extern "C" int lsdgpu_frame_activate(lsdgpu_ctx* ctx, int frame_id)
     if (r) return r;
     PyrPtrs pp;
     for (int l = 0; l < LSD_LEVELS; l++) pp.l[l] = a.image[l];
-    k_image_pyramid<PYR_F32><<<dim3(ctx->w / 16, ctx->h / 16), 256, 0, ctx->stream>>>((const uint8_t*)m->image[0], pp, ctx->w, ctx->h);
+    k_image_pyramid<PYR_F32><<<dim3(ctx->w / 16, ctx->h / 16), 256, 0, ctx->stream>>>((const uint8_t*)m->image[0], ctx->w * 4, pp, ctx->w,
+                                                                                      ctx->h);
     LAUNCH(ctx);
     GradPtrs gp;
     for (int l = 0; l < LSD_LEVELS; l++) { gp.img[l] = a.image[l]; gp.grad[l] = a.grad[l]; gp.w[l] = ctx->w >> l; gp.h[l] = ctx->h >> l; }
@@ -279,9 +310,9 @@ int ensureIdepthPyramid(lsdgpu_ctx* ctx, FrameSlot* s)
     return 0;
 }
 
-extern "C" int lsdgpu_frame_download(lsdgpu_ctx* ctx, int frame_id, int what, int level, void* out)
-{ LSD_LOCK(ctx);
-    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+// The plane lsdgpu_frame_download and lsdgpu_frame_download_device copy: checks the request and returns its frame and size
+static int downloadPlane(lsdgpu_ctx* ctx, int frame_id, int what, int level, FrameSlot** slot, size_t* bytes)
+{
     FrameSlot* s = findFrame(ctx, frame_id);
     if (!s) return lsd_fail(ctx, "unknown frame id");
     if (level < 0 || level >= LSD_LEVELS) return lsd_fail(ctx, "bad level");
@@ -290,24 +321,70 @@ extern "C" int lsdgpu_frame_download(lsdgpu_ctx* ctx, int frame_id, int what, in
         return -2;
     }
     const size_t n = ((size_t)ctx->w * ctx->h) >> (2 * level);
-    const void* src = nullptr;
-    size_t bytes = 0;
     switch (what) {
-    case LSDGPU_BUF_IMAGE: src = s->image[level]; bytes = n * 4; break;
-    case LSDGPU_BUF_GRADIENTS: src = s->grad[level]; bytes = n * 16; break;
-    case LSDGPU_BUF_MAXGRAD: if (level != 0) return lsd_fail(ctx, "maxGradients exists at level 0 only"); src = s->maxgrad; bytes = n * 4; break;
+    case LSDGPU_BUF_IMAGE: *bytes = n * 4; break;
+    case LSDGPU_BUF_GRADIENTS: *bytes = n * 16; break;
+    case LSDGPU_BUF_MAXGRAD: if (level != 0) return lsd_fail(ctx, "maxGradients exists at level 0 only"); *bytes = n * 4; break;
     case LSDGPU_BUF_IDEPTH:
-    case LSDGPU_BUF_IDEPTH_VAR:
-        if (!s->hasDepth) return lsd_fail(ctx, "frame has no depth");
-        if (level > 0) { int r = ensureIdepthPyramid(ctx, s); if (r) return r; }
-        src = (what == LSDGPU_BUF_IDEPTH) ? s->idepth[level] : s->idepthVar[level]; bytes = n * 4; break;
-    case LSDGPU_BUF_GOODMASK:
-        if (!s->hasGoodMask) { memset(out, 1, ((size_t)ctx->w * ctx->h) / 4); return 0; }   // Frame.h:433: initialised to true
-        src = s->goodMask; bytes = ((size_t)ctx->w * ctx->h) / 4; break;
+    case LSDGPU_BUF_IDEPTH_VAR: if (!s->hasDepth) return lsd_fail(ctx, "frame has no depth"); *bytes = n * 4; break;
+    case LSDGPU_BUF_GOODMASK: *bytes = ((size_t)ctx->w * ctx->h) / 4; break;
     default: return lsd_fail(ctx, "bad buffer selector");
     }
+    *slot = s;
+    return 0;
+}
+// its source, once the request has been accepted: builds the idepth pyramid if needed; nullptr for a good mask that was never
+// written (it reads as all 1s, Frame.h:433: initialised to true)
+static int downloadSource(lsdgpu_ctx* ctx, FrameSlot* s, int what, int level, const void** src)
+{
+    switch (what) {
+    case LSDGPU_BUF_IMAGE: *src = s->image[level]; break;
+    case LSDGPU_BUF_GRADIENTS: *src = s->grad[level]; break;
+    case LSDGPU_BUF_MAXGRAD: *src = s->maxgrad; break;
+    case LSDGPU_BUF_IDEPTH:
+    case LSDGPU_BUF_IDEPTH_VAR:
+        if (level > 0) { int r = ensureIdepthPyramid(ctx, s); if (r) return r; }
+        *src = (what == LSDGPU_BUF_IDEPTH) ? s->idepth[level] : s->idepthVar[level]; break;
+    default: *src = s->hasGoodMask ? s->goodMask : nullptr; break;
+    }
+    return 0;
+}
+
+extern "C" int lsdgpu_frame_download(lsdgpu_ctx* ctx, int frame_id, int what, int level, void* out)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    FrameSlot* s;
+    size_t bytes;
+    const void* src;
+    int r = downloadPlane(ctx, frame_id, what, level, &s, &bytes);
+    if (r || (r = downloadSource(ctx, s, what, level, &src))) return r;
+    if (!src) { memset(out, 1, bytes); return 0; }
     LSD_CHECK(ctx, cudaMemcpyAsync(out, src, bytes, cudaMemcpyDeviceToHost, ctx->stream));
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+extern "C" int lsdgpu_frame_download_device(lsdgpu_ctx* ctx, int frame_id, int what, int level, void* d_out, size_t capacity, void* stream)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    FrameSlot* s;
+    size_t bytes;
+    const void* src;
+    int r = downloadPlane(ctx, frame_id, what, level, &s, &bytes);
+    if (r) return r;
+    if (capacity < bytes) {
+        char msg[160];
+        snprintf(msg, sizeof(msg), "frame_download_device: the plane has %zu bytes, the output holds %zu", bytes, capacity);
+        return lsd_fail(ctx, msg);
+    }
+    if ((r = checkDevicePtr(ctx, "frame_download_device", "the output", d_out,
+                            what == LSDGPU_BUF_GRADIENTS ? 16 : what == LSDGPU_BUF_GOODMASK ? 1 : 4)))
+        return r;
+    LSD_CHECK(ctx, afterCallerStream(ctx, stream));
+    if ((r = downloadSource(ctx, s, what, level, &src))) return r;
+    if (src) LSD_CHECK(ctx, cudaMemcpyAsync(d_out, src, bytes, cudaMemcpyDeviceToDevice, ctx->stream));
+    else LSD_CHECK(ctx, cudaMemsetAsync(d_out, 1, bytes, ctx->stream));
+    LSD_CHECK(ctx, beforeCallerStream(ctx, stream));
     return 0;
 }
 
@@ -577,7 +654,21 @@ extern "C" int lsdgpu_frame_upload_distorted_u8(lsdgpu_ctx* ctx, int frame_id, c
     if (!s) return failMissing(ctx, frame_id, "no free frame slot (release frames or raise max_frames)");
     int r = uploadRaw(ctx, raw);
     if (r) return r;
-    return buildFrameFromDeviceU8(ctx, s, ctx->dRaw, ctx->dCvMap1 ? PYR_OPENCV : ctx->dRemapX ? PYR_PTAM : PYR_U8);
+    return buildFrameFromDeviceU8(ctx, s, ctx->dRaw, ctx->rawW, ctx->dCvMap1 ? PYR_OPENCV : ctx->dRemapX ? PYR_PTAM : PYR_U8);
+}
+
+extern "C" int lsdgpu_frame_upload_distorted_device_u8(lsdgpu_ctx* ctx, int frame_id, const uint8_t* d_raw, size_t pitch, void* stream)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    if (!ctx->undistorterSet) return lsd_fail(ctx, "no undistorter installed (lsdgpu_set_undistorter)");
+    int r = checkDeviceImage(ctx, "frame_upload_distorted_device_u8", d_raw, pitch, ctx->rawW, ctx->rawH);
+    if (r) return r;
+    FrameSlot* s = acquireSlot(ctx, frame_id);
+    if (!s) return failMissing(ctx, frame_id, "no free frame slot (release frames or raise max_frames)");
+    LSD_CHECK(ctx, afterCallerStream(ctx, stream));
+    if ((r = buildFrameFromDeviceU8(ctx, s, d_raw, (int)pitch, ctx->dCvMap1 ? PYR_OPENCV : ctx->dRemapX ? PYR_PTAM : PYR_U8))) return r;
+    LSD_CHECK(ctx, beforeCallerStream(ctx, stream));
+    return 0;
 }
 
 // ------------------------------------------------------------------------------------------------------

@@ -200,6 +200,8 @@ struct lsdgpu_ctx {
     cudaEvent_t cloudKernDone[2], cloudCopyDone[2];
     cudaEvent_t cloudT0 = nullptr, cloudT1 = nullptr;
     bool cloudTimed = false;
+    // the *_device entry points: callerIn orders the context's stream after the caller's stream, callerOut the caller's after it
+    cudaEvent_t callerIn = nullptr, callerOut = nullptr;
 
     // timers
     cudaEvent_t tBegin[8], tEnd[8];
@@ -285,11 +287,59 @@ static inline int failMissing(lsdgpu_ctx* ctx, int id, const char* msg)
     return -2;
 }
 
+// ---- the *_device entry points (include/lsdgpu.h): the caller's stream and the caller's device pointers ------------------------
+// NULL is the legacy default stream (the library's own default stream need not be the legacy one)
+static inline cudaStream_t callerStream(void* stream) { return stream ? (cudaStream_t)stream : cudaStreamLegacy; }
+// the context's next work starts after everything enqueued on the caller's stream so far
+static inline cudaError_t afterCallerStream(lsdgpu_ctx* ctx, void* stream)
+{
+    cudaError_t e = cudaEventRecord(ctx->callerIn, callerStream(stream));
+    return e != cudaSuccess ? e : cudaStreamWaitEvent(ctx->stream, ctx->callerIn, 0);
+}
+// the caller's later work on its stream starts after everything enqueued on the context's stream so far
+static inline cudaError_t beforeCallerStream(lsdgpu_ctx* ctx, void* stream)
+{
+    cudaError_t e = cudaEventRecord(ctx->callerOut, ctx->stream);
+    return e != cudaSuccess ? e : cudaStreamWaitEvent(callerStream(stream), ctx->callerOut, 0);
+}
+// 0 if p is device or managed memory of the context's device, aligned to `align` bytes; otherwise an error naming `what`
+static inline int checkDevicePtr(lsdgpu_ctx* ctx, const char* fn, const char* what, const void* p, size_t align)
+{
+    char msg[256];
+    cudaPointerAttributes pa;
+    const cudaError_t e = p ? cudaPointerGetAttributes(&pa, p) : cudaErrorInvalidValue;
+    if (e != cudaSuccess) cudaGetLastError();
+    if (!p || e != cudaSuccess || (pa.type != cudaMemoryTypeDevice && pa.type != cudaMemoryTypeManaged)) {
+        snprintf(msg, sizeof(msg), "%s: %s is not device memory", fn, what);
+        return lsd_fail(ctx, msg);
+    }
+    if (pa.device != ctx->device) {
+        snprintf(msg, sizeof(msg), "%s: %s is memory of device %d, the context's device is %d", fn, what, pa.device, ctx->device);
+        return lsd_fail(ctx, msg);
+    }
+    if ((uintptr_t)p % align) {
+        snprintf(msg, sizeof(msg), "%s: %s is not %zu-byte aligned", fn, what, align);
+        return lsd_fail(ctx, msg);
+    }
+    return 0;
+}
+// a caller's device image of width x height bytes with row pitch `pitch` (the kernels index it with int arithmetic)
+static inline int checkDeviceImage(lsdgpu_ctx* ctx, const char* fn, const uint8_t* p, size_t pitch, int width, int height)
+{
+    char msg[256];
+    if (pitch < (size_t)width || pitch > (size_t)INT32_MAX / (size_t)height) {
+        snprintf(msg, sizeof(msg), "%s: row pitch %zu bytes for an image %d bytes wide (%d rows)", fn, pitch, width, height);
+        return lsd_fail(ctx, msg);
+    }
+    return checkDevicePtr(ctx, fn, "the image", p, 1);
+}
+
 static inline int divUp(int a, int b) { return (a + b - 1) / b; }
 static inline size_t alignUp(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 // ---- host helpers shared by the units of the library (each defined once, in the unit named) ---------------------------
 int ensureIdepthPyramid(lsdgpu_ctx* ctx, FrameSlot* s);     // frames.cu: levels 1..4 of a keyframe's idepth / idepthVar
+cudaError_t ensureRecordPool(lsdgpu_ctx* ctx);              // frames.cu: the context's stream-ordered memory pool (recordPool)
 cudaError_t trackPersistentSetup(lsdgpu_ctx* ctx);          // tracking.cu: launch shape of the persistent tracker
 void cloudRelease(lsdgpu_ctx* ctx);                         // output.cu: frees the point-cloud reservation
 

@@ -10,9 +10,13 @@ camToWorld.  The context reserves K keyframes per launch, so an export is one ke
                = 12 B per interior pixel (idepth, idepthVar, image read once) + 16 B per kept point, over that time, against the
                H100 SXM data sheet's 3.35 TB/s
   end to end   wall clock of the whole call (descriptor upload, kernel, device-to-host copy of the points into a reused host array)
+  device out   lsdgpu_map_export_pointcloud_device into a reused CUDA tensor (no reservation, one launch, no copy of the points):
+               CUDA events around the call on the caller's stream, and the wall clock of the call (it waits for the point count);
+               run alternately with the host export, in the same repetitions
   CPU          lsd_slam_viewer's KeyFrameDisplay::refreshPC + flushPC compiled unmodified (oracle/_ref/libviewer_ref.so), one
                thread as in the viewer, over the same keyframes' keyframeMsg.pointcloud; per keyframe, message packing excluded
-Exits with 3 unless the GPU's points (PLY and vertex layouts) and counts are identical to the viewer's (NaN compared as NaN).
+Exits with 3 unless the GPU's points (PLY and vertex layouts, both arms) and counts are identical to the viewer's (NaN compared
+as NaN).
 Card name, power limit and SM clock are sampled in the same run (bench.py's sampler).  Prints one JSON line per size and K.
 """
 from __future__ import annotations
@@ -96,9 +100,12 @@ def run(w, h, K, reps, level):
     wl, hl = w >> level, h >> level
     interior = (wl - 2) * (hl - 2)
     out = np.empty(K * interior, abi.CLOUD_PLY_DTYPE)
+    out_dev = torch.empty((K * interior, 4), dtype=torch.float32, device="cuda")
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")      # larger than the H100's 50 MB L2
     ctx.export_pointcloud(ids, c2w, level=level, out=out)                  # warm-up: module load, page-in of out
-    dev_ms, e2e_ms = [], []
+    ctx.export_pointcloud(ids, c2w, level=level, out=out_dev)              # warm-up: the memory pool's first block
+    dev_ms, e2e_ms, dout_ev_ms, dout_wall_ms = [], [], [], []
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     for _ in range(reps):
         flush.zero_()
         torch.cuda.synchronize()
@@ -106,8 +113,20 @@ def run(w, h, K, reps, level):
         pts, counts = ctx.export_pointcloud(ids, c2w, level=level, out=out)
         e2e_ms.append((time.perf_counter() - t0) * 1e3)
         dev_ms.append(ctx.cloud_kernel_ms())
+        flush.zero_()
+        torch.cuda.synchronize()
+        e0.record()
+        t0 = time.perf_counter()
+        dpts, dcounts = ctx.export_pointcloud(ids, c2w, level=level, out=out_dev)
+        dout_wall_ms.append((time.perf_counter() - t0) * 1e3)
+        e1.record()
+        e1.synchronize()
+        dout_ev_ms.append(e0.elapsed_time(e1))
     kept = int(counts[:, 1].sum())
+    dpts = dpts.cpu().numpy()
     vert, vcounts = ctx.export_pointcloud(ids, c2w, level=level, layout=abi.CLOUD_VERTEX)
+    dvert, dvcounts = ctx.export_pointcloud(ids, c2w, level=level, layout=abi.CLOUD_VERTEX, out=out_dev)
+    dvert = dvert.cpu().numpy()
 
     # the viewer's own code, one keyframe after the other (its message packing not timed)
     cam = level_cam(ctx, level)
@@ -122,6 +141,8 @@ def run(w, h, K, reps, level):
         ref_counts.append((total, shown))
     ok = (same(pts, np.concatenate(ref_ply)) and same(vert, np.concatenate(ref_vert))
           and np.array_equal(counts, np.array(ref_counts, np.int32)) and np.array_equal(vcounts, counts))
+    ok_dev = (same(dpts, np.concatenate(ref_ply)) and same(dvert, np.concatenate(ref_vert))
+              and np.array_equal(dcounts, counts) and np.array_equal(dvcounts, counts))
     ctx.close()
     algo_bytes = 12.0 * interior * K + 16.0 * kept
     dev = float(np.median(dev_ms))
@@ -129,7 +150,10 @@ def run(w, h, K, reps, level):
             "device_ms": dev, "device_ms_all": [round(x, 4) for x in dev_ms], "algorithmic_bytes": algo_bytes,
             "device_GBps": algo_bytes / dev / 1e6, "hbm_fraction": algo_bytes / dev / 1e-3 / HBM_BYTES_PER_S,
             "e2e_ms": float(np.median(e2e_ms)), "e2e_ms_all": [round(x, 3) for x in e2e_ms],
-            "cpu_viewer_ms": cpu_s * 1e3, "speedup_e2e_vs_viewer": cpu_s * 1e3 / float(np.median(e2e_ms)), "parity": bool(ok)}
+            "device_out_event_ms": float(np.median(dout_ev_ms)), "device_out_event_ms_all": [round(x, 4) for x in dout_ev_ms],
+            "device_out_wall_ms": float(np.median(dout_wall_ms)), "device_out_wall_ms_all": [round(x, 3) for x in dout_wall_ms],
+            "cpu_viewer_ms": cpu_s * 1e3, "speedup_e2e_vs_viewer": cpu_s * 1e3 / float(np.median(e2e_ms)),
+            "parity": bool(ok), "parity_device_out": bool(ok_dev)}
 
 
 def main():
@@ -163,7 +187,7 @@ def main():
         with open(args.json, "a") as f:
             for r in results:
                 f.write(json.dumps(dict(r, clocks=clocks)) + "\n")
-    if not all(r["parity"] for r in results):
+    if not all(r["parity"] and r["parity_device_out"] for r in results):
         print("PARITY FAILED: the GPU export differs from the viewer's code", file=sys.stderr)
         raise SystemExit(3)
 
