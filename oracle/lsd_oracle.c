@@ -76,7 +76,7 @@ void lsdo_default_globals(lsdo_globals* g)
 {   /* util/settings.cpp:77-88 */
     g->minUseGrad = 5; g->cameraPixelNoise2 = 4*4; g->depthSmoothingFactor = 1;
     g->allowNegativeIdepths = 1; g->useSubpixelStereo = 1; g->useAffineLightningEstimation = 1;
-    g->multiThreading = 1; g->useSSE = 0; g->exactAffineSums = 0; g->exactTrackingSums = 0;
+    g->multiThreading = 1; g->useSSE = 0; g->exactAffineSums = 0; g->exactTrackingSums = 0; g->exactSim3Sums = 0;
 }
 void lsdo_set_globals(const lsdo_globals* g) { G = *g; }
 void lsdo_get_globals(lsdo_globals* g) { *g = G; }

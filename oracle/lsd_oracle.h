@@ -68,6 +68,9 @@ typedef struct {
                                        * sums, residual sums, LGS6 A / b / error) in double from the same fp32 terms -- the result the
                                        * reference's sequential fp32 accumulation approximates.  Used to measure the reference's OWN
                                        * summation noise in the tracked pose (tests/test_gpu_fullsize.py, DESIGN.md section 5) */
+    int   exactSim3Sums;              /* DIAGNOSTIC, default 0 = the reference: 1 accumulates every sum of the scalar Sim3 tracker
+                                       * (the five affine-lighting sums, the depth and photometric residual sums, LGS4 / LGS6 A / b /
+                                       * error) in double from the same fp32 terms -- what the device's tree sums approach */
 } lsdo_globals;
 
 /* DenseDepthTrackerSettings, util/settings.h:355-402 */

@@ -40,7 +40,7 @@ class Globals(C.Structure):
     _fields_ = [("minUseGrad", C.c_float), ("cameraPixelNoise2", C.c_float), ("depthSmoothingFactor", C.c_float),
                 ("allowNegativeIdepths", C.c_int), ("useSubpixelStereo", C.c_int),
                 ("useAffineLightningEstimation", C.c_int), ("multiThreading", C.c_int), ("useSSE", C.c_int),
-                ("exactAffineSums", C.c_int), ("exactTrackingSums", C.c_int)]
+                ("exactAffineSums", C.c_int), ("exactTrackingSums", C.c_int), ("exactSim3Sums", C.c_int)]
 
 
 class TrackSettings(C.Structure):

@@ -8,8 +8,8 @@ from lsd_slam_b200.stream import GpuStream, GpuStreamGroup, sim3_mul_qts
 from tests.pin_cases import (AB, MAPPED_FRAMES, MAPPED_KF_EVERY, PERMA_FRAME, POSE_SENSITIVE_DEPTH_RESIDUAL, SIM3_DT, SIM3_SCALE,
                              adversarial_edit, set_depth)
 from tests.util import (IDENT, Pair, check_perma_overlap, check_perma_track, check_se3_eval, check_se3_track, check_sim3_eval,
-                        check_sim3_track, kf_depth_equal, new_depth, observe, oracle_sim3_track, perma_noise, pose_err, se3_inverse,
-                        sim3_err, sim3_init, sim3_inverse, sim3_mul, tracked_pair)
+                        check_sim3_track, kf_depth_equal, new_depth, observe, oracle_sim3_exact, oracle_sim3_track, perma_noise,
+                        pose_err, se3_inverse, sim3_err, sim3_init, sim3_inverse, sim3_mul, tracked_pair)
 
 
 # ---- depth map, bit for bit -------------------------------------------------------------------------------------------------
@@ -423,13 +423,14 @@ def pyramid_mismatches(ctx, kf, of):
 
 class MappedRun:
     """A GpuStream of the seed-1234 sequence of `motion` (tests/motions.py; the default twist by default) with its finished
-    keyframes resident and an oracle mirror of each.  After every keyframe change it compares the pyramids of every resident
-    keyframe with the oracle (`checks`)."""
+    keyframes resident and an oracle mirror of each.  `seq`, if given, is run instead; `motion` then only names the run, as the
+    key of POSE_SENSITIVE_DEPTH_RESIDUAL.  After every keyframe change it compares the pyramids of every resident keyframe with
+    the oracle (`checks`)."""
 
-    def __init__(self, oracle, w, h, motion="default"):
+    def __init__(self, oracle, w, h, motion="default", seq=None):
         from tests import motions
         self.motion = motion
-        self.seq = seq = motions.sequence(motion, w, h)
+        self.seq = seq = motions.sequence(motion, w, h) if seq is None else seq
         self.ctx = ctx = abi.Context(w, h, seq.K, max_frames=12)
         self.gs = gs = GpuStream(ctx, kf_every=MAPPED_KF_EVERY, keep_keyframes=True)
         self.images = {}
@@ -522,9 +523,17 @@ def mapped_sim3_eval_settings(run, oracle):
             check_sim3_eval(trk.eval(ref, fr, lvl, r2f, a, b), oracle.sim3_eval(run.of[ref], run.of[fr], lvl, r2f, a, b, settings=st))
 
 
-def mapped_sim3_track(run, oracle):
+def _sum_noise(oracle, ref, fr, init, lo, hi, *results):
+    """-> (the all-sums-exact twin of trackFrameSim3, each result's pose distance to it): how far the fp32 summation of each
+    oracle result alone moved its pose"""
+    tw = oracle_sim3_exact(oracle, ref, fr, init, lo, hi)
+    return tw, [max(sim3_err(r.frameToRef_qts, tw.frameToRef_qts)) for r in results]
+
+
+def mapped_sim3_track(run, oracle, sum_noise=False):
     """trackFrameSim3 per ordered pair over levels 4..1 and 3..2 (lastDepthResidual of pin_cases.POSE_SENSITIVE_DEPTH_RESIDUAL
-    against the exact-sum twin to the reference tolerance)"""
+    against the exact-sum twin to the reference tolerance).  sum_noise: the pose may also differ from each oracle result by
+    that result's own distance to the all-sums-exact twin, which holds the device to POSE_TOL"""
     trk = abi.Sim3Tracker(run.ctx)
     n_converged = 0
     for ref, fr in run.pairs():
@@ -532,16 +541,20 @@ def mapped_sim3_track(run, oracle):
         for lo, hi in ((4, 1), (3, 2)):
             est = trk.trackFrameSim3(ref, fr, init, lo, hi)
             want, exact = oracle_sim3_track(oracle, run.of[ref], run.of[fr], init, lo, hi)
-            check_sim3_track(trk.last, want)
+            noise = (0.0, 0.0)
+            if sum_noise:
+                tw, noise = _sum_noise(oracle, run.of[ref], run.of[fr], init, lo, hi, want, exact)
+                check_sim3_track(trk.last, tw)
+            check_sim3_track(trk.last, want, pose_noise=noise[0])
             sensitive = (run.motion, ref, fr, lo, hi) in POSE_SENSITIVE_DEPTH_RESIDUAL
-            check_sim3_track(trk.last, exact, res_tol=5e-4, depth_res_tol=2e-2 if sensitive else None)
+            check_sim3_track(trk.last, exact, res_tol=5e-4, depth_res_tol=2e-2 if sensitive else None, pose_noise=noise[1])
             assert np.array_equal(est, np.array(trk.last.frameToRef_qts))
             n_converged += not want.diverged
     assert n_converged >= len(run.pairs())
 
 
-def mapped_sim3_batch(run, oracle):
-    """every ordered pair in one launch == one by one (bit-identical) == the oracle"""
+def mapped_sim3_batch(run, oracle, sum_noise=False):
+    """every ordered pair in one launch == one by one (bit-identical) == the oracle (sum_noise: as mapped_sim3_track)"""
     trk = abi.Sim3Tracker(run.ctx)
     pairs = run.pairs()
     inits = np.array([run.frame_to_ref(oracle, ref, fr) for ref, fr in pairs])
@@ -549,7 +562,12 @@ def mapped_sim3_batch(run, oracle):
     for (ref, fr), init, r in zip(pairs, inits, res):
         trk.trackFrameSim3(ref, fr, init, 4, 1)
         assert bytes(trk.last) == bytes(r)
-        check_sim3_track(r, oracle.sim3_track(run.of[ref], run.of[fr], init, 4, 1))
+        want = oracle.sim3_track(run.of[ref], run.of[fr], init, 4, 1)
+        noise = (0.0,)
+        if sum_noise:
+            tw, noise = _sum_noise(oracle, run.of[ref], run.of[fr], init, 4, 1, want)
+            check_sim3_track(r, tw)
+        check_sim3_track(r, want, pose_noise=noise[0])
 
 
 def mapped_perma(run, oracle, noise_aware=False):

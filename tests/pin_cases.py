@@ -6,7 +6,8 @@ tests/test_ref_pin.py runs the cases at the reference's default run-time setting
 tests/test_ref_pin_globals.py under the settings of SETS, tests/test_ref_pin_motions.py under the camera motions of
 tests/motions.py (with two more cases only those reach), tests/test_ref_pin_sim3.py runs the Sim3 tracker and the permaRef
 path on keyframes the mapper finished, under every motion, tests/test_ref_pin_photometry.py runs cases under the exposure
-schedules of tests/photometry.py; tests/golden/make_golden*.py record each of them."""
+schedules of tests/photometry.py, tests/test_ref_pin_cameras.py the cases that read K through the cameras of tests/cameras.py;
+tests/golden/make_golden*.py record each of them."""
 import contextlib
 import ctypes as C
 import hashlib
@@ -15,7 +16,7 @@ import os
 import numpy as np
 
 from oracle import pyoracle as po
-from tests import motions, photometry
+from tests import cameras, motions, photometry
 from tests.util import IDENT, pose_err
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -1006,4 +1007,41 @@ def record_photometry():
     out = {}
     for s, c in PHOTOMETRY_PAIRS:
         out.update(run_under_exposure(s, c, None).rec)
+    return out
+
+
+# ---- cameras other than synth.pinhole_K (tests/cameras.py) -------------------------------------------------------------------
+GOLD_CAMERAS = os.path.join(GOLDEN, "ref_pin_cameras_320x240.npz")
+
+# case -> (function, C-restatement flavour, reference-compiled flavour), as CASES: every case that reads K
+CAMERA_CASES = {c: CASES[c] for c in ("frame_builders", "point_cloud") + GEOMETRY}
+CAMERA_CASES.update(SIM3_CASES)
+CAMERA_STREAMS = cameras.SMALL + (cameras.VERTICAL,)
+CAMERA_ONLY = {c: cameras.SMALL for c in CAMERA_CASES if c not in DEPTH}          # the vertical stream: the depth-map cases
+CAMERA_ONLY.update({c: ("offset", "general") for c in SIM3_CASES})
+# (camera, reference keyframe, frame keyframe, startLevel, finalLevel) of a trackFrameSim3 call whose pose the reference's
+# sequential fp32 sums of the normal equations move by a large part of POSE_TOL (tests/test_ref_pin_cameras.py)
+SIM3_SUM_SENSITIVE = ("offset", 10, 5, 4, 1)
+CAMERA_PAIRS = [(cam, c) for cam in CAMERA_STREAMS for c in CAMERA_CASES if cam in CAMERA_ONLY.get(c, (cam,))]
+
+
+def run_under_camera(camera, case, gold, seq=None):
+    """runs one case through one camera on the C restatement (gold = the record) or on the reference-compiled library
+    (gold = None); returns the case's Pin.  seq: another sequence that the case reads K from instead, with the camera's images"""
+    fn, fl, ref_fl = CAMERA_CASES[case]
+    fl = ref_fl if gold is None else fl
+    cam_seq, frames = cameras.stream(camera)
+    p = Pin(f"{camera}/{case}", gold)
+    try:
+        fn(p, fl, cam_seq if seq is None else seq, frames)
+    finally:
+        po.set_globals(fl)
+    return p
+
+
+def record_cameras():
+    """every (camera, case) on the reference-compiled library (needs oracle/_ref): the arrays of ref_pin_cameras_320x240.npz"""
+    out = {}
+    for cam, c in CAMERA_PAIRS:
+        out.update(run_under_camera(cam, c, None).rec)
     return out

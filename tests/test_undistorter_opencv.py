@@ -215,40 +215,86 @@ def _distort_frames(seq, frames, calib, in_size, K_new, out_size):
 
 
 @pytest.mark.gpu
-def test_gpu_track_and_map_on_distorted_frames(seq_small, frames_small):
+def test_gpu_track_and_map_on_distorted_frames(oracle, seq_small, frames_small):
     """10 frames, GT-depth init: upload_distorted + se3_track + depth_update_keyframe gives the poses and depth maps of the same
-    calls fed with host-undistorted frames"""
+    calls fed with host-undistorted frames; and the host leg agrees with the oracle fed the same undistorted images and getK():
+    every pose tracked from the same start to 1e-4 plus the reference's own summation noise on that step, and every map bit for
+    bit when the oracle maps with the device's pose, residual and good mask"""
+    from tests.pin_cases import set_depth
+    from tests.util import hyp_equal_report, pose_err
     seq = seq_small
     K = seq.K.astype(np.float64)
     calib = [K[0, 0] * 1.02, K[1, 1] * 1.02, K[0, 2] + 1.5, K[1, 2] - 1.0, -0.18, 0.05, 0.0007, -0.0004]
     in_size = out_size = (seq.w, seq.h)
     u = abi.UndistorterOpenCV(calib, in_size, "crop", out_size)
+    Ku = u.getK()
+    assert Ku[0, 0] != Ku[1, 1]
     imgs = [frames_small[k][0] for k in range(10)]
     raws, (du, dv) = _distort_frames(seq, imgs, calib, in_size, u.K_new, out_size)
     depth0 = frames_small[0][1][dv, du]
     legs = {}
+    L = oracle.lib()
     for leg in ("fused", "host"):
-        ctx = abi.Context(seq.w, seq.h, u.getK(), max_frames=12)
+        ctx = abi.Context(seq.w, seq.h, Ku, max_frames=12)
         u.install(ctx)
         trk, dm = abi.SE3Tracker(ctx, mode=1), abi.DepthMap(ctx)
         poses, maps = [], []
         last = np.array([0, 0, 0, 1, 0, 0, 0], np.float64)
+        keep = []
         for k, raw in enumerate(raws):
+            img = cvo.remap(raw, u.map1, u.map2)
             if leg == "fused":
                 ctx.upload_distorted(k, raw)
             else:
-                ctx.upload(k, cvo.remap(raw, u.map1, u.map2))
+                ctx.upload(k, img)
             if k == 0:
                 ctx.set_depth_gt(0, depth0)
                 dm.initializeFromGTDepth(0)
+                if leg == "host":
+                    okf = oracle.Frame(0, img, Ku)
+                    okf.setDepthFromGroundTruth(depth0)
+                    odm = oracle.DepthMap(seq.w, seq.h, Ku)
+                    odm.initializeFromGTDepth(okf)
+                    img0 = img
                 continue
             if k == 1 or ctx.depth_updated_flag(0):
                 trk.importFrame(0)
             pose = trk.trackFrame(0, k, last)
             poses.append((pose.tobytes(), trk.trackingWasGood))
+            counters = ctx.get_counters(0)
+            if leg == "host":
+                # the same tracking on the oracle, and on its twin with every sum exact (the reference's own noise on this step)
+                L.lsdo_frame_set_depthHasBeenUpdatedFlag(okf.ptr, 0)
+                oracle.set_globals(exactTrackingSums=1)
+                try:
+                    xkf = oracle.Frame(0, img0, Ku)
+                    if k == 1:
+                        xkf.setDepthFromGroundTruth(depth0)
+                    else:
+                        set_depth(xkf, odm.current())
+                    rx = oracle.se3_track(xkf, oracle.Frame(k, img, Ku), last)
+                finally:
+                    oracle.set_globals()
+                of = oracle.Frame(k, img, Ku)
+                keep.append(of)
+                r = oracle.se3_track(okf, of, last)
+                assert bool(r.trackingWasGood) == trk.trackingWasGood and not r.diverged, k
+                dt, ang = pose_err(pose, r.frameToRef_qt)
+                nt, na = pose_err(r.frameToRef_qt, rx.frameToRef_qt)
+                assert dt <= 1e-4 + nt and ang <= 1e-6 + na, (k, dt, nt, ang, na)
+                qts, _, itr = ctx.get_pose(k)
+                of.set_thisToParent(np.array(qts, np.float64), okf)
+                L.lsdo_frame_set_initialTrackedResidual(of.ptr, float(itr))
+                of.refPixelWasGood(create=True)[:] = ctx.download(k, abi.BUF_GOODMASK)
+                L.lsdo_frame_set_counters(okf.ptr, int(counters[0]), int(counters[1]))
             dm.updateKeyframe([k])
             ctx.clear_good_mask(k)
             maps.append(dm.current().tobytes())
+            if leg == "host":
+                odm.updateKeyframe([of])
+                L.lsdo_frame_clear_refPixelWasGood(of.ptr)
+                rep = hyp_equal_report(dm.current(), odm.current())
+                assert rep["n_valid"] > 3000 and all(v == 0 for key, v in rep.items() if key.endswith(("mismatch", "bitdiff"))), (k, rep)
             last = pose
         legs[leg] = (poses, maps)
         ctx.close()

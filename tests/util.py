@@ -274,6 +274,19 @@ def oracle_sim3_track(oracle, ref, fr, init, lo=4, hi=1, g=None):
     return want, exact
 
 
+def oracle_sim3_exact(oracle, ref, fr, init, lo=4, hi=1, g=None):
+    """the same trackFrameSim3 with EVERY sum of the Sim3 tracker accumulated in double from the same fp32 terms (the affine
+    sums, the residual sums, LGS4 / LGS6 A and b: lsdo_globals.exactSim3Sums), under the settings g.  oracle_sim3_track's twin
+    makes only the affine sums exact; on some calls the sequential fp32 sums of the normal equations move the reference's pose
+    much further (DESIGN.md section 5, Cameras), and the device's tree sums follow the exact values"""
+    g = g or {}
+    oracle.set_globals(exactSim3Sums=1, **g)
+    try:
+        return oracle.sim3_track(ref, fr, init, lo, hi)
+    finally:
+        oracle.set_globals(**g)
+
+
 # ---- permaRef -----------------------------------------------------------------------------------------------------------------
 def check_perma_track(g, o, noise=(0.0, 0.0)):
     """one trackFrameOnPermaref result against the oracle's: the outcome; unless diverged the pose (to POSE_TOL and PERMA_ANG_TOL
