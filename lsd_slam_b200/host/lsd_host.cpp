@@ -13,6 +13,14 @@
 
 namespace lsd_slam {
 
+// util/settings.cpp:80-88
+float minUseGrad = 5;
+float cameraPixelNoise2 = 4 * 4;
+float depthSmoothingFactor = 1;
+bool allowNegativeIdepths = true;
+bool useSubpixelStereo = true;
+bool useAffineLightningEstimation = true;
+
 static void qmul(const double a[4], const double b[4], double o[4])
 {
     double w = a[3] * b[3] - a[0] * b[0] - a[1] * b[1] - a[2] * b[2];
@@ -93,11 +101,25 @@ DeviceContext::DeviceContext(int device, int w, int h, const Matrix3f& K, int ma
         ctx_ = nullptr;
         throw LsdGpuError(msg);
     }
+    followGlobals();                                      // a context starts with the values in force, not the defaults
 }
 DeviceContext::~DeviceContext() { if (ctx_) lsdgpu_destroy(ctx_); }
 void DeviceContext::check(int rc, const char* where) const
 {
     if (rc != 0) throw LsdGpuError(std::string(where) + ": " + lsdgpu_last_error(ctx_));
+}
+void DeviceContext::followGlobals()
+{
+    lsdgpu_globals want, have;
+    want.minUseGrad = minUseGrad;
+    want.cameraPixelNoise2 = cameraPixelNoise2;
+    want.depthSmoothingFactor = depthSmoothingFactor;
+    want.allowNegativeIdepths = allowNegativeIdepths;
+    want.useSubpixelStereo = useSubpixelStereo;
+    want.useAffineLightningEstimation = useAffineLightningEstimation;
+    check(lsdgpu_get_globals(ctx_, &have), "DeviceContext::followGlobals");
+    if (std::memcmp(&want, &have, sizeof(want)) != 0)     // six 4-byte fields, no padding
+        check(lsdgpu_set_globals(ctx_, &want), "DeviceContext::followGlobals");
 }
 
 FrameMemory::FrameMemory(DeviceContext& dev, int maxActive) : dev_(dev), maxActive_(maxActive) {}
@@ -123,6 +145,7 @@ void FrameMemory::makeRoom()
 }
 void FrameMemory::activateFrame(Frame* frame)
 {
+    dev_.followGlobals();
     std::lock_guard<std::recursive_mutex> l(mu_);
     if (frame->isActive) {
         activeFrames.remove(frame);
@@ -135,6 +158,7 @@ void FrameMemory::activateFrame(Frame* frame)
 }
 void FrameMemory::deactivateFrame(Frame* frame)
 {
+    dev_.followGlobals();
     std::lock_guard<std::recursive_mutex> l(mu_);
     if (!frame->isActive) return;
     activeFrames.remove(frame);
@@ -143,6 +167,7 @@ void FrameMemory::deactivateFrame(Frame* frame)
 }
 void FrameMemory::pruneActiveFrames()
 {
+    dev_.followGlobals();
     std::lock_guard<std::recursive_mutex> l(mu_);
     while ((int)activeFrames.size() > maxActive_) minimizeLeastRecent();
 }
@@ -172,6 +197,7 @@ ActiveFrames::~ActiveFrames()
 Frame::Frame(DeviceContext& dev, int id, int width, int height, const Matrix3f&, double timestamp, const unsigned char* image, bool distorted)
     : dev_(dev), id_(id), w_(width), h_(height), timestamp_(timestamp)
 {
+    dev_.followGlobals();
     pose = new FramePoseStruct();
     pose->frameID = id;
     FrameMemory& m = dev_.frameMemory();
@@ -199,42 +225,60 @@ bool Frame::minimizeInMemory()
 void Frame::getActiveLock() { dev_.frameMemory().activateFrame(this); }
 void Frame::setDepthFromGroundTruth(const float* depth, float cov_scale)
 {
+    dev_.followGlobals();
     getActiveLock();                                                    // Frame.cpp:247
     dev_.check(lsdgpu_frame_set_depth_gt(dev_.raw(), id_, depth, cov_scale), "Frame::setDepthFromGroundTruth");
 }
 void Frame::clear_refPixelWasGood()
 {
     if (!isActive) return;                                              // minimizeInMemory cleared it, Frame.cpp:388
+    dev_.followGlobals();
     dev_.check(lsdgpu_frame_clear_good_mask(dev_.raw(), id_), "Frame::clear_refPixelWasGood");
 }
 float Frame::meanIdepth()
 {
+    dev_.followGlobals();
     float m = 1; int n = 0, f = 0;
     dev_.check(lsdgpu_frame_get_depth_stats(dev_.raw(), id_, &m, &n, &f), "Frame::meanIdepth");
     return m;
 }
 int Frame::numPoints()
 {
+    dev_.followGlobals();
     float m = 1; int n = 0, f = 0;
     dev_.check(lsdgpu_frame_get_depth_stats(dev_.raw(), id_, &m, &n, &f), "Frame::numPoints");
     return n;
 }
 bool Frame::depthHasBeenUpdatedFlag() const
 {
+    dev_.followGlobals();
     int f = 0;
     dev_.check(lsdgpu_frame_get_depth_stats(dev_.raw(), id_, nullptr, nullptr, &f), "Frame::depthHasBeenUpdatedFlag");
     return f != 0;
 }
 void Frame::downloadIdepth(int level, std::vector<float>& idepth, std::vector<float>& idepthVar)
 {
+    dev_.followGlobals();
     if (level > 0) getActiveLock();                                     // levels 1..4 are rebuilt on activation (Frame::require)
     size_t n = (size_t)width(level) * height(level);
     idepth.resize(n); idepthVar.resize(n);
     dev_.check(lsdgpu_frame_download(dev_.raw(), id_, LSDGPU_BUF_IDEPTH, level, idepth.data()), "Frame::idepth");
     dev_.check(lsdgpu_frame_download(dev_.raw(), id_, LSDGPU_BUF_IDEPTH_VAR, level, idepthVar.data()), "Frame::idepthVar");
 }
+void Frame::setPermaRef(TrackingReference* reference)
+{   // Frame.cpp:149-174
+    if (reference->frameID != id_)                                      // assert(reference->frameID == id()), :151
+        throw LsdGpuError("Frame::setPermaRef: the TrackingReference holds frame " + std::to_string(reference->frameID) + ", not frame " +
+                          std::to_string(id_));
+    dev_.followGlobals();
+    ActiveFrames held(dev_.frameMemory(), { this });                    // the TrackingReference holds the keyframe's active lock
+    int n = 0;
+    dev_.check(lsdgpu_frame_set_perma_ref(dev_.raw(), id_, &n), "Frame::setPermaRef");
+    permaRefNumPts = n;
+}
 void Frame::downloadRefPixelWasGood(std::vector<unsigned char>& mask)
 {
+    dev_.followGlobals();
     getActiveLock();
     mask.resize((size_t)width(1) * height(1));
     dev_.check(lsdgpu_frame_download(dev_.raw(), id_, LSDGPU_BUF_GOODMASK, 1, mask.data()), "Frame::refPixelWasGood");
@@ -242,6 +286,7 @@ void Frame::downloadRefPixelWasGood(std::vector<unsigned char>& mask)
 
 void TrackingReference::importFrame(Frame* sourceKF)
 {
+    sourceKF->dev().followGlobals();
     sourceKF->getActiveLock();                                          // TrackingReference.cpp:74
     keyframe = sourceKF;
     frameID = sourceKF->id();
@@ -253,11 +298,17 @@ SE3Tracker::SE3Tracker(DeviceContext& dev, int w, int h, const Matrix3f&) : dev_
     if (w != dev.width() || h != dev.height()) throw LsdGpuError("SE3Tracker: size differs from the device context");
 }
 
+static void se3ToQt(const SE3& a, double o[7])
+{
+    for (int i = 0; i < 4; i++) o[i] = a.q[i];
+    for (int i = 0; i < 3; i++) o[4 + i] = a.t[i];
+}
+
 SE3 SE3Tracker::trackFrame(TrackingReference* reference, Frame* frame, const SE3& frameToReference_initialEstimate)
 {
+    dev_.followGlobals();
     double init[7];
-    for (int i = 0; i < 4; i++) init[i] = frameToReference_initialEstimate.q[i];
-    for (int i = 0; i < 3; i++) init[4 + i] = frameToReference_initialEstimate.t[i];
+    se3ToQt(frameToReference_initialEstimate, init);
     ActiveFrames held(dev_.frameMemory(), { reference->keyframe, frame });   // SE3Tracker.cpp:286; the keyframe's levels live in its slot
     lsdgpu_track_result r;
     dev_.check(lsdgpu_se3_track(dev_.raw(), reference->keyframe->id(), frame->id(), init, &settings, mode, &r), "SE3Tracker::trackFrame");
@@ -273,6 +324,41 @@ SE3 SE3Tracker::trackFrame(TrackingReference* reference, Frame* frame, const SE3
     frame->initialTrackedResidual = r.initialTrackedResidual;         // :482
     frame->pose->thisToParent_raw = sim3FromSE3(out, 1);              // :483
     frame->pose->trackingParent = reference->keyframe->pose;          // :484
+    return out;
+}
+
+float SE3Tracker::checkPermaRefOverlap(Frame* reference, SE3 referenceToFrame)
+{   // reads only the permaRef, which a minimized keyframe keeps in its record
+    dev_.followGlobals();
+    const int kfId = reference->id();
+    double qt[7];
+    se3ToQt(referenceToFrame, qt);
+    float usage = 0;
+    if (int rc = lsdgpu_perma_overlap_batch(dev_.raw(), 1, &kfId, qt, &usage))
+        dev_.check(rc, ("SE3Tracker::checkPermaRefOverlap (keyframe " + std::to_string(kfId) + ")").c_str());
+    pointUsage = usage;                                               // :155
+    return pointUsage;
+}
+
+SE3 SE3Tracker::trackFrameOnPermaref(Frame* reference, Frame* frame, SE3 referenceToFrame)
+{
+    dev_.followGlobals();
+    ActiveFrames held(dev_.frameMemory(), { frame });                 // :170; the reference's permaRef needs no slot
+    const int kfId = reference->id();
+    double init[7];
+    se3ToQt(referenceToFrame, init);
+    lsdgpu_track_result r;
+    if (int rc = lsdgpu_perma_track_batch(dev_.raw(), 1, &kfId, frame->id(), init, &r))
+        dev_.check(rc, ("SE3Tracker::trackFrameOnPermaref (keyframe " + std::to_string(kfId) + ")").c_str());
+    // the last calcResidualAndBuffers sets these, also on the diverging one
+    pointUsage = r.pointUsage; lastGoodCount = r.lastGoodCount; lastBadCount = r.lastBadCount; lastMeanRes = r.lastMeanRes;
+    affineEstimation_a = r.affineEstimation_a; affineEstimation_b = r.affineEstimation_b;
+    diverged = r.diverged != 0; trackingWasGood = r.trackingWasGood != 0;
+    SE3 out;
+    if (diverged) return out;                                         // SE3(), :180-185, :215-220; lastResidual keeps its value
+    lastResidual = r.lastResidual;                                    // :265
+    for (int i = 0; i < 4; i++) out.q[i] = r.frameToRef_qt[i];        // referenceToFrame, :271
+    for (int i = 0; i < 3; i++) out.t[i] = r.frameToRef_qt[4 + i];
     return out;
 }
 
@@ -311,6 +397,7 @@ Sim3 Sim3Tracker::take(const lsdgpu_sim3_result& r)
 Sim3 Sim3Tracker::trackFrameSim3(TrackingReference* reference, Frame* frame, const Sim3& frameToReference_initialEstimate,
                                  int startLevel, int finalLevel)
 {
+    dev_.followGlobals();
     double init[8];
     sim3ToQts(frameToReference_initialEstimate, init);
     ActiveFrames held(dev_.frameMemory(), { reference->keyframe, frame });   // Sim3Tracker.cpp:155
@@ -324,6 +411,7 @@ void Sim3Tracker::trackFrameSim3Batch(const std::vector<TrackingReference*>& ref
                                       const std::vector<Sim3>& inits, int startLevel, int finalLevel,
                                       std::vector<Sim3>& frameToReference, std::vector<lsdgpu_sim3_result>& results)
 {
+    dev_.followGlobals();
     const size_t n = references.size();
     if (frames.size() != n || inits.size() != n) throw LsdGpuError("Sim3Tracker::trackFrameSim3Batch: list lengths differ");
     std::vector<int> refIds(n), frIds(n);
@@ -376,6 +464,7 @@ UndistorterPTAM::UndistorterPTAM(const char* configFileName)
 
 void UndistorterPTAM::install(DeviceContext& dev) const
 {
+    dev.followGlobals();
     if (!valid) throw LsdGpuError("UndistorterPTAM: invalid calibration");
     if (dev.width() != out_width || dev.height() != out_height) throw LsdGpuError("UndistorterPTAM: output size differs from the device context");
     dev.check(lsdgpu_set_undistorter(dev.raw(), in_width, in_height, passThrough ? nullptr : remapX.data(), passThrough ? nullptr : remapY.data()),
@@ -384,6 +473,7 @@ void UndistorterPTAM::install(DeviceContext& dev) const
 
 void UndistorterPTAM::undistort(DeviceContext& dev, const unsigned char* image, unsigned char* result) const
 {
+    dev.followGlobals();
     dev.check(lsdgpu_undistort_u8(dev.raw(), image, result), "UndistorterPTAM::undistort");
 }
 
@@ -412,6 +502,7 @@ UndistorterOpenCV::UndistorterOpenCV(const char* configFileName)
 
 void UndistorterOpenCV::install(DeviceContext& dev) const
 {
+    dev.followGlobals();
     if (!valid) throw LsdGpuError("UndistorterOpenCV: invalid calibration");
     if (dev.width() != out_width || dev.height() != out_height) throw LsdGpuError("UndistorterOpenCV: output size differs from the device context");
     dev.check(lsdgpu_set_undistorter_opencv(dev.raw(), in_width, in_height, map1_.data(), map2_.data()), "UndistorterOpenCV::install");
@@ -419,6 +510,7 @@ void UndistorterOpenCV::install(DeviceContext& dev) const
 
 void UndistorterOpenCV::undistort(DeviceContext& dev, const unsigned char* image, unsigned char* result) const
 {
+    dev.followGlobals();
     dev.check(lsdgpu_undistort_u8(dev.raw(), image, result), "UndistorterOpenCV::undistort");
 }
 
@@ -444,20 +536,27 @@ DepthMap::DepthMap(DeviceContext& dev, int w, int h, const Matrix3f&) : dev_(dev
     if (w != dev.width() || h != dev.height()) throw LsdGpuError("DepthMap: size differs from the device context");
     reset();
 }
-void DepthMap::reset() { dev_.check(lsdgpu_depth_reset(dev_.raw()), "DepthMap::reset"); }
+void DepthMap::reset()
+{
+    dev_.followGlobals();
+    dev_.check(lsdgpu_depth_reset(dev_.raw()), "DepthMap::reset");
+}
 void DepthMap::invalidate()
 {
+    dev_.followGlobals();
     activeKeyFrame = nullptr;
     dev_.check(lsdgpu_depth_invalidate(dev_.raw()), "DepthMap::invalidate");
 }
 void DepthMap::initializeFromGTDepth(Frame* new_frame)
 {
+    dev_.followGlobals();
     new_frame->getActiveLock();                                         // DepthMap.cpp:969
     dev_.check(lsdgpu_depth_init_from_gt(dev_.raw(), new_frame->id()), "DepthMap::initializeFromGTDepth");
     activeKeyFrame = new_frame;
 }
 void DepthMap::initializeRandomly(Frame* new_frame)
 {   // DepthMap.cpp:883-916: the rand() draws stay on the host, the hypotheses are uploaded
+    dev_.followGlobals();
     new_frame->getActiveLock();                                         // DepthMap.cpp:885
     std::vector<float> maxGrad((size_t)width_ * height_);
     dev_.check(lsdgpu_frame_download(dev_.raw(), new_frame->id(), LSDGPU_BUF_MAXGRAD, 0, maxGrad.data()), "DepthMap::initializeRandomly");
@@ -481,8 +580,17 @@ void DepthMap::initializeRandomly(Frame* new_frame)
     dev_.check(lsdgpu_depth_set_hypotheses(dev_.raw(), new_frame->id(), hyp.data(), 0, 1), "DepthMap::initializeRandomly");
     activeKeyFrame = new_frame;
 }
+void DepthMap::setFromExistingKF(Frame* kf)
+{   // DepthMap.cpp:920-962
+    dev_.followGlobals();
+    kf->getActiveLock();                                                // :924; rebuilds the levels of a minimized keyframe
+    dev_.check(lsdgpu_depth_set_from_existing_kf(dev_.raw(), kf->id()), "DepthMap::setFromExistingKF");
+    kf->numMappedOnThis = 0; kf->numFramesTrackedOnThis = 0;            // :932-933
+    activeKeyFrame = kf;
+}
 void DepthMap::setFromExistingKF(Frame* kf, const float* idepth, const float* idepthVar, const unsigned char* validity)
 {   // DepthMap.cpp:920-962
+    dev_.followGlobals();
     kf->getActiveLock();                                                // DepthMap.cpp:924
     std::vector<lsdgpu_hyp> hyp((size_t)width_ * height_);
     std::memset(hyp.data(), 0, hyp.size() * sizeof(lsdgpu_hyp));
@@ -502,6 +610,7 @@ void DepthMap::setFromExistingKF(Frame* kf, const float* idepth, const float* id
 }
 void DepthMap::updateKeyframe(std::deque<std::shared_ptr<Frame>> referenceFrames)
 {
+    dev_.followGlobals();
     if (!isValid()) throw LsdGpuError("DepthMap::updateKeyframe: assert(isValid())");
     std::vector<Frame*> used{ activeKeyFrame };
     for (auto& f : referenceFrames) used.push_back(f.get());            // the device reads their images and masks
@@ -531,6 +640,7 @@ void DepthMap::updateKeyframe(std::deque<std::shared_ptr<Frame>> referenceFrames
 }
 void DepthMap::createKeyFrame(Frame* new_keyframe)
 {
+    dev_.followGlobals();
     if (!isValid()) throw LsdGpuError("DepthMap::createKeyFrame: assert(isValid())");
     if (!new_keyframe || !new_keyframe->hasTrackingParent()) throw LsdGpuError("DepthMap::createKeyFrame: new keyframe has no tracking parent");
     ActiveFrames held(dev_.frameMemory(), { activeKeyFrame, new_keyframe });   // DepthMap.cpp:1256, :1229
@@ -545,12 +655,14 @@ void DepthMap::createKeyFrame(Frame* new_keyframe)
 }
 void DepthMap::finalizeKeyFrame()
 {
+    dev_.followGlobals();
     if (!isValid()) throw LsdGpuError("DepthMap::finalizeKeyFrame: assert(isValid())");
     activeKeyFrame->getActiveLock();
     dev_.check(lsdgpu_depth_finalize_keyframe(dev_.raw()), "DepthMap::finalizeKeyFrame");
 }
 void DepthMap::download(std::vector<lsdgpu_hyp>& out)
 {
+    dev_.followGlobals();
     out.resize((size_t)width_ * height_);
     dev_.check(lsdgpu_depth_download(dev_.raw(), out.data()), "DepthMap::download");
 }

@@ -5,6 +5,10 @@
 //   lsd_slam::DepthMap::updateKeyframe        DepthEstimation/DepthMap.h:58
 //   lsd_slam::DepthMap::createKeyFrame        DepthEstimation/DepthMap.h:63
 //
+// and the calls SlamSystem's SLAM mode adds (SlamSystem.cpp:405, 496, 1298-1304; TrackableKeyFrameSearch.cpp:126-135;
+// Relocalizer.cpp:172-188): Frame::setPermaRef, SE3Tracker::checkPermaRefOverlap / trackFrameOnPermaref and
+// DepthMap::setFromExistingKF(Frame*).
+//
 // The reference's headers need Eigen / Sophus / Boost / OpenCV, none of which exist in this image, so this
 // header carries minimal stand-ins (lsd_slam::SE3, Sim3, Matrix3f) with the same semantics; inside
 // lsd_slam_core the adapter in INTEGRATION.md maps them 1:1 onto Sophus::SE3d / Sophus::Sim3d / Eigen::Matrix3f.
@@ -67,6 +71,15 @@ public:
 
 class Frame;
 class DeviceContext;
+class TrackingReference;
+
+// util/settings.cpp:80-88: the run-time globals the device path reads, with the reference's defaults.  As in the reference they
+// are process-wide and read at every use: every adapter call that reaches the device first hands them to its context
+// (DeviceContext::followGlobals), so a change takes effect at the next call, on every context driven through the adapter.
+// With the adapter these variables are the source of truth: a direct lsdgpu_set_globals on the same context is overwritten
+// at the next adapter call.
+extern float minUseGrad, cameraPixelNoise2, depthSmoothingFactor;
+extern bool allowNegativeIdepths, useSubpixelStereo, useAffineLightningEstimation;
 
 // DataStructures/FrameMemory.h: the active-frame list of FrameMemory (FrameMemory.cpp:129-166), one per DeviceContext.  The
 // reference's heap is unbounded; a context has max_frames slots, so activating a frame (or constructing one) with every slot
@@ -107,7 +120,10 @@ private:
     size_t n_ = 0;
 };
 
-// One device context per SlamSystem (SlamSystem owns one SE3Tracker + one DepthMap, SlamSystem.h:126,131)
+// One device context per SlamSystem, shared by every tracker and the depth map of that SlamSystem: the main tracker and the
+// DepthMap, the constraint thread's SE3Tracker and Sim3Tracker (SlamSystem.cpp:89-90), TrackableKeyFrameSearch's and the
+// Relocalizer's trackers.  Frames live in the context that uploaded them; calls from several threads serialise on the
+// context's mutex.
 class DeviceContext {
 public:
     DeviceContext(int device, int w, int h, const Matrix3f& K, int maxFrames = 16);
@@ -116,6 +132,9 @@ public:
     DeviceContext& operator=(const DeviceContext&) = delete;
     lsdgpu_ctx* raw() const { return ctx_; }
     void check(int rc, const char* where) const;
+    // the globals above into the context when its values differ (lsdgpu_get_globals / lsdgpu_set_globals); every method of
+    // the adapter that reaches the device calls it first (destructors aside: releasing reads no global)
+    void followGlobals();
     int width() const { return w_; }
     int height() const { return h_; }
     int maxFrames() const { return maxFrames_; }
@@ -166,11 +185,15 @@ public:
     bool minimizeInMemory();
     // Frame.h:138-141: makes the frame active (FrameMemory::activateFrame); the device's calls need the frame in a slot
     void getActiveLock();
+    // Frame.cpp:149-174: freezes the keyframe's current level-4 point cloud for the permaRef trackers
+    // (lsdgpu_frame_set_perma_ref).  `reference` must hold this frame; otherwise LsdGpuError and nothing changes.
+    void setPermaRef(TrackingReference* reference);
 
     FramePoseStruct* pose;
     bool isActive = true;
     float initialTrackedResidual = 0;
     int numFramesTrackedOnThis = 0, numMappedOnThis = 0, numMappedOnThisTotal = 0;
+    int permaRefNumPts = 0;                                                         // Frame.h:176
 
     DeviceContext& dev() const { return dev_; }
 
@@ -203,6 +226,13 @@ public:
     SE3Tracker(const SE3Tracker&) = delete;
 
     SE3 trackFrame(TrackingReference* reference, Frame* frame, const SE3& frameToReference_initialEstimate);
+    // SE3Tracker.cpp:121-157 (lsdgpu_perma_overlap_batch, one candidate): sets and returns pointUsage
+    float checkPermaRefOverlap(Frame* reference, SE3 referenceToFrame);
+    // SE3Tracker.cpp:162-272 (lsdgpu_perma_track_batch, one candidate): tracks `frame` on the permaRef of `reference` and returns
+    // referenceToFrame (not inverted, :271), or SE3() when it diverges.  `frame` is held active for the call; `reference` is not
+    // activated: a minimized keyframe is tracked from its record and stays minimized.  Leaves numFramesTrackedOnThis and the
+    // frame's pose and tracking parent alone.
+    SE3 trackFrameOnPermaref(Frame* reference, Frame* frame, SE3 referenceToFrame);
 
     DenseDepthTrackerSettings settings;
     float pointUsage = 0, lastGoodCount = 0, lastMeanRes = 0, lastBadCount = 0, lastResidual = 0;
@@ -337,6 +367,9 @@ public:
     bool isValid() const { return activeKeyFrame != nullptr; }
     void initializeFromGTDepth(Frame* new_frame);
     void initializeRandomly(Frame* new_frame);
+    // DepthMap.cpp:920-962 from the reactivation data finalizeKeyFrame took on the device (lsdgpu_depth_set_from_existing_kf);
+    // activates kf first if FrameMemory minimized it (its record keeps that data)
+    void setFromExistingKF(Frame* kf);
     void setFromExistingKF(Frame* kf, const float* idepth_reAct, const float* idepthVar_reAct, const unsigned char* validity_reAct);
     // currentDepthMap in the reference's AoS layout (w*h records)
     void download(std::vector<lsdgpu_hyp>& out);
