@@ -431,10 +431,31 @@ int lsdgpu_depth_reset(lsdgpu_ctx* ctx);                                  /* Dep
 int lsdgpu_depth_is_valid(lsdgpu_ctx* ctx);                               /* DepthMap::isValid, DepthMap.h:71 */
 int lsdgpu_depth_invalidate(lsdgpu_ctx* ctx);                             /* DepthMap::invalidate :1215-1220 */
 int lsdgpu_depth_init_from_gt(lsdgpu_ctx* ctx, int kf_id);                /* initializeFromGTDepth :965-1018 */
-/* initializeRandomly :883-916 (host draws rand()) and setFromExistingKF :920-962 both reduce to
- * "load these hypotheses for keyframe kf_id"; reactivated != 0 also runs the regularizeDepthMap(false,24)
- * of :961 and sets activeKeyFrameIsReactivated.  do_set_depth mirrors the trailing setDepth of :915. */
+/* Load these hypotheses for keyframe kf_id (a host-side DepthMap, or setFromExistingKF :920-962 from host arrays);
+ * reactivated != 0 also runs the regularizeDepthMap(false,24) of :961 and sets activeKeyFrameIsReactivated.  do_set_depth
+ * mirrors the trailing setDepth of :915.  initializeRandomly has its own device entry point, lsdgpu_depth_init_random. */
 int lsdgpu_depth_set_hypotheses(lsdgpu_ctx* ctx, int kf_id, const lsdgpu_hyp* aos, int reactivated, int do_set_depth);
+/* ---- DepthMap::initializeRandomly on the device, with the process's rand() stream ------------------------------------------
+ * Found by symbol lookup (dlsym), like lsdgpu_track_and_map_group; LSDGPU_ABI_VERSION is unchanged.
+ * rand() is glibc's random() (stdlib/random_r.c), in any of its five state types: TYPE_0 (the LCG, 8-byte initstate buffer)
+ * and TYPE_1..TYPE_4 (additive lagged-Fibonacci tables of 7, 15, 31, 63 words; TYPE_3 is what srand() / rand() use unless
+ * initstate() chose another).  The state is random_r's table and its rear index: r[i] = the i-th table word (TYPE_0: r[0] = the
+ * LCG state), rear = the rear pointer's index (TYPE_0: 0).  glibc's initstate() / setstate() buffers hold the same table after
+ * one word of MAX_TYPES * rear + type (5 * rear + type). */
+typedef struct { int32_t type; int32_t rear; uint32_t r[63]; } lsdgpu_rand_state;
+/* srandom_r(seed) (stdlib/random_r.c) for a buffer of the given type, including its deg * 10 discarded draws.  Host-only. */
+int lsdgpu_rand_state_seed(int type, unsigned seed, lsdgpu_rand_state* st);
+/* n calls of random_r: out = the n values (NULL: the state jumps ahead in O(deg^2 log n) without producing them).  Host-only. */
+int lsdgpu_rand_state_advance(lsdgpu_rand_state* st, int64_t n, int32_t* out);
+/* DepthMap::initializeRandomly(new_frame), DepthEstimation/DepthMap.cpp:883-916: kf_id becomes the active keyframe (not
+ * re-activated); every interior pixel (1 <= x <= w-2, 1 <= y <= h-2) with maxGradients > minUseGrad draws, in raster order,
+ * idepth = 0.5f + 1.0f * ((rand() % 100001) / 100000.0f) and becomes DepthMapPixelHypothesis(idepth, idepth,
+ * VAR_RANDOM_INIT_INITIAL, VAR_RANDOM_INIT_INITIAL, 20); every other interior pixel gets isValid = 0, blacklisted = 0 and keeps
+ * its other fields; border pixels keep everything.  Then Frame::setDepth (:915).  The draws are computed on the device from
+ * *state by jump-ahead.  *state is read on entry and holds the state after the last draw on return; *n_draws (may be NULL)
+ * = the number of draws.  An unknown or minimized kf_id, or a bad state (type outside 0..4, rear outside the table), is rejected
+ * before anything changes.  Waits for the device. */
+int lsdgpu_depth_init_random(lsdgpu_ctx* ctx, int kf_id, lsdgpu_rand_state* state, int64_t* n_draws);
 /* DepthMap::updateKeyframe(referenceFrames) :1072-1213; ref_ids oldest first, all tracked on the active KF */
 int lsdgpu_depth_update_keyframe(lsdgpu_ctx* ctx, const int* ref_ids, int n_refs);
 /* The same with the reference-frame set-up of :1085-1101 spelled out.  DepthMap::updateKeyframe accepts frames that were tracked

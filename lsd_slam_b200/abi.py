@@ -84,6 +84,37 @@ class GroupStep(C.Structure):
 GROUP_MAX_STEPS = 8
 
 
+class RandState(C.Structure):
+    """lsdgpu_rand_state (include/lsdgpu.h): glibc's random() state -- random_r's table and its rear index, in any of the five
+    state types (0: the LCG; 1..4: tables of 7, 15, 31, 63 words; rand() after srand() uses type 3).  The stream
+    ``DepthMap.initializeRandomly`` draws from (DepthMap.cpp:898)."""
+    _fields_ = [("type", C.c_int32), ("rear", C.c_int32), ("r", C.c_uint32 * 63)]
+
+    @classmethod
+    def from_seed(cls, seed: int, type: int = 3) -> "RandState":
+        """srandom_r(seed) for a buffer of the given type (srand(seed) for type 3)"""
+        st = cls()
+        if load().lsdgpu_rand_state_seed(int(type), C.c_uint(seed & 0xffffffff), C.byref(st)) != 0:
+            raise ValueError(f"bad random state type {type}")
+        return st
+
+    def copy(self) -> "RandState":
+        st = RandState()
+        C.memmove(C.byref(st), C.byref(self), C.sizeof(RandState))
+        return st
+
+    def advance(self, n: int, values: bool = True):
+        """n calls of random(): returns them (int32) when ``values``, otherwise jumps ahead; the state moves on in place"""
+        out = np.zeros(n, np.int32) if values else None
+        p = out.ctypes.data_as(C.POINTER(C.c_int32)) if values else None
+        if load().lsdgpu_rand_state_advance(C.byref(self), C.c_int64(n), p) != 0:
+            raise ValueError("bad random state or count")
+        return out
+
+    def __eq__(self, other) -> bool:
+        return isinstance(other, RandState) and bytes(self) == bytes(other)
+
+
 # every symbol include/lsdgpu.h declares: (name, restype, argtypes)
 _vp, _fp, _dp, _ip, _u8p = C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_double), C.POINTER(C.c_int), C.POINTER(C.c_uint8)
 class Sim3Result(C.Structure):
@@ -204,6 +235,9 @@ SYMBOLS = [
     ("lsdgpu_depth_invalidate", C.c_int, [_vp]),
     ("lsdgpu_depth_init_from_gt", C.c_int, [_vp, C.c_int]),
     ("lsdgpu_depth_set_hypotheses", C.c_int, [_vp, C.c_int, C.POINTER(Hyp), C.c_int, C.c_int]),
+    ("lsdgpu_rand_state_seed", C.c_int, [C.c_int, C.c_uint, C.POINTER(RandState)]),
+    ("lsdgpu_rand_state_advance", C.c_int, [C.POINTER(RandState), C.c_int64, C.POINTER(C.c_int32)]),
+    ("lsdgpu_depth_init_random", C.c_int, [_vp, C.c_int, C.POINTER(RandState), C.POINTER(C.c_int64)]),
     ("lsdgpu_depth_update_keyframe", C.c_int, [_vp, _ip, C.c_int]),
     ("lsdgpu_depth_update_keyframe_refs", C.c_int, [_vp, C.c_void_p, C.c_int]),
     ("lsdgpu_peer_export", C.c_int, [_vp, C.c_void_p]),
@@ -791,6 +825,16 @@ class DepthMap:
 
     def initializeFromGTDepth(self, kf_id: int):
         self.ctx._ck(self.ctx.L.lsdgpu_depth_init_from_gt(self.ctx.ptr, kf_id))
+
+    def initializeRandomly(self, kf_id: int, state: RandState) -> RandState:
+        """DepthMap::initializeRandomly (DepthMap.cpp:883-916) on the device, drawing from ``state`` as the reference draws from
+        rand(); returns the state after the last draw (``state`` itself is left as it was).  The number of draws is kept in
+        ``last_draws``."""
+        st = state.copy()
+        n = C.c_int64(0)
+        self.ctx._ck(self.ctx.L.lsdgpu_depth_init_random(self.ctx.ptr, kf_id, C.byref(st), C.byref(n)))
+        self.last_draws = n.value
+        return st
 
     def setHypotheses(self, kf_id: int, hyp: np.ndarray, reactivated=False, do_set_depth=True):
         a = np.ascontiguousarray(hyp)

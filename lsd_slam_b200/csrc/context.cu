@@ -99,6 +99,9 @@ static size_t carveArena(lsdgpu_ctx* ctx, char* base)
     ctx->seqCounts = (int*)take((size_t)seqRuns * 4);
     ctx->dLastMask = (uint8_t*)take(n0 / 4);
     ctx->dGroupSegs = take(TP_MAX_GROUP * sizeof(TrackGroupSeg));
+    ctx->rndTab = (uint32_t*)take((size_t)RND_TYPES * RND_TYPE_WORDS * 4);
+    ctx->rndTiles = (int*)take(((size_t)divUp((int)n0, RND_TILE) + 1) * 4);
+    ctx->rndOut = (uint32_t*)take(4 + RND_ROW * 4);
     return used;
 }
 

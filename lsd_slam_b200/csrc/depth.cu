@@ -4,6 +4,7 @@
 #include "internal.cuh"
 #include "depth.cuh"
 #include "seqsum.cuh"
+#include "rand.cuh"
 
 #include <utility>
 
@@ -66,6 +67,242 @@ extern "C" int lsdgpu_depth_init_from_gt(lsdgpu_ctx* ctx, int kf_id)
     LAUNCH(ctx);
     LSD_CHECK(ctx, cudaGetLastError());
     return setDepthOnKeyframe(ctx, kf);
+}
+
+// ---- DepthMap::initializeRandomly, DepthMap.cpp:883-916, with the caller's rand() stream (rand.cuh) ----------------------------
+// Three kernels: the draws per tile of RND_TILE pixels, their offsets (a scan), and per tile the jump to its first draw, its
+// draws and the cells.  A pixel's draw index is the number of selected pixels before it in raster order.
+struct RndEntry {
+    int type, deg, winLen;               // winLen: words of the window (deg, 1 for the LCG)
+    float minGrad;                       // MIN_ABS_GRAD_CREATE == minUseGrad, util/settings.h:157
+    uint32_t W[RND_ROW];                 // the window before the first draw
+};
+
+// exclusive prefix of v over the block (NW warps); total = the block's sum
+template <int NW>
+__device__ __forceinline__ int rndBlockScan(int v, int* sWarp, int& total)
+{
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    int x = v;
+    for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) sWarp[wid] = x;
+    __syncthreads();
+    int off = 0;
+    total = 0;
+    for (int k = 0; k < NW; k++) {
+        const int t = sWarp[k];
+        if (k < wid) off += t;
+        total += t;
+    }
+    __syncthreads();
+    return off + x - v;
+}
+
+// the interior pixels (DepthMap.cpp:892-894) with maxGradients > MIN_ABS_GRAD_CREATE (:896) among the 4 pixels from i0
+__device__ __forceinline__ int rndSelect4(const float* __restrict__ maxgrad, int i0, int w, int h, float minGrad, bool sel[4])
+{
+    int c = 0;
+    const float4 g = *(const float4*)(maxgrad + i0);           // w % 16 == 0: the 4 pixels share a row
+    const float gv[4] = { g.x, g.y, g.z, g.w };
+    const int y = i0 / w, x0 = i0 - y * w;
+    const bool row = y >= 1 && y <= h - 2;
+    for (int k = 0; k < 4; k++) {
+        sel[k] = row && x0 + k >= 1 && x0 + k <= w - 2 && gv[k] > minGrad;
+        c += sel[k];
+    }
+    return c;
+}
+
+__global__ void __launch_bounds__(256) k_rnd_count(const float* __restrict__ maxgrad, int w, int h, float minGrad, int* __restrict__ tiles)
+{
+    __shared__ int sWarp[8];
+    const int i0 = blockIdx.x * RND_TILE + 4 * threadIdx.x;
+    bool sel[4];
+    const int c = i0 < w * h ? rndSelect4(maxgrad, i0, w, h, minGrad, sel) : 0;
+    int total;
+    rndBlockScan<8>(c, sWarp, total);
+    if (threadIdx.x == 0) tiles[blockIdx.x] = total;
+}
+
+// tiles[t] <- the first draw of tile t, tiles[nTiles] = out[0] = the number of draws N; the window after the last draw starts with
+// the entry window's words that no draw replaces
+__global__ void __launch_bounds__(1024) k_rnd_scan(int* __restrict__ tiles, int nTiles, RndEntry e, uint32_t* __restrict__ out)
+{
+    __shared__ int sWarp[32];
+    int carry = 0;
+    for (int base = 0; base < nTiles; base += 1024) {
+        const int i = base + threadIdx.x;
+        const int v = i < nTiles ? tiles[i] : 0;
+        int total;
+        const int x = rndBlockScan<32>(v, sWarp, total);
+        if (i < nTiles) tiles[i] = carry + x;
+        carry += total;
+    }
+    if (threadIdx.x == 0) { tiles[nTiles] = carry; out[0] = (uint32_t)carry; }
+    for (int m = threadIdx.x; m + carry < e.winLen; m += blockDim.x) out[1 + m] = e.W[m + carry];
+}
+
+// out[o] = sum_m rows[o * rowStride + m] * vecs[o * vecStride + m] over m < n, for o < nOut <= 64: four threads per output.
+// out may alias vecs: every read is done before the first write.
+__device__ __forceinline__ void rndBlockDots(const uint32_t* rows, int rowStride, const uint32_t* vecs, int vecStride, int n, int nOut,
+                                             uint32_t* out)
+{
+    const int o = threadIdx.x >> 2, q = threadIdx.x & 3;
+    uint32_t s = o < nOut ? rndDot(rows + o * rowStride, vecs + o * vecStride, n, q, 4) : 0u;
+    s += __shfl_xor_sync(0xffffffffu, s, 1);
+    s += __shfl_xor_sync(0xffffffffu, s, 2);
+    __syncthreads();
+    if (o < nOut && q == 0) out[o] = s;
+    __syncthreads();
+}
+
+__global__ void __launch_bounds__(256) k_rnd_fill(HypField cur, const float* __restrict__ maxgrad, int w, int h, const int* __restrict__ tiles,
+                                                  const uint32_t* __restrict__ tab, RndEntry e, uint32_t* __restrict__ out)
+{
+    __shared__ uint32_t sW[RND_ROW], sExt[2 * RND_ROW], sVal[RND_TILE + RND_ROW];
+    __shared__ int sWarp[8];
+    const int n = w * h;
+    const int i0 = blockIdx.x * RND_TILE + 4 * threadIdx.x;
+    bool sel[4] = { false, false, false, false };
+    const int c = i0 < n ? rndSelect4(maxgrad, i0, w, h, e.minGrad, sel) : 0;
+    int total;
+    int idx = rndBlockScan<8>(c, sWarp, total);
+    const int s = tiles[blockIdx.x];                        // the tile's first draw
+    const int N = tiles[gridDim.x];
+    if (total > 0) {
+        if (e.type == 0) {
+            for (int j = threadIdx.x; j < total; j += blockDim.x) sVal[j] = rndLcgAt(e.W[0], (uint64_t)s + j + 1);
+            __syncthreads();
+        } else {
+            const uint32_t* pw = tab + e.type * RND_TYPE_WORDS;
+            const uint32_t* gen = pw + RND_POW_ROWS * RND_ROW;
+            if (threadIdx.x < e.deg) sW[threadIdx.x] = e.W[threadIdx.x];
+            __syncthreads();
+            for (int b = 0; (s >> b) != 0; b++) {               // the window at draw s: one jump per set bit
+                if (!((s >> b) & 1)) continue;
+                if (threadIdx.x < e.deg) sExt[threadIdx.x] = sW[threadIdx.x];
+                rndBlockDots(gen, RND_ROW, sW, 0, e.deg, e.deg - 1, sExt + e.deg);
+                rndBlockDots(pw + b * RND_ROW, 0, sExt, 1, e.deg, e.deg, sW);
+            }
+            for (int q = 0; q < total; q += RND_ROW) {          // 64 draws at a time, then the window 64 draws later
+                rndBlockDots(gen, RND_ROW, sW, 0, e.deg, RND_ROW, sVal + q);
+                if (threadIdx.x < e.deg) sW[threadIdx.x] = sVal[q + RND_ROW - e.deg + threadIdx.x];
+                __syncthreads();
+            }
+        }
+    }
+    if (i0 < n) {
+        const int y = i0 / w, x0 = i0 - y * w;
+        for (int k = 0; k < 4; k++) {
+            const int i = i0 + k;
+            if (y < 1 || y > h - 2 || x0 + k < 1 || x0 + k > w - 2) continue;   // border: untouched
+            if (sel[k]) {                                       // DepthMapPixelHypothesis(idepth, idepth, VAR, VAR, 20), :898-903
+                const float id = rndIdepth(rndOutput(e.type, sVal[idx++]));
+                cur.hf[i] = make_float4(id, VAR_RANDOM_INIT_INITIAL, id, VAR_RANDOM_INIT_INITIAL);
+                cur.hi[i] = make_int4(1, 0, 20, __float_as_int(0.f));
+            } else {                                            // :907-908
+                int4 hi = cur.hi[i];
+                hi.x = 0; hi.y = 0;
+                cur.hi[i] = hi;
+            }
+        }
+    }
+    for (int j = threadIdx.x; j < total; j += blockDim.x) {    // the last winLen draws are the window after the last draw
+        const int m = s + j + e.winLen - N;
+        if (m >= 0) out[1 + m] = sVal[j];
+    }
+}
+
+static bool rndStateOk(const lsdgpu_rand_state* st)
+{
+    return st && st->type >= 0 && st->type < RND_TYPES && st->rear >= 0 && st->rear < rndWindowLen(st->type);
+}
+
+extern "C" int lsdgpu_rand_state_seed(int type, unsigned seed, lsdgpu_rand_state* st)
+{   // __srandom_r, stdlib/random_r.c
+    if (!st || type < 0 || type >= RND_TYPES) return -2;
+    memset(st, 0, sizeof(*st));
+    st->type = type;
+    if (seed == 0) seed = 1;
+    st->r[0] = seed;
+    if (type == 0) return 0;
+    const RndKind k = rndKind(type);
+    int32_t word = (int32_t)seed;
+    for (int i = 1; i < k.deg; i++) {                        // state[i] = (16807 * state[i - 1]) % 2147483647
+        const long hi = word / 127773, lo = word % 127773;
+        word = (int32_t)(16807 * lo - 2836 * hi);
+        if (word < 0) word += 2147483647;
+        st->r[i] = (uint32_t)word;
+    }
+    return lsdgpu_rand_state_advance(st, (int64_t)k.deg * 10, nullptr);
+}
+
+extern "C" int lsdgpu_rand_state_advance(lsdgpu_rand_state* st, int64_t n, int32_t* out)
+{   // __random_r, stdlib/random_r.c, n times
+    if (!rndStateOk(st) || n < 0) return -2;
+    if (st->type == 0) {
+        if (!out) { st->r[0] = rndLcgAt(st->r[0], (uint64_t)n); return 0; }
+        for (int64_t i = 0; i < n; i++) out[i] = (int32_t)(st->r[0] = (st->r[0] * 1103515245u + 12345u) & 0x7fffffffu);
+        return 0;
+    }
+    const RndKind k = rndKind(st->type);
+    if (out) {
+        int r = st->rear, f = (r + k.sep) % k.deg;
+        for (int64_t i = 0; i < n; i++) {
+            st->r[f] += st->r[r];
+            out[i] = rndOutput(st->type, st->r[f]);
+            if (++f == k.deg) f = 0;
+            if (++r == k.deg) r = 0;
+        }
+        st->rear = r;
+        return 0;
+    }
+    uint32_t W[RND_ROW];
+    rndTableToWindow(st->type, st->rear, st->r, W);
+    rndJumpWindow(st->type, W, (uint64_t)n);
+    st->rear = (int)((st->rear + n) % k.deg);
+    rndWindowToTable(st->type, st->rear, W, st->r);
+    return 0;
+}
+
+extern "C" int lsdgpu_depth_init_random(lsdgpu_ctx* ctx, int kf_id, lsdgpu_rand_state* state, int64_t* n_draws)
+{ LSD_LOCK(ctx);   // DepthMap::initializeRandomly :883-916
+    if (!ctx) return -2;
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    FrameSlot* kf = findSlot(ctx, kf_id);
+    if (!kf) return failMissing(ctx, kf_id, "initializeRandomly: unknown keyframe id");
+    if (!rndStateOk(state)) return lsd_fail(ctx, "initializeRandomly: bad random state (type outside 0..4, or rear index outside its table)");
+    if (!ctx->rndTabReady) {
+        LSD_CHECK(ctx, cudaMemcpyAsync(ctx->rndTab, rndTables().w, sizeof(RndTables::w), cudaMemcpyHostToDevice, ctx->stream));
+        ctx->rndTabReady = true;
+    }
+    RndEntry e;
+    memset(&e, 0, sizeof(e));
+    e.type = state->type; e.deg = rndKind(e.type).deg; e.winLen = rndWindowLen(e.type);
+    e.minGrad = ctx->g.minUseGrad;
+    rndTableToWindow(e.type, state->rear, state->r, e.W);
+    const int n = ctx->w * ctx->h, nTiles = divUp(n, RND_TILE);
+    k_rnd_count<<<nTiles, 256, 0, ctx->stream>>>(kf->maxgrad, ctx->w, ctx->h, e.minGrad, ctx->rndTiles);
+    LAUNCH(ctx);
+    k_rnd_scan<<<1, 1024, 0, ctx->stream>>>(ctx->rndTiles, nTiles, e, ctx->rndOut);
+    LAUNCH(ctx);
+    k_rnd_fill<<<nTiles, 256, 0, ctx->stream>>>(ctx->cur, kf->maxgrad, ctx->w, ctx->h, ctx->rndTiles, ctx->rndTab, e, ctx->rndOut);
+    LAUNCH(ctx);
+    LSD_CHECK(ctx, cudaGetLastError());
+    ctx->activeKf = kf_id; ctx->activeKfReactivated = false;       // :887-890
+    int r = setDepthOnKeyframe(ctx, kf);                            // :915
+    if (r) return r;
+    uint32_t* res = (uint32_t*)ctx->hStageF;
+    LSD_CHECK(ctx, cudaMemcpyAsync(res, ctx->rndOut, (1 + RND_ROW) * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+    const int64_t draws = res[0];
+    if (e.type != 0) state->rear = (int)((state->rear + draws) % e.deg);
+    rndWindowToTable(e.type, state->rear, res + 1, state->r);
+    if (n_draws) *n_draws = draws;
+    return 0;
 }
 
 static int runRegularize(lsdgpu_ctx* ctx, bool removeOcclusions, int validityTH)

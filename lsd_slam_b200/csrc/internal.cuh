@@ -104,6 +104,15 @@ struct ObserveParams {
 // number of reduction channels of one tracker evaluation (see track.cuh)
 #define EV_NCH 40
 
+// sizes of the random start's buffers (the generator itself is rand.cuh): glibc's 5 state types, polynomials / windows of up to
+// 63 words padded to 64, per type 63 jump rows + 64 draw rows; the depth map is split into tiles of RND_TILE pixels
+#define RND_TYPES 5
+#define RND_ROW 64
+#define RND_POW_ROWS 63
+#define RND_GEN_ROWS 64
+#define RND_TYPE_WORDS ((RND_POW_ROWS + RND_GEN_ROWS) * RND_ROW)
+#define RND_TILE 1024
+
 struct lsdgpu_ctx {
     // Every entry point of the C ABI holds this for its whole duration (LSD_LOCK): one context may be shared by SlamSystem's
     // tracking and mapping threads (SlamSystem.cpp:111, :206) -- their calls serialise here, as they do on the frame / keyframe
@@ -139,6 +148,12 @@ struct lsdgpu_ctx {
     float4* propVal = nullptr;           // per-source (new_idepth, new_var, validity, -)
     double* dScalars = nullptr;          // small device scratch for reductions (sum, count)
     double* hScalars = nullptr;          // pinned mirror
+    // DepthMap::initializeRandomly (lsdgpu_depth_init_random, rand.cuh): the generator's tables of all types (copied on first use),
+    // per-tile draw counts then offsets, and the result (number of draws, then the window after the last draw)
+    uint32_t* rndTab = nullptr;
+    bool rndTabReady = false;
+    int* rndTiles = nullptr;
+    uint32_t* rndOut = nullptr;
 
     // tracker scratch
     float* evPartials = nullptr;         // [maxBlocks][EV_NCH]

@@ -555,29 +555,28 @@ void DepthMap::initializeFromGTDepth(Frame* new_frame)
     activeKeyFrame = new_frame;
 }
 void DepthMap::initializeRandomly(Frame* new_frame)
-{   // DepthMap.cpp:883-916: the rand() draws stay on the host, the hypotheses are uploaded
+{   // DepthMap.cpp:883-916 on the device, drawing from the process's rand() stream and leaving it where the reference's loop would
     dev_.followGlobals();
     new_frame->getActiveLock();                                         // DepthMap.cpp:885
-    std::vector<float> maxGrad((size_t)width_ * height_);
-    dev_.check(lsdgpu_frame_download(dev_.raw(), new_frame->id(), LSDGPU_BUF_MAXGRAD, 0, maxGrad.data()), "DepthMap::initializeRandomly");
-    lsdgpu_globals g;
-    dev_.check(lsdgpu_get_globals(dev_.raw(), &g), "DepthMap::initializeRandomly");
-    const float minAbsGradCreate = g.minUseGrad;                    // MIN_ABS_GRAD_CREATE == minUseGrad (util/settings.h:157)
-    // interior pixels as in the reference; the border keeps the constructor's state (isValid = false, blacklisted = 0),
-    // which is what a freshly constructed / reset DepthMap holds there (DepthMapPixelHypothesis.h:63-64, DepthMap.cpp:102-109)
-    std::vector<lsdgpu_hyp> hyp((size_t)width_ * height_);
-    std::memset(hyp.data(), 0, hyp.size() * sizeof(lsdgpu_hyp));
-    for (int y = 1; y < height_ - 1; y++)
-        for (int x = 1; x < width_ - 1; x++) {
-            lsdgpu_hyp& h = hyp[x + y * width_];
-            if (maxGrad[x + y * width_] > minAbsGradCreate) {
-                float idepth = 0.5f + 1.0f * ((rand() % 100001) / 100000.0f);
-                h.isValid = 1; h.blacklisted = 0; h.nextStereoFrameMinID = 0; h.validity_counter = 20;
-                h.idepth = idepth; h.idepth_smoothed = idepth;
-                h.idepth_var = 0.5f * 0.5f * 0.5f; h.idepth_var_smoothed = 0.5f * 0.5f * 0.5f;   // VAR_RANDOM_INIT_INITIAL
-            }
-        }
-    dev_.check(lsdgpu_depth_set_hypotheses(dev_.raw(), new_frame->id(), hyp.data(), 0, 1), "DepthMap::initializeRandomly");
+    // initstate() switches rand() to `tmp` and returns the word before the live table: 5 * rear + type (glibc's MAX_TYPES == 5),
+    // then the table; setstate() of the same pointer switches back and reads that word again
+    int32_t tmp[32];
+    int32_t* live = (int32_t*)initstate(1, (char*)tmp, sizeof(tmp));
+    if (!live) throw LsdGpuError("DepthMap::initializeRandomly: cannot read the rand() state");
+    lsdgpu_rand_state st;
+    std::memset(&st, 0, sizeof(st));
+    st.type = live[0] % 5;
+    st.rear = st.type == 0 ? 0 : live[0] / 5;
+    static const int kDeg[5] = { 1, 7, 15, 31, 63 };                    // table words per type (stdlib/random_r.c)
+    const int deg = st.type >= 0 && st.type < 5 ? kDeg[st.type] : 0;
+    std::memcpy(st.r, live + 1, (size_t)deg * 4);
+    const int rc = lsdgpu_depth_init_random(dev_.raw(), new_frame->id(), &st, nullptr);
+    if (rc == 0) {
+        live[0] = st.type == 0 ? 0 : 5 * st.rear + st.type;
+        std::memcpy(live + 1, st.r, (size_t)deg * 4);
+    }
+    setstate((char*)live);
+    dev_.check(rc, "DepthMap::initializeRandomly");
     activeKeyFrame = new_frame;
 }
 void DepthMap::setFromExistingKF(Frame* kf)

@@ -94,6 +94,16 @@ class GpuStream:
         self.last_pose = IDENT.copy()
         self.keyframe_ids, self.keyframe_cam_to_world = [fid], [IDENT_QTS.copy()]
 
+    def init_random(self, fid: int, image_u8: np.ndarray, state: abi.RandState) -> abi.RandState:
+        """SlamSystem::randomInit, SlamSystem.cpp:857-886: the map starts from one image, its hypotheses drawn on the device from
+        ``state`` (the rand() stream, DepthMap.cpp:898).  Returns the state after the last draw."""
+        self.ctx.upload(fid, image_u8)
+        st = self.map.initializeRandomly(fid, state)
+        self.kf_id = fid
+        self.last_pose = IDENT.copy()
+        self.keyframe_ids, self.keyframe_cam_to_world = [fid], [IDENT_QTS.copy()]
+        return st
+
     def keyframe_cam_to_world_f7(self) -> np.ndarray:
         """(n, 7) float32 camToWorld of keyframe_ids, as keyframeMsg carries them"""
         return np.stack([qts_to_sim3f(q) for q in self.keyframe_cam_to_world])
