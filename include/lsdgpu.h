@@ -344,6 +344,25 @@ int lsdgpu_frame_download_device(lsdgpu_ctx* ctx, int frame_id, int what, int le
 int lsdgpu_map_export_pointcloud_device(lsdgpu_ctx* ctx, int n, const int* kf_ids, const float* camToWorld, int level,
                                         const lsdgpu_cloud_filter* f, int layout, void* d_out, int64_t capacity_points,
                                         int64_t* n_points_out, int32_t* counts, void* stream);
+/* Depth in and out of device memory, under the same rules.  Float planes are the context's w x h floats with a row pitch in bytes
+ * that is a multiple of 4 and >= 4 * w, 4-byte aligned.  Hypotheses are w * h lsdgpu_hyp records (32 B, the reference's
+ * DepthMapPixelHypothesis layout) in raster order, 16-byte aligned.  An unknown or minimized id is rejected as by the host twin.
+ * Frame::setDepthFromGroundTruth (Frame.cpp:245-293), as lsdgpu_frame_set_depth_gt, from a device plane of metric depth */
+int lsdgpu_frame_set_depth_gt_device(lsdgpu_ctx* ctx, int frame_id, const float* d_depth, size_t pitch_bytes, float cov_scale,
+                                     void* stream);
+/* lsdgpu_frame_set_idepth from two device planes with the same pitch: two device-to-device copies */
+int lsdgpu_frame_set_idepth_device(lsdgpu_ctx* ctx, int frame_id, const float* d_idepth, const float* d_idepthVar, size_t pitch_bytes,
+                                   void* stream);
+/* lsdgpu_depth_set_hypotheses (the hypotheses of a host-side DepthMap or a saved filter state, then optionally the
+ * regularizeDepthMap(false,24) of a re-activation and setDepth) from w * h device records */
+int lsdgpu_depth_set_hypotheses_device(lsdgpu_ctx* ctx, int kf_id, const lsdgpu_hyp* d_aos, int reactivated, int do_set_depth,
+                                       void* stream);
+/* lsdgpu_depth_download (currentDepthMap) into w * h device records, pad bytes 0; capacity_bytes >= 32 * w * h */
+int lsdgpu_depth_download_device(lsdgpu_ctx* ctx, lsdgpu_hyp* d_aos, size_t capacity_bytes, void* stream);
+/* lsdgpu_keyframe_pack_pointcloud (keyframeMsg.pointcloud, ROSOutput3DWrapper.cpp:91-110) written straight into d_out: (w >> level) *
+ * (h >> level) records of 12 B, 4-byte aligned; capacity_bytes >= 12 per record */
+int lsdgpu_keyframe_pack_pointcloud_device(lsdgpu_ctx* ctx, int kf_id, int publish_level, lsdgpu_input_point_dense* d_out,
+                                           size_t capacity_bytes, void* stream);
 /* Frame::takeReActivationData(currentDepthMap), DataStructures/Frame.cpp:107-145: snapshot of the ACTIVE depth map into the
  * keyframe's idepth_reAct / idepthVar_reAct / validity_reAct -- kept on the device.  lsdgpu_depth_finalize_keyframe calls it
  * (DepthMap.cpp:1387); exposed for re-activation bookkeeping outside finalize. */

@@ -220,6 +220,11 @@ SYMBOLS = [
     ("lsdgpu_frame_download_device", C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, _vp]),
     ("lsdgpu_map_export_pointcloud_device", C.c_int, [_vp, C.c_int, _ip, _fp, C.c_int, C.c_void_p, C.c_int, _vp, C.c_int64,
                                                       C.POINTER(C.c_int64), C.POINTER(C.c_int32), _vp]),
+    ("lsdgpu_frame_set_depth_gt_device", C.c_int, [_vp, C.c_int, _vp, C.c_size_t, C.c_float, _vp]),
+    ("lsdgpu_frame_set_idepth_device", C.c_int, [_vp, C.c_int, _vp, _vp, C.c_size_t, _vp]),
+    ("lsdgpu_depth_set_hypotheses_device", C.c_int, [_vp, C.c_int, _vp, C.c_int, C.c_int, _vp]),
+    ("lsdgpu_depth_download_device", C.c_int, [_vp, _vp, C.c_size_t, _vp]),
+    ("lsdgpu_keyframe_pack_pointcloud_device", C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_size_t, _vp]),
     ("lsdgpu_frame_take_reactivation_data", C.c_int, [_vp, C.c_int]),
     ("lsdgpu_frame_download_reactivation_data", C.c_int, [_vp, C.c_int, _fp, _fp, C.POINTER(C.c_uint8)]),
     ("lsdgpu_depth_set_from_existing_kf", C.c_int, [_vp, C.c_int]),
@@ -304,14 +309,43 @@ def _cuda_stream(t, device: int, what: str) -> int:
     return torch.cuda.current_stream(t.device).cuda_stream
 
 
-def _device_image(t, device: int, w: int, h: int, what: str):
-    """a 2-D uint8 CUDA tensor of h x w whose rows are contiguous -> (pointer, row pitch in bytes, stream)"""
-    _tensor_dtype(t, "uint8", what)
+def _device_image(t, device: int, w: int, h: int, what: str, dtype: str = "uint8"):
+    """a 2-D CUDA tensor of h x w (uint8, or `dtype`) whose rows are contiguous -> (pointer, row pitch in bytes, stream)"""
+    _tensor_dtype(t, dtype, what)
     if t.dim() != 2 or tuple(t.shape) != (h, w):
         raise ValueError(f"{what}: needs shape ({h}, {w}), not {tuple(t.shape)}")
     if t.stride(1) != 1 or t.stride(0) < w:
         raise ValueError(f"{what}: needs contiguous rows (stride(1) == 1, stride(0) >= {w}), not strides {t.stride()}")
-    return t.data_ptr(), t.stride(0), _cuda_stream(t, device, what)
+    return t.data_ptr(), t.stride(0) * t.element_size(), _cuda_stream(t, device, what)
+
+
+def _device_out(t, dtype: str, n: int, device: int, what: str) -> int:
+    """a contiguous CUDA tensor of `dtype` with at least n elements -> the stream its device work is ordered on"""
+    _tensor_dtype(t, dtype, what)
+    if not t.is_contiguous() or t.numel() < n:
+        raise ValueError(f"{what}: needs a contiguous tensor of at least {n} elements")
+    return _cuda_stream(t, device, what)
+
+
+HYP_FIELDS = [(name, HYP_DTYPE.fields[name][1], HYP_DTYPE.fields[name][0]) for name in HYP_DTYPE.names if name != "_pad"]
+
+
+def hyp_fields(t) -> dict:
+    """the eight DepthMapPixelHypothesis fields of a (h, w, 32) uint8 tensor of hypotheses (``DepthMap.current(out=...)``, the input
+    of ``DepthMap.setHypotheses``) as (h, w) strided views of it, without copies: isValid uint8, blacklisted and validity_counter
+    int32, the others float32.  Writes to a view write the hypotheses."""
+    import torch
+    _tensor_dtype(t, "uint8", "hyp_fields")
+    if t.dim() != 3 or t.shape[2] != HYP_DTYPE.itemsize or not t.is_contiguous():
+        raise ValueError(f"hyp_fields: needs a contiguous (h, w, {HYP_DTYPE.itemsize}) uint8 tensor, not {tuple(t.shape)}")
+    out = {}
+    for name, offset, dt in HYP_FIELDS:
+        if dt == np.uint8:
+            out[name] = t[:, :, offset]
+        else:
+            words = t.view(torch.int32 if dt == np.int32 else torch.float32)       # (h, w, 8)
+            out[name] = words[:, :, offset // 4]
+    return out
 
 
 class UndistorterPTAM:
@@ -526,11 +560,28 @@ class Context:
         self._ck(self.L.lsdgpu_frame_download(self.ptr, fid, what, level, out.ctypes.data_as(_vp)))
         return out
 
-    def set_depth_gt(self, fid: int, depth: np.ndarray, cov_scale: float = 1.0):
+    def set_depth_gt(self, fid: int, depth, cov_scale: float = 1.0):
+        """Frame::setDepthFromGroundTruth from metric depth: a host array (numpy), or a 2-D float32 CUDA tensor of (h, w) with
+        contiguous rows, read on the device in order on its current stream (lsdgpu_frame_set_depth_gt_device)"""
+        if _is_tensor(depth):
+            ptr, pitch, stream = _device_image(depth, self.device, self.w, self.h, "set_depth_gt", "float32")
+            self._ck(self.L.lsdgpu_frame_set_depth_gt_device(self.ptr, fid, ptr, pitch, cov_scale, stream))
+            return
         d = np.ascontiguousarray(depth, np.float32)
         self._ck(self.L.lsdgpu_frame_set_depth_gt(self.ptr, fid, d.ctypes.data_as(_fp), cov_scale))
 
-    def set_idepth(self, fid: int, idepth: np.ndarray, var: np.ndarray):
+    def set_idepth(self, fid: int, idepth, var):
+        """level-0 idepth and idepthVar of a frame: host arrays, or two float32 CUDA tensors as set_depth_gt takes them, with the
+        same row stride (lsdgpu_frame_set_idepth_device)"""
+        if _is_tensor(idepth) or _is_tensor(var):
+            if not (_is_tensor(idepth) and _is_tensor(var)):
+                raise ValueError("set_idepth: idepth and var must both be CUDA tensors or both host arrays")
+            pa, pitch, stream = _device_image(idepth, self.device, self.w, self.h, "set_idepth", "float32")
+            pb, pitch_b, _ = _device_image(var, self.device, self.w, self.h, "set_idepth", "float32")
+            if pitch_b != pitch:
+                raise ValueError(f"set_idepth: idepth and var need the same row stride, not {idepth.stride(0)} and {var.stride(0)}")
+            self._ck(self.L.lsdgpu_frame_set_idepth_device(self.ptr, fid, pa, pb, pitch, stream))
+            return
         a = np.ascontiguousarray(idepth, np.float32)
         b = np.ascontiguousarray(var, np.float32)
         self._ck(self.L.lsdgpu_frame_set_idepth(self.ptr, fid, a.ctypes.data_as(_fp), b.ctypes.data_as(_fp)))
@@ -608,9 +659,15 @@ class Context:
         raw = np.ascontiguousarray(raw_u8, np.uint8)
         self._ck(self.L.lsdgpu_frame_upload_distorted_u8(self.ptr, fid, raw.ctypes.data_as(C.POINTER(C.c_uint8))))
 
-    def pack_pointcloud(self, kf_id: int, level: int = 0) -> np.ndarray:
-        """keyframeMsg.pointcloud of ROSOutput3DWrapper::publishKeyframe (ROSOutput3DWrapper.cpp:91-110), packed on the device"""
+    def pack_pointcloud(self, kf_id: int, level: int = 0, out=None):
+        """keyframeMsg.pointcloud of ROSOutput3DWrapper::publishKeyframe (ROSOutput3DWrapper.cpp:91-110), packed on the device.
+        out = a contiguous uint8 CUDA tensor of at least 12 bytes per record: the records are written there, ordered on its
+        current stream (lsdgpu_keyframe_pack_pointcloud_device); returns a (n, 12) view of out"""
         n = (self.w >> level) * (self.h >> level)
+        if out is not None:
+            stream = _device_out(out, "uint8", n * POINT_DENSE.itemsize, self.device, "pack_pointcloud(out=)")
+            self._ck(self.L.lsdgpu_keyframe_pack_pointcloud_device(self.ptr, kf_id, level, out.data_ptr(), out.numel(), stream))
+            return out.reshape(-1)[:n * POINT_DENSE.itemsize].view(n, POINT_DENSE.itemsize)
         out = np.zeros(n, POINT_DENSE)
         self._ck(self.L.lsdgpu_keyframe_pack_pointcloud(self.ptr, kf_id, level, out.ctypes.data_as(_vp)))
         return out
@@ -836,7 +893,18 @@ class DepthMap:
         self.last_draws = n.value
         return st
 
-    def setHypotheses(self, kf_id: int, hyp: np.ndarray, reactivated=False, do_set_depth=True):
+    def setHypotheses(self, kf_id: int, hyp, reactivated=False, do_set_depth=True):
+        """the hypotheses of keyframe kf_id: a HYP_DTYPE host array of (h, w), or a contiguous uint8 CUDA tensor of its w * h * 32
+        bytes (16-byte aligned, e.g. from current(out=...)), read on the device in order on its current stream
+        (lsdgpu_depth_set_hypotheses_device)"""
+        if _is_tensor(hyp):
+            n = self.ctx.w * self.ctx.h * HYP_DTYPE.itemsize
+            stream = _device_out(hyp, "uint8", n, self.ctx.device, "setHypotheses")
+            if hyp.numel() != n:
+                raise ValueError(f"setHypotheses: needs {n} bytes of hypotheses, not {hyp.numel()}")
+            self.ctx._ck(self.ctx.L.lsdgpu_depth_set_hypotheses_device(self.ctx.ptr, kf_id, hyp.data_ptr(), int(reactivated),
+                                                                       int(do_set_depth), stream))
+            return
         a = np.ascontiguousarray(hyp)
         assert a.dtype == HYP_DTYPE
         self.ctx._ck(self.ctx.L.lsdgpu_depth_set_hypotheses(self.ctx.ptr, kf_id, a.ctypes.data_as(C.POINTER(Hyp)),
@@ -885,7 +953,15 @@ class DepthMap:
     def propagateDepth(self, new_kf_id: int):
         self.ctx._ck(self.ctx.L.lsdgpu_depth_propagate(self.ctx.ptr, new_kf_id))
 
-    def current(self) -> np.ndarray:
+    def current(self, out=None):
+        """currentDepthMap as a HYP_DTYPE host array of (h, w), or -- out = a contiguous uint8 CUDA tensor of at least w * h * 32
+        bytes, 16-byte aligned -- written into out on the device, ordered on its current stream; returns a (h, w, 32) view of out
+        (lsdgpu_depth_download_device), whose fields hyp_fields() gives"""
+        if out is not None:
+            h, w, rec = self.ctx.h, self.ctx.w, HYP_DTYPE.itemsize
+            stream = _device_out(out, "uint8", h * w * rec, self.ctx.device, "current(out=)")
+            self.ctx._ck(self.ctx.L.lsdgpu_depth_download_device(self.ctx.ptr, out.data_ptr(), out.numel(), stream))
+            return out.reshape(-1)[:h * w * rec].view(h, w, rec)
         out = np.zeros((self.ctx.h, self.ctx.w), HYP_DTYPE)
         self.ctx._ck(self.ctx.L.lsdgpu_depth_download(self.ctx.ptr, out.ctypes.data_as(C.POINTER(Hyp))))
         return out

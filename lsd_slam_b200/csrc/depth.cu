@@ -357,16 +357,12 @@ static int runFillHoles(lsdgpu_ctx* ctx)
     return 0;
 }
 
-extern "C" int lsdgpu_depth_set_hypotheses(lsdgpu_ctx* ctx, int kf_id, const lsdgpu_hyp* aos, int reactivated, int do_set_depth)
-{ LSD_LOCK(ctx);
-    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
-    FrameSlot* kf = findSlot(ctx, kf_id);
-    if (!kf) return failMissing(ctx, kf_id, "unknown keyframe id");
+// the hypotheses of keyframe kf from a 16-byte aligned device AoS (the staging buffer or a caller's), then the optional
+// re-activation regularization and setDepth
+static int setHypotheses(lsdgpu_ctx* ctx, int kf_id, FrameSlot* kf, const lsdgpu_hyp* daos, int reactivated, int do_set_depth)
+{
     const int n = ctx->w * ctx->h;
-    LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
-    memcpy(ctx->hStageF, aos, (size_t)n * 32);
-    LSD_CHECK(ctx, cudaMemcpyAsync(ctx->dStageF, ctx->hStageF, (size_t)n * 32, cudaMemcpyHostToDevice, ctx->stream));
-    k_hyp_from_aos<<<divUp(n, 256), 256, 0, ctx->stream>>>((const lsdgpu_hyp*)ctx->dStageF, ctx->cur, n);
+    k_hyp_from_aos<<<divUp(n, 256), 256, 0, ctx->stream>>>(daos, ctx->cur, n);
     LAUNCH(ctx);
     LSD_CHECK(ctx, cudaGetLastError());
     ctx->activeKf = kf_id; ctx->activeKfReactivated = reactivated != 0;
@@ -379,6 +375,32 @@ extern "C" int lsdgpu_depth_set_hypotheses(lsdgpu_ctx* ctx, int kf_id, const lsd
     return 0;
 }
 
+extern "C" int lsdgpu_depth_set_hypotheses(lsdgpu_ctx* ctx, int kf_id, const lsdgpu_hyp* aos, int reactivated, int do_set_depth)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    FrameSlot* kf = findSlot(ctx, kf_id);
+    if (!kf) return failMissing(ctx, kf_id, "unknown keyframe id");
+    const int n = ctx->w * ctx->h;
+    LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+    memcpy(ctx->hStageF, aos, (size_t)n * 32);
+    LSD_CHECK(ctx, cudaMemcpyAsync(ctx->dStageF, ctx->hStageF, (size_t)n * 32, cudaMemcpyHostToDevice, ctx->stream));
+    return setHypotheses(ctx, kf_id, kf, (const lsdgpu_hyp*)ctx->dStageF, reactivated, do_set_depth);
+}
+
+extern "C" int lsdgpu_depth_set_hypotheses_device(lsdgpu_ctx* ctx, int kf_id, const lsdgpu_hyp* d_aos, int reactivated,
+                                                  int do_set_depth, void* stream)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    FrameSlot* kf = findSlot(ctx, kf_id);
+    if (!kf) return failMissing(ctx, kf_id, "unknown keyframe id");
+    int r = checkDevicePtr(ctx, "depth_set_hypotheses_device", "the hypotheses", d_aos, 16);
+    if (r) return r;
+    LSD_CHECK(ctx, afterCallerStream(ctx, stream));
+    if ((r = setHypotheses(ctx, kf_id, kf, d_aos, reactivated, do_set_depth))) return r;
+    LSD_CHECK(ctx, beforeCallerStream(ctx, stream));
+    return 0;
+}
+
 extern "C" int lsdgpu_depth_download(lsdgpu_ctx* ctx, lsdgpu_hyp* aos_out)
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
@@ -388,6 +410,20 @@ extern "C" int lsdgpu_depth_download(lsdgpu_ctx* ctx, lsdgpu_hyp* aos_out)
     LSD_CHECK(ctx, cudaGetLastError());
     LSD_CHECK(ctx, cudaMemcpyAsync(aos_out, ctx->dStageF, (size_t)n * 32, cudaMemcpyDeviceToHost, ctx->stream));
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+extern "C" int lsdgpu_depth_download_device(lsdgpu_ctx* ctx, lsdgpu_hyp* d_aos, size_t capacity, void* stream)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    const int n = ctx->w * ctx->h;
+    int r = checkCapacity(ctx, "depth_download_device", "the depth map", (size_t)n * sizeof(lsdgpu_hyp), capacity);
+    if (r || (r = checkDevicePtr(ctx, "depth_download_device", "the output", d_aos, 16))) return r;
+    LSD_CHECK(ctx, afterCallerStream(ctx, stream));
+    k_hyp_to_aos<<<divUp(n, 256), 256, 0, ctx->stream>>>(ctx->cur, d_aos, n);
+    LAUNCH(ctx);
+    LSD_CHECK(ctx, cudaGetLastError());
+    LSD_CHECK(ctx, beforeCallerStream(ctx, stream));
     return 0;
 }
 

@@ -1064,26 +1064,28 @@ __global__ void __launch_bounds__(256) k_init_from_gt(HypField cur, const float*
     cur.hi[i] = hi;
 }
 
-// AoS (reference layout) <-> the two 16-byte planes
+// AoS (reference layout) <-> the two 16-byte planes.  aos is 16-byte aligned (the staging buffer, or a caller's buffer checked by
+// lsdgpu_depth_set_hypotheses_device / lsdgpu_depth_download_device), so a 32-byte record moves as two 128-bit accesses: the
+// words {isValid + pad, blacklisted, nextStereoFrameMinID, validity_counter}, then the four idepth floats.
 __global__ void __launch_bounds__(256) k_hyp_from_aos(const lsdgpu_hyp* __restrict__ aos, HypField f, int n)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    lsdgpu_hyp h = aos[i];
-    f.hf[i] = make_float4(h.idepth, h.idepth_var, h.idepth_smoothed, h.idepth_var_smoothed);
-    f.hi[i] = make_int4(h.isValid ? 1 : 0, h.blacklisted, h.validity_counter, __float_as_int(h.nextStereoFrameMinID));
+    const int4* rec = reinterpret_cast<const int4*>(aos + i);
+    const int4 a = __ldg(rec);
+    const float4 b = __ldg(reinterpret_cast<const float4*>(rec + 1));
+    f.hf[i] = b;
+    f.hi[i] = make_int4((a.x & 0xff) ? 1 : 0, a.y, a.w, a.z);     // isValid is the low byte of word 0 (little endian)
 }
 __global__ void __launch_bounds__(256) k_hyp_to_aos(HypField f, lsdgpu_hyp* __restrict__ aos, int n)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    float4 a = f.hf[i];
-    int4 b = f.hi[i];
-    lsdgpu_hyp h;
-    h.isValid = b.x ? 1 : 0; h._pad[0] = h._pad[1] = h._pad[2] = 0;
-    h.blacklisted = b.y; h.nextStereoFrameMinID = __int_as_float(b.w); h.validity_counter = b.z;
-    h.idepth = a.x; h.idepth_var = a.y; h.idepth_smoothed = a.z; h.idepth_var_smoothed = a.w;
-    aos[i] = h;
+    const float4 a = f.hf[i];
+    const int4 b = f.hi[i];
+    int4* rec = reinterpret_cast<int4*>(aos + i);
+    rec[0] = make_int4(b.x ? 1 : 0, b.y, b.w, b.z);              // isValid as 0 / 1 with its three pad bytes 0
+    *reinterpret_cast<float4*>(rec + 1) = a;
 }
 
 // validityIntegralBuffer on demand (parity hook only; the hot path never builds it), DepthMap.cpp:722-754

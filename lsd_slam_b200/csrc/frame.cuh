@@ -207,15 +207,16 @@ __global__ void __launch_bounds__(256) k_gradients(const __grid_constant__ GradP
     p.maxgrad0[i] = r;
 }
 
-// Frame::setDepthFromGroundTruth, Frame.cpp:264-285
-__global__ void __launch_bounds__(256) k_set_depth_gt(const float* __restrict__ depth, const float* __restrict__ maxgrad,
+// Frame::setDepthFromGroundTruth, Frame.cpp:264-285.  `stride` is the row stride of depth in floats: w for the library's own
+// staging copy, any value >= w for a caller's device plane (lsdgpu_frame_set_depth_gt_device).
+__global__ void __launch_bounds__(256) k_set_depth_gt(const float* __restrict__ depth, int stride, const float* __restrict__ maxgrad,
                                                       float* __restrict__ idepth, float* __restrict__ idepthVar,
                                                       int w, int h, float minUseGrad, float cov_scale)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= w * h) return;
     const int x = i % w, y = i / w;
-    const float d = depth[i];
+    const float d = depth[y * stride + x];
     if (x > 0 && x < w - 1 && y > 0 && y < h - 1 && maxgrad[i] >= minUseGrad && !isnan(d) && d > 0) {
         idepth[i] = 1.0f / d;
         idepthVar[i] = 0.01f * 0.01f * cov_scale;     // VAR_GT_INIT_INITIAL * cov_scale

@@ -371,12 +371,7 @@ extern "C" int lsdgpu_frame_download_device(lsdgpu_ctx* ctx, int frame_id, int w
     size_t bytes;
     const void* src;
     int r = downloadPlane(ctx, frame_id, what, level, &s, &bytes);
-    if (r) return r;
-    if (capacity < bytes) {
-        char msg[160];
-        snprintf(msg, sizeof(msg), "frame_download_device: the plane has %zu bytes, the output holds %zu", bytes, capacity);
-        return lsd_fail(ctx, msg);
-    }
+    if (r || (r = checkCapacity(ctx, "frame_download_device", "the plane", bytes, capacity))) return r;
     if ((r = checkDevicePtr(ctx, "frame_download_device", "the output", d_out,
                             what == LSDGPU_BUF_GRADIENTS ? 16 : what == LSDGPU_BUF_GOODMASK ? 1 : 4)))
         return r;
@@ -385,6 +380,17 @@ extern "C" int lsdgpu_frame_download_device(lsdgpu_ctx* ctx, int frame_id, int w
     if (src) LSD_CHECK(ctx, cudaMemcpyAsync(d_out, src, bytes, cudaMemcpyDeviceToDevice, ctx->stream));
     else LSD_CHECK(ctx, cudaMemsetAsync(d_out, 1, bytes, ctx->stream));
     LSD_CHECK(ctx, beforeCallerStream(ctx, stream));
+    return 0;
+}
+
+// Frame::setDepthFromGroundTruth from a device plane of metric depth, `stride` floats per row
+static int setDepthGT(lsdgpu_ctx* ctx, FrameSlot* s, const float* ddepth, int stride, float cov_scale)
+{
+    k_set_depth_gt<<<divUp(ctx->w * ctx->h, 256), 256, 0, ctx->stream>>>(ddepth, stride, s->maxgrad, s->idepth[0], s->idepthVar[0],
+                                                                         ctx->w, ctx->h, ctx->g.minUseGrad, cov_scale);
+    LAUNCH(ctx);
+    LSD_CHECK(ctx, cudaGetLastError());
+    s->hasDepth = true; s->idepthPyrValid = false;
     return 0;
 }
 
@@ -397,11 +403,20 @@ extern "C" int lsdgpu_frame_set_depth_gt(lsdgpu_ctx* ctx, int frame_id, const fl
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
     memcpy(ctx->hStageF, depth, (size_t)n * 4);
     LSD_CHECK(ctx, cudaMemcpyAsync(ctx->dStageF, ctx->hStageF, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
-    k_set_depth_gt<<<divUp(n, 256), 256, 0, ctx->stream>>>(ctx->dStageF, s->maxgrad, s->idepth[0], s->idepthVar[0], ctx->w, ctx->h,
-                                                           ctx->g.minUseGrad, cov_scale);
-    LAUNCH(ctx);
-    LSD_CHECK(ctx, cudaGetLastError());
-    s->hasDepth = true; s->idepthPyrValid = false;
+    return setDepthGT(ctx, s, ctx->dStageF, ctx->w, cov_scale);
+}
+
+extern "C" int lsdgpu_frame_set_depth_gt_device(lsdgpu_ctx* ctx, int frame_id, const float* d_depth, size_t pitch, float cov_scale,
+                                                void* stream)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    FrameSlot* s = findSlot(ctx, frame_id);
+    if (!s) return failMissing(ctx, frame_id, "unknown frame id");
+    int r = checkDevicePlaneF32(ctx, "frame_set_depth_gt_device", "the depth", d_depth, pitch);
+    if (r) return r;
+    LSD_CHECK(ctx, afterCallerStream(ctx, stream));
+    if ((r = setDepthGT(ctx, s, d_depth, (int)(pitch / 4), cov_scale))) return r;
+    LSD_CHECK(ctx, beforeCallerStream(ctx, stream));
     return 0;
 }
 
@@ -416,6 +431,23 @@ extern "C" int lsdgpu_frame_set_idepth(lsdgpu_ctx* ctx, int frame_id, const floa
     memcpy(ctx->hStageF + n, idepthVar, n * 4);
     LSD_CHECK(ctx, cudaMemcpyAsync(s->idepth[0], ctx->hStageF, n * 4, cudaMemcpyHostToDevice, ctx->stream));
     LSD_CHECK(ctx, cudaMemcpyAsync(s->idepthVar[0], ctx->hStageF + n, n * 4, cudaMemcpyHostToDevice, ctx->stream));
+    s->hasDepth = true; s->idepthPyrValid = false;
+    return 0;
+}
+
+extern "C" int lsdgpu_frame_set_idepth_device(lsdgpu_ctx* ctx, int frame_id, const float* d_idepth, const float* d_idepthVar,
+                                              size_t pitch, void* stream)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    FrameSlot* s = findSlot(ctx, frame_id);
+    if (!s) return failMissing(ctx, frame_id, "unknown frame id");
+    int r = checkDevicePlaneF32(ctx, "frame_set_idepth_device", "the idepth", d_idepth, pitch);
+    if (r || (r = checkDevicePlaneF32(ctx, "frame_set_idepth_device", "the idepthVar", d_idepthVar, pitch))) return r;
+    const size_t row = (size_t)ctx->w * 4;
+    LSD_CHECK(ctx, afterCallerStream(ctx, stream));
+    LSD_CHECK(ctx, cudaMemcpy2DAsync(s->idepth[0], row, d_idepth, pitch, row, ctx->h, cudaMemcpyDefault, ctx->stream));
+    LSD_CHECK(ctx, cudaMemcpy2DAsync(s->idepthVar[0], row, d_idepthVar, pitch, row, ctx->h, cudaMemcpyDefault, ctx->stream));
+    LSD_CHECK(ctx, beforeCallerStream(ctx, stream));
     s->hasDepth = true; s->idepthPyrValid = false;
     return 0;
 }

@@ -348,6 +348,26 @@ static inline int checkDeviceImage(lsdgpu_ctx* ctx, const char* fn, const uint8_
     }
     return checkDevicePtr(ctx, fn, "the image", p, 1);
 }
+// a caller's device plane of the context's w x h floats with row pitch `pitch` bytes: whole floats, at least w of them (the kernels
+// index it in floats with int arithmetic)
+static inline int checkDevicePlaneF32(lsdgpu_ctx* ctx, const char* fn, const char* what, const float* p, size_t pitch)
+{
+    char msg[256];
+    if (pitch % 4 || pitch < (size_t)ctx->w * 4 || pitch / 4 > (size_t)INT32_MAX / (size_t)ctx->h) {
+        snprintf(msg, sizeof(msg), "%s: row pitch %zu bytes for %s of %d floats per row (%d rows): needs a multiple of 4 >= %d",
+                 fn, pitch, what, ctx->w, ctx->h, ctx->w * 4);
+        return lsd_fail(ctx, msg);
+    }
+    return checkDevicePtr(ctx, fn, what, p, 4);
+}
+// 0 if a caller's output of `capacity` bytes holds the `need` bytes of `what`
+static inline int checkCapacity(lsdgpu_ctx* ctx, const char* fn, const char* what, size_t need, size_t capacity)
+{
+    if (capacity >= need) return 0;
+    char msg[192];
+    snprintf(msg, sizeof(msg), "%s: %s has %zu bytes, the output holds %zu", fn, what, need, capacity);
+    return lsd_fail(ctx, msg);
+}
 
 static inline int divUp(int a, int b) { return (a + b - 1) / b; }
 static inline size_t alignUp(size_t v, size_t a) { return (v + a - 1) / a * a; }

@@ -10,21 +10,53 @@
 // ------------------------------------------------------------------------------------------------------
 // keyframe output formats (SURVEY 8f row 4)
 // ------------------------------------------------------------------------------------------------------
-extern "C" int lsdgpu_keyframe_pack_pointcloud(lsdgpu_ctx* ctx, int kf_id, int publish_level, lsdgpu_input_point_dense* out)
-{ LSD_LOCK(ctx);
-    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+// The request of lsdgpu_keyframe_pack_pointcloud and its device twin: checks the keyframe and level, returns the record count
+static int packRequest(lsdgpu_ctx* ctx, int kf_id, int publish_level, FrameSlot** slot, int* n)
+{
     FrameSlot* kf = findSlot(ctx, kf_id);
     if (!kf) return failMissing(ctx, kf_id, "unknown keyframe id");
     if (publish_level < 0 || publish_level >= LSD_LEVELS) return lsd_fail(ctx, "bad level");
+    if (!kf->hasDepth) return lsd_fail(ctx, "keyframe has no depth");
+    *slot = kf;
+    *n = (ctx->w >> publish_level) * (ctx->h >> publish_level);
+    return 0;
+}
+// the packing kernel of an accepted request, writing into `out` (the staging buffer or a caller's)
+static int packPointcloud(lsdgpu_ctx* ctx, FrameSlot* kf, int publish_level, int n, uint32_t* out)
+{
     int r = ensureIdepthPyramid(ctx, kf);                      // f->idepth(publishLvl), ROSOutput3DWrapper.cpp:96-97
     if (r) return r;
-    const int n = (ctx->w >> publish_level) * (ctx->h >> publish_level);
     k_pack_pointcloud<<<divUp(3 * n, 256), 256, 0, ctx->stream>>>(kf->idepth[publish_level], kf->idepthVar[publish_level],
-                                                                  kf->image[publish_level], n, ctx->dPacked);
+                                                                  kf->image[publish_level], n, out);
     LAUNCH(ctx);
     LSD_CHECK(ctx, cudaGetLastError());
+    return 0;
+}
+
+extern "C" int lsdgpu_keyframe_pack_pointcloud(lsdgpu_ctx* ctx, int kf_id, int publish_level, lsdgpu_input_point_dense* out)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    FrameSlot* kf;
+    int n;
+    int r = packRequest(ctx, kf_id, publish_level, &kf, &n);
+    if (r || (r = packPointcloud(ctx, kf, publish_level, n, ctx->dPacked))) return r;
     LSD_CHECK(ctx, cudaMemcpyAsync(out, ctx->dPacked, (size_t)n * 12, cudaMemcpyDeviceToHost, ctx->stream));
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+extern "C" int lsdgpu_keyframe_pack_pointcloud_device(lsdgpu_ctx* ctx, int kf_id, int publish_level, lsdgpu_input_point_dense* d_out,
+                                                      size_t capacity, void* stream)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    FrameSlot* kf;
+    int n;
+    int r = packRequest(ctx, kf_id, publish_level, &kf, &n);
+    if (r || (r = checkCapacity(ctx, "keyframe_pack_pointcloud_device", "the point cloud", (size_t)n * 12, capacity))) return r;
+    if ((r = checkDevicePtr(ctx, "keyframe_pack_pointcloud_device", "the output", d_out, 4))) return r;
+    LSD_CHECK(ctx, afterCallerStream(ctx, stream));
+    if ((r = packPointcloud(ctx, kf, publish_level, n, (uint32_t*)d_out))) return r;
+    LSD_CHECK(ctx, beforeCallerStream(ctx, stream));
     return 0;
 }
 

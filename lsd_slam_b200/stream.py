@@ -85,8 +85,10 @@ class GpuStream:
         self._res = abi.TrackResult()
         self._qts = np.zeros(8, np.float64)
 
-    def init_gt(self, fid: int, image_u8: np.ndarray, depth: np.ndarray):
-        """SlamSystem::gtDepthInit, SlamSystem.cpp:831-854"""
+    def init_gt(self, fid: int, image_u8, depth):
+        """SlamSystem::gtDepthInit, SlamSystem.cpp:831-854.  image_u8 and depth may be host arrays or CUDA tensors (uint8 and
+        float32, (h, w), contiguous rows): from tensors the map starts without a host copy or a host wait, ordered on the current
+        stream."""
         self.ctx.upload(fid, image_u8)
         self.ctx.set_depth_gt(fid, depth)
         self.map.initializeFromGTDepth(fid)
