@@ -406,7 +406,8 @@ int lsdgpu_sim3_track_batch(lsdgpu_ctx* ctx, int n, const int* ref_kf_ids, const
                             int start_level, int final_level, const lsdgpu_track_settings* s, lsdgpu_sim3_result* results);
 
 /* ---- permaRef tracking, batched (SURVEY 8f row 2) ------------------------------------------------------------
- * Frame::setPermaRef Frame.cpp:149-174: freeze the keyframe's CURRENT level-4 point cloud (positions, colour, variance). */
+ * Frame::setPermaRef Frame.cpp:149-174: freeze the keyframe's CURRENT level-4 point cloud (positions, colour, variance).  A keyframe
+ * without points gets a permaRef of 0 points: its overlap is 0/0 and its tracking diverges, as in the reference. */
 int lsdgpu_frame_set_perma_ref(lsdgpu_ctx* ctx, int kf_id, int* num_points_out);
 /* SE3Tracker::checkPermaRefOverlap SE3Tracker.cpp:121-157 for n candidates in one launch:
  * usage_out[i] = pointUsage of keyframe kf_ids[i] under referenceToFrame refToFrame_qt[7*i..] */

@@ -34,6 +34,7 @@ extern "C" int lsdgpu_frame_set_perma_ref(lsdgpu_ctx* ctx, int kf_id, int* num_p
             pv.push_back(var[idx]);
         }
     kf->permaNumPts = (int)pc.size();
+    kf->permaSet = true;
     if (kf->permaNumPts) {
         LSD_CHECK(ctx, cudaMemcpyAsync(kf->permaPC, pc.data(), pc.size() * 16, cudaMemcpyHostToDevice, ctx->stream));
         LSD_CHECK(ctx, cudaMemcpyAsync(kf->permaVar, pv.data(), pv.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
@@ -50,7 +51,8 @@ static int fillPermaItems(lsdgpu_ctx* ctx, int n, const int* kf_ids, const doubl
     for (int i = 0; i < n; i++) {
         FrameSlot* kf = findFrame(ctx, kf_ids[i]);           // a minimized keyframe's permaRef is read from its record
         if (!kf) return lsd_fail(ctx, "unknown keyframe id");
-        if (kf->permaNumPts <= 0) return lsd_fail(ctx, "keyframe has no permaRef (call lsdgpu_frame_set_perma_ref)");
+        // a permaRef of 0 points is a result, as in the reference: overlap 0/0, tracking diverged (:121-157, :162-185)
+        if (!kf->permaSet) return lsd_fail(ctx, "keyframe has no permaRef (call lsdgpu_frame_set_perma_ref)");
         lsd::SE3<double> T;
         for (int k = 0; k < 4; k++) T.q[k] = qt[7 * i + k];
         for (int k = 0; k < 3; k++) T.t[k] = qt[7 * i + 4 + k];

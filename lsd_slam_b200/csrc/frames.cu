@@ -24,7 +24,7 @@ static FrameSlot* acquireSlot(lsdgpu_ctx* ctx, int id)
             fresh.thisToParent[3] = 1; fresh.thisToParent[7] = 1;
             fresh.parentId = -1; fresh.initialTrackedResidual = 0;
             fresh.numFramesTrackedOnThis = fresh.numMappedOnThis = 0;
-            fresh.permaNumPts = 0;
+            fresh.permaNumPts = 0; fresh.permaSet = false;
             fresh.reactAllocated = false; fresh.reactValid = false;
             c = fresh;
             return &c;

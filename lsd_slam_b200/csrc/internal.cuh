@@ -46,6 +46,7 @@ struct FrameSlot {
     float4* permaPC = nullptr;           // permaRef: (x, y, z, colour) per level-4 point (Frame::setPermaRef)
     float* permaVar = nullptr;
     int permaNumPts = 0;
+    bool permaSet = false;               // setPermaRef ran (a keyframe without points has a permaRef of 0 points)
     float* reactIdepth = nullptr;        // Frame::idepth_reAct / idepthVar_reAct / validity_reAct (Frame.cpp:107-145), device-resident
     float* reactVar = nullptr;
     uint8_t* reactValidity = nullptr;

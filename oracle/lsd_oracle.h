@@ -276,6 +276,11 @@ enum {
     LSDO_BR_CREATE_BLACKLIST,   /* observeDepthCreate: blacklisted-- on -3 or -2, :269-273 */
     LSDO_BR_PROP_MASK,          /* propagateDepth: source dropped by the tracking mask, :550-555 */
     LSDO_BR_PROP_COLOR,         /* propagateDepth without a mask: source dropped by the colour difference, :559-569 */
+    LSDO_BR_REG_OCCLUSION,      /* regularizeDepthMapRow<true>: invalidated by numOccluding > numNotOccluding, :826-834 */
+    LSDO_BR_REG_VALIDITY,       /* regularizeDepthMapRow: dropped by val_sum < validityTH, :815-823 */
+    LSDO_BR_FILL_CREATE,        /* regularizeDepthMapFillHolesRow: hypothesis created, :690-700 */
+    LSDO_BR_EPL_REJECT_GRAD,    /* makeAndCheckEPL: gradient along the epipolar line below MIN_EPL_GRAD_SQUARED, :213-217 */
+    LSDO_BR_EPL_REJECT_ANGLE,   /* makeAndCheckEPL: angle to the epipolar line above MIN_EPL_ANGLE_SQUARED, :221-225 */
     LSDO_BR_COUNT
 };
 void lsdo_depth_branch_counts(int64_t out[LSDO_BR_COUNT]);

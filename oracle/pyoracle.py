@@ -235,7 +235,8 @@ BRANCHES = ("depth_x", "depth_y", "firstx_gate", "rescale_gate", "near_clamp", "
             "clip_left", "clip_right", "clip_top", "clip_bottom", "subpixel_pre", "subpixel_post", "subpixel_none",
             "prop_skip", "prop_invalidate", "prop_merge", "prop_merge_cap",
             "stereo_err_search", "stereo_err_interp", "stereo_unclear", "stereo_negative",
-            "update_fail_invalidate", "update_inconsistent", "create_blacklist", "prop_mask", "prop_color")
+            "update_fail_invalidate", "update_inconsistent", "create_blacklist", "prop_mask", "prop_color",
+            "reg_occlusion", "reg_validity", "fill_create", "epl_reject_grad", "epl_reject_angle")
 
 
 def branch_counts(fast=False) -> dict:

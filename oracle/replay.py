@@ -62,6 +62,38 @@ def map_report(a, b):
     return rep
 
 
+def oracle_keyframe(seq, snap: Snapshot):
+    """the oracle's keyframe and depth map in the device's pre-step state of `snap` (C restatement, current settings)"""
+    L = po.lib(False)
+    hyp_c = np.ascontiguousarray(snap.hyp)
+    kf = po.Frame(snap.kf_id, snap.kf_image, seq.K, fast=False)
+    kf.setDepthFromGroundTruth(np.ones((seq.h, seq.w), np.float32))    # only to attach the frame as the active keyframe
+    dm = po.DepthMap(seq.w, seq.h, seq.K, fast=False)
+    dm.initializeFromGTDepth(kf)
+    dm.set_current(snap.hyp)
+    L.lsdo_frame_setDepth(kf.ptr, hyp_c.ctypes.data_as(po.C.POINTER(po.Hyp)))   # Frame::setDepth(currentDepthMap), DepthMap.cpp:1153 / 1311
+    L.lsdo_frame_set_counters(kf.ptr, int(snap.counters[0]), int(snap.counters[1]))
+    L.lsdo_frame_set_depthHasBeenUpdatedFlag(kf.ptr, 0)
+    return kf, dm
+
+
+def start_outcomes(seq, snap: Snapshot, fid: int, image_u8, n=20, eps=1e-6, seed=0):
+    """the oracle's trackFrame of the step of `snap` from its start pose with the translation moved by eps (relative) in n seeded
+    directions (a start near the identity by eps * 1e-2 absolute) -> list of (pose, numCalcResidualCalls, numCalcWarpUpdateCalls).  Where the tracking cost has several minima
+    close together (a texture that repeats along the motion), starts closer than the fp32 resolution of a pose can end in
+    different minima: these are the outcomes the reference arithmetic itself reaches from the step's state"""
+    rng = np.random.default_rng(seed)
+    outs = []
+    for _ in range(n):
+        q = np.array(snap.last_pose, np.float64)
+        d = rng.normal(size=3)
+        q[4:7] += d / np.linalg.norm(d) * eps * max(np.linalg.norm(q[4:7]), 1e-2)       # an identity start moves by 1e-2 eps
+        kf, _dm = oracle_keyframe(seq, snap)
+        r = po.se3_track(kf, po.Frame(fid, image_u8, seq.K, fast=False), q, po.default_track_settings(False))
+        outs.append((np.array(r.frameToRef_qt, np.float64), list(r.numCalcResidualCalls), list(r.numCalcWarpUpdateCalls)))
+    return outs
+
+
 def replay_step(seq, snap: Snapshot, fid: int, image_u8, gs, settings=None, globals_kw=None):
     """Replay on the oracle the step GpuStream `gs` has JUST executed for frame `fid` from state `snap`, under the run-time settings
     of util/settings.cpp:80-88 the context holds (or `globals_kw` instead, e.g. to show that other values give another result).
@@ -73,19 +105,9 @@ def replay_step(seq, snap: Snapshot, fid: int, image_u8, gs, settings=None, glob
     po.set_globals(fl, **g)
     L = po.lib(fl)
     st = settings or po.default_track_settings(fl)
-    # keyframe + depth map in the device's pre-step state
-    hyp_c = np.ascontiguousarray(snap.hyp)
 
     def make_kf():
-        kf = po.Frame(snap.kf_id, snap.kf_image, seq.K, fast=fl)
-        kf.setDepthFromGroundTruth(np.ones((seq.h, seq.w), np.float32))    # only to attach the frame as the active keyframe
-        dm = po.DepthMap(seq.w, seq.h, seq.K, fast=fl)
-        dm.initializeFromGTDepth(kf)
-        dm.set_current(snap.hyp)
-        L.lsdo_frame_setDepth(kf.ptr, hyp_c.ctypes.data_as(po.C.POINTER(po.Hyp)))   # Frame::setDepth(currentDepthMap), DepthMap.cpp:1153 / 1311
-        L.lsdo_frame_set_counters(kf.ptr, int(snap.counters[0]), int(snap.counters[1]))
-        L.lsdo_frame_set_depthHasBeenUpdatedFlag(kf.ptr, 0)
-        return kf, dm
+        return oracle_keyframe(seq, snap)
 
     # the reference's OWN summation noise on this step: the same tracking with every sum accumulated exactly (diagnostic twin of
     # the oracle, lsdo_globals.exactTrackingSums) -- what the sequential fp32 sums of SE3Tracker.cpp approximate
@@ -104,6 +126,7 @@ def replay_step(seq, snap: Snapshot, fid: int, image_u8, gs, settings=None, glob
     out["pose_rel"], out["rot_rad"] = pose_err(pose_g, pose_o)
     out["ref_noise_rel"], out["ref_noise_rot"] = pose_err(pose_o, pose_x)      # reference (fp32 sequential sums) vs exact sums
     out["pose_rel_exact"], _ = pose_err(pose_g, pose_x)                        # device vs exact sums
+    out["pose"], out["residual_calls"] = pose_g, list(res.numCalcResidualCalls)
     out["counts_equal"] = (list(res.numCalcResidualCalls) == list(r.numCalcResidualCalls)
                            and list(res.numCalcWarpUpdateCalls) == list(r.numCalcWarpUpdateCalls))
     out["stats"] = {"lastResidual": (res.lastResidual, r.lastResidual), "pointUsage": (res.pointUsage, r.pointUsage),
@@ -162,11 +185,12 @@ def finish_replay(seq, snap: Snapshot, out, gs, mask_before_clear=None, rescale_
 
 
 def run_with_replay(seq, frames, n_frames, kf_every=20, sample=None, mode=1, device=0, max_frames=8, globals_kw=None,
-                    before_step=None):
+                    before_step=None, keep_snapshots=False):
     """GpuStream over frames 1..n_frames-1 with the oracle replaying the steps in `sample` (None = every step).
     Returns the list of per-step reports.  The stream itself never sees the oracle (it continues from ITS OWN state).
     globals_kw: the context's run-time settings (default: the reference's); before_step(k, ctx) runs before step k, e.g. to change
-    them between two frames as a dynamic-reconfigure callback does.  The oracle is back at the default settings afterwards."""
+    them between two frames as a dynamic-reconfigure callback does.  keep_snapshots: each report also holds its step's state
+    ("snap") and image ("image"), for start_outcomes.  The oracle is back at the default settings afterwards."""
     from lsd_slam_b200 import abi
     from lsd_slam_b200.stream import GpuStream
     images = {k: frames[k][0] for k in range(n_frames)}
@@ -195,6 +219,8 @@ def run_with_replay(seq, frames, n_frames, kf_every=20, sample=None, mode=1, dev
             ctx.clear_good_mask = orig_clear
         out = replay_step(seq, snap, k, frames[k][0], gs)
         out = finish_replay(seq, snap, out, gs, mask_before_clear=mask_holder.get("mask"))
+        if keep_snapshots:
+            out["snap"], out["image"] = snap, frames[k][0]
         reports.append(out)
     ctx.close()
     po.set_globals(False)

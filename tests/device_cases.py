@@ -530,10 +530,12 @@ def _sum_noise(oracle, ref, fr, init, lo, hi, *results):
     return tw, [max(sim3_err(r.frameToRef_qts, tw.frameToRef_qts)) for r in results]
 
 
-def mapped_sim3_track(run, oracle, sum_noise=False):
+def mapped_sim3_track(run, oracle, sum_noise=False, lm_flips=()):
     """trackFrameSim3 per ordered pair over levels 4..1 and 3..2 (lastDepthResidual of pin_cases.POSE_SENSITIVE_DEPTH_RESIDUAL
     against the exact-sum twin to the reference tolerance).  sum_noise: the pose may also differ from each oracle result by
-    that result's own distance to the all-sums-exact twin, which holds the device to POSE_TOL"""
+    that result's own distance to the all-sums-exact twin, which holds the device to POSE_TOL.  lm_flips (with sum_noise): the
+    (motion, reference keyframe, frame keyframe, startLevel, finalLevel) calls where the reference arithmetic takes another LM
+    decision than its all-sums-exact twin; there the device is held to the twin alone"""
     trk = abi.Sim3Tracker(run.ctx)
     n_converged = 0
     for ref, fr in run.pairs():
@@ -545,6 +547,11 @@ def mapped_sim3_track(run, oracle, sum_noise=False):
             if sum_noise:
                 tw, noise = _sum_noise(oracle, run.of[ref], run.of[fr], init, lo, hi, want, exact)
                 check_sim3_track(trk.last, tw)
+                if (run.motion, ref, fr, lo, hi) in lm_flips:
+                    assert list(want.numCalcResidualCalls) != list(tw.numCalcResidualCalls)
+                    assert np.array_equal(est, np.array(trk.last.frameToRef_qts))
+                    n_converged += not want.diverged
+                    continue
             check_sim3_track(trk.last, want, pose_noise=noise[0])
             sensitive = (run.motion, ref, fr, lo, hi) in POSE_SENSITIVE_DEPTH_RESIDUAL
             check_sim3_track(trk.last, exact, res_tol=5e-4, depth_res_tol=2e-2 if sensitive else None, pose_noise=noise[1])

@@ -6,7 +6,8 @@ tests/test_ref_pin.py runs the cases at the reference's default run-time setting
 tests/test_ref_pin_globals.py under the settings of SETS, tests/test_ref_pin_motions.py under the camera motions of
 tests/motions.py (with two more cases only those reach), tests/test_ref_pin_sim3.py runs the Sim3 tracker and the permaRef
 path on keyframes the mapper finished, under every motion, tests/test_ref_pin_photometry.py runs cases under the exposure
-schedules of tests/photometry.py, tests/test_ref_pin_cameras.py the cases that read K through the cameras of tests/cameras.py;
+schedules of tests/photometry.py, tests/test_ref_pin_cameras.py the cases that read K through the cameras of tests/cameras.py,
+tests/test_ref_pin_scenes.py the depth-map, tracker and cloud cases on the scenes of tests/scenes.py;
 tests/golden/make_golden*.py record each of them."""
 import contextlib
 import ctypes as C
@@ -16,7 +17,7 @@ import os
 import numpy as np
 
 from oracle import pyoracle as po
-from tests import cameras, motions, photometry
+from tests import cameras, motions, photometry, scenes
 from tests.util import IDENT, pose_err
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -1044,4 +1045,128 @@ def record_cameras():
     out = {}
     for cam, c in CAMERA_PAIRS:
         out.update(run_under_camera(cam, c, None).rec)
+    return out
+
+
+# ---- scenes other than the smooth height field (tests/scenes.py) -------------------------------------------------------------
+GOLD_SCENES = os.path.join(GOLDEN, "ref_pin_scenes_320x240.npz")
+
+EMPTY_SIM3_KF = 6               # the textured keyframe empty_keyframe pairs the blank one with in the Sim3 tracker
+EMPTY_RAND_DRAWS = 16           # rand() values drawn after initializeRandomly: the state the call leaves
+
+
+def propagate_from_gt(pin, fl, seq, frames):
+    """propagateDepth of the ground-truth map to frame PROPAGATION_FRAME, without and with a tracking mask: on a scene with a
+    near object its sources land behind and in front of each other (DepthMap.cpp:588-601) and uncover background whose colour
+    disagrees (:559-569)"""
+    propagation_exposure(pin, fl, seq, frames)
+
+
+def _bits_equal(pin, what, x, n_pose=0):
+    """x against the record bit for bit, NaN payloads included; a leading pose of n_pose doubles to 1e-12 (_same_pose)"""
+    x = np.ascontiguousarray(x, np.float64)
+    y = np.asarray(pin.value(what, x), np.float64)
+    assert x.shape == y.shape and np.allclose(x[:n_pose], y[:n_pose], rtol=0, atol=1e-12), (what, x[:n_pose], y[:n_pose])
+    assert np.array_equal(x[n_pose:].view(np.uint64), y[n_pose:].view(np.uint64)), (what, x, y)
+
+
+def empty_keyframe(pin, fl, seq, frames):
+    """a keyframe with (almost) no texture: initializeRandomly (the map it leaves and the rand() values after it), updateKeyframe,
+    fill-holes and both regularisers on that map; SE3 evaluation and trackFrame, makePointCloud, setPermaRef and
+    trackFrameOnPermaref, Sim3 evaluation and trackFrameSim3 against a textured ground-truth keyframe of the default scene, on
+    ground-truth depth.  Every value bit for bit, NaN included: an empty sum is 0 and a mean over no point 0/0 in the reference"""
+    s = Side(seq, frames, fl, "random")
+    rnd = np.array([C.CDLL(None).rand() for _ in range(EMPTY_RAND_DRAWS)], np.int64)
+    pin.exact("rand_after", rnd)
+    pin.value("selected", np.int64(pin.hyp("initializeRandomly", s.dm.current())))
+    for k in (2, 3):
+        s.add_frame(k, _gt_qts(seq, k))
+    s.dm.updateKeyframe([s.fr[2], s.fr[3]])
+    pin.hyp("updateKeyframe", s.dm.current())
+    s.dm.regularizeFillHoles()
+    pin.hyp("fillHoles", s.dm.current())
+    for occl in (False, True):
+        s.dm.regularize(occl, 24)
+        pin.hyp(f"regularize<{str(occl).lower()}>", s.dm.current())
+
+    set_globals(fl)
+    kf = po.Frame(0, frames[0][0], seq.K, fast=fl)
+    kf.setDepthFromGroundTruth(frames[0][1])
+    f = po.Frame(3, frames[3][0], seq.K, fast=fl)
+    inv = np.zeros(7)
+    g = np.ascontiguousarray(seq.frame_to_ref_qt(3), np.float64)
+    po.lib(False).lsdo_se3d_inverse(g.ctypes.data_as(C.POINTER(C.c_double)), inv.ctypes.data_as(C.POINTER(C.c_double)))
+    names = ("warpedSize", "goodCount", "badCount", "pointUsage", "meanUnweightedRes", "meanWeightedRes", "lsError", "meanRes",
+             "affine_a_lastIt", "affine_b_lastIt")
+    for lvl in (4, 3, 2, 1):
+        r = po.se3_eval(kf, f, lvl, inv.astype(np.float32), 1.0, 0.0, po.default_track_settings(fl), write_mask=(lvl == 1))
+        _bits_equal(pin, f"se3_eval/L{lvl}", [getattr(r, n) for n in names] + list(r.A) + list(r.b))
+    pin.exact("se3_eval/mask", f.refPixelWasGood(create=False) != 0)
+    r = po.se3_track(kf, po.Frame(3, frames[3][0], seq.K, fast=fl), IDENT, po.default_track_settings(fl))
+    x = list(r.frameToRef_qt) + [r.lastResidual, r.pointUsage, r.lastGoodCount, r.lastBadCount, r.lastMeanRes,
+                                 r.affineEstimation_a, r.affineEstimation_b, r.diverged, r.trackingWasGood]
+    if not r.diverged:                  # a diverged trackFrame returns before it writes the frame's value (SE3Tracker.cpp:326, :482)
+        x.append(r.initialTrackedResidual)
+    _bits_equal(pin, "se3_track", x, 7)
+    for lvl in (1, 2, 3, 4):
+        pin.value(f"point_cloud/L{lvl}", np.int64(len(kf.point_cloud(lvl)[0])))
+
+    pr = po.PermaRef(kf)
+    pin.value("perma/n", np.int64(pr.n))
+    fp = po.Frame(PERMA_FRAME, frames[PERMA_FRAME][0], seq.K, fast=fl)
+    gt = _qts_op("lsdo_se3d_inverse", 7, seq.frame_to_ref_qt(PERMA_FRAME))
+    _bits_equal(pin, "perma/overlap", [pr.overlap(gt)])
+    for name, init in (("gt", gt), ("identity", IDENT)):
+        _bits_equal(pin, f"perma/track_{name}", perma_track_fields(pr.track(fp, init)), 7)
+
+    from lsd_slam_b200 import synth
+    other = synth.Sequence(seq.w, seq.h, seed=motions.SEED)
+    img6, d6 = other.render(EMPTY_SIM3_KF)
+    tex = po.Frame(EMPTY_SIM3_KF, img6, seq.K, fast=fl)
+    tex.setDepthFromGroundTruth(d6)
+    fr_to_ref = np.concatenate([seq.frame_to_ref_qt(EMPTY_SIM3_KF), [1.0]])
+    fr_to_ref[4:7] += SIM3_DT
+    fr_to_ref[7] *= SIM3_SCALE
+    st = po.default_track_settings(fl, main_tracker=False)
+    for ref, fr, q, tag in ((kf, tex, fr_to_ref, "blank->tex"), (tex, kf, _qts_op("lsdo_sim3d_inverse", 8, fr_to_ref), "tex->blank")):
+        r2f = _qts_op("lsdo_sim3d_inverse", 8, q)
+        for lvl in (4, 3, 2, 1):
+            _bits_equal(pin, f"sim3_eval/{tag}/L{lvl}", sim3_eval_fields(po.sim3_eval(ref, fr, lvl, r2f, 1.0, 0.0, settings=st)))
+        r = po.sim3_track(ref, fr, q, 4, 1)
+        x = sim3_track_fields(r)
+        if r.diverged:                  # left at level 4 (Sim3Tracker.cpp:186-190): the reference never wrote lastSim3Hessian
+            x = np.concatenate([x[:8], x[57:]])
+        _bits_equal(pin, f"sim3_track/{tag}", x, 8)
+
+
+# case -> (function, C-restatement flavour, reference-compiled flavour), as CASES
+SCENE_CASES = {c: CASES[c] for c in DEPTH + TRACK + ("point_cloud",)}
+SCENE_CASES["propagate_from_gt"] = (propagate_from_gt, False, "ref")
+SCENE_CASES.update({c: SIM3_CASES[c] for c in ("sim3_eval_mapped", "sim3_track_mapped", "perma_mapped")})
+SCENE_CASES["empty_keyframe"] = (empty_keyframe, False, "ref")
+TEXTURED = ("occluder", "posts", "stripes", "flat")
+SCENE_ONLY = {c: TEXTURED for c in SCENE_CASES}
+SCENE_ONLY["empty_keyframe"] = ("blank", "blank_const")
+SCENE_PAIRS = [(sc, c) for sc in scenes.NAMES for c in SCENE_CASES if sc in SCENE_ONLY[c]]
+
+
+def run_under_scene(scene, case, gold):
+    """runs one case on one scene on the C restatement (gold = the record) or on the reference-compiled library (gold = None);
+    returns the case's Pin"""
+    fn, fl, ref_fl = SCENE_CASES[case]
+    fl = ref_fl if gold is None else fl
+    seq, frames = scenes.stream(scene)
+    p = Pin(f"{scene}/{case}", gold)
+    try:
+        fn(p, fl, seq, frames)
+    finally:
+        po.set_globals(fl)
+    return p
+
+
+def record_scenes():
+    """every (scene, case) on the reference-compiled library (needs oracle/_ref): the arrays of ref_pin_scenes_320x240.npz"""
+    out = {}
+    for sc, c in SCENE_PAIRS:
+        out.update(run_under_scene(sc, c, None).rec)
     return out
