@@ -170,8 +170,24 @@ int lsdgpu_frame_minimize(lsdgpu_ctx* ctx, int frame_id);
 /* FrameMemory::activateFrame (FrameMemory.cpp:129-137) + Frame::require (Frame.cpp:319-338): takes a free slot, restores the record
  * and rebuilds image levels 1..4, the gradients and maxGradients from level 0 (3 kernels); the idepth pyramid is rebuilt on first
  * use.  The frame is byte-identical to the frame before lsdgpu_frame_minimize, except that its refPixelWasGood mask is cleared.
- * Already active: nothing to do (0).  No free slot: an error, and the frame stays minimized. */
+ * Already active: nothing to do (0).  No free slot: an error, and the frame stays minimized.  An offloaded frame is activated the
+ * same way: its host body is read over the bus, then the body and the residue are freed. */
 int lsdgpu_frame_activate(lsdgpu_ctx* ctx, int frame_id);
+/* The host tier of minimized frames.  The reference keeps a minimized frame in host RAM (Frame.cpp:377-395, FrameMemory.cpp:149-166);
+ * here a minimized record stays in device memory until the caller offloads it.  lsdgpu_frame_offload splits the record of a
+ * minimized frame: its host body (image, idepth and idepthVar of level 0, the reactivation data) moves to pinned host memory from
+ * a stream-ordered pool of the context on the device's host NUMA node, mapped into the device; a device residue (the depth
+ * statistics and the permaRef, ~20 KB) stays in device memory.  The old record is freed in stream order; the call never waits
+ * for the device.  An offloaded frame serves every call a minimized frame serves, with identical bytes (the kernels read the body
+ * over the bus), and every other call refuses it as it refuses a minimized frame.  Already offloaded: nothing to do (0).  A frame
+ * in a slot (minimize it first) or an unknown id: an error, nothing changes.  No host memory: an error, and the frame stays
+ * minimized in device memory.  Which frames to offload is the caller's choice: the library keeps no budget.  Found by symbol
+ * lookup (dlsym), like lsdgpu_frame_minimize; LSDGPU_ABI_VERSION is unchanged. */
+int lsdgpu_frame_offload(lsdgpu_ctx* ctx, int frame_id);
+/* The minimized frames of each tier (FrameMemory.cpp:149-166 bounds the active ones; this counts the rest): n_device records wholly
+ * in device memory and n_host offloaded ones; device_bytes = the layout bytes (DESIGN.md section 3) of every device record and
+ * residue, host_bytes = those of the host bodies.  Any pointer may be NULL.  Found by symbol lookup (dlsym). */
+int lsdgpu_frame_memory_usage(lsdgpu_ctx* ctx, int* n_device, size_t* device_bytes, int* n_host, size_t* host_bytes);
 
 /* ---- Tracking: Tracking/TrackingReference.cpp + Tracking/SE3Tracker.cpp -------------------------- */
 /* TrackingReference::importFrame :71-87 (+ the depthHasBeenUpdatedFlag=false of SlamSystem.cpp:907-912):

@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+from typing import NamedTuple
 
 import numpy as np
 
@@ -82,6 +83,15 @@ class GroupStep(C.Structure):
 
 
 GROUP_MAX_STEPS = 8
+
+
+class MemoryUsage(NamedTuple):
+    """Context.memory_usage: minimized frames whose record is in device memory, offloaded ones, and the records' layout bytes in
+    each tier (an offloaded frame's device residue counts under device_bytes)"""
+    n_device: int
+    device_bytes: int
+    n_host: int
+    host_bytes: int
 
 
 class RandState(C.Structure):
@@ -195,6 +205,8 @@ SYMBOLS = [
     ("lsdgpu_frame_clear_good_mask", C.c_int, [_vp, C.c_int]),
     ("lsdgpu_frame_minimize", C.c_int, [_vp, C.c_int]),
     ("lsdgpu_frame_activate", C.c_int, [_vp, C.c_int]),
+    ("lsdgpu_frame_offload", C.c_int, [_vp, C.c_int]),
+    ("lsdgpu_frame_memory_usage", C.c_int, [_vp, _ip, C.POINTER(C.c_size_t), _ip, C.POINTER(C.c_size_t)]),
     ("lsdgpu_ref_import", C.c_int, [_vp, C.c_int]),
     ("lsdgpu_se3_eval", C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _fp, C.c_float, C.c_float, C.POINTER(TrackSettings), C.c_int, C.POINTER(EvalResult)]),
     ("lsdgpu_se3_track", C.c_int, [_vp, C.c_int, C.c_int, _dp, C.POINTER(TrackSettings), C.c_int, C.POINTER(TrackResult)]),
@@ -536,6 +548,17 @@ class Context:
     def activate(self, fid: int):
         """FrameMemory::activateFrame + Frame::require (lsdgpu_frame_activate): a minimized frame takes a free slot again"""
         self._ck(self.L.lsdgpu_frame_activate(self.ptr, fid))
+
+    def offload(self, fid: int):
+        """moves a minimized frame's record to host memory, keeping its depth statistics and permaRef on the device
+        (lsdgpu_frame_offload); the frame serves the same calls as before, and activate brings it back into a slot"""
+        self._ck(self.L.lsdgpu_frame_offload(self.ptr, fid))
+
+    def memory_usage(self) -> "MemoryUsage":
+        """the minimized frames in each tier and their records' layout bytes (lsdgpu_frame_memory_usage)"""
+        nd, nh, db, hb = C.c_int(), C.c_int(), C.c_size_t(), C.c_size_t()
+        self._ck(self.L.lsdgpu_frame_memory_usage(self.ptr, C.byref(nd), C.byref(db), C.byref(nh), C.byref(hb)))
+        return MemoryUsage(nd.value, db.value, nh.value, hb.value)
 
     def download(self, fid: int, what: int, level: int = 0, out=None):
         """one plane of a frame as a numpy array, or -- out = a contiguous CUDA tensor (float32; uint8 for BUF_GOODMASK) of at

@@ -173,8 +173,12 @@ extern "C" void lsdgpu_destroy(lsdgpu_ctx* ctx)
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     peerCloseAll(ctx);
     cloudRelease(ctx);
-    for (auto& m : ctx->minimized) cudaFreeAsync(m.record, ctx->stream);
+    for (auto& m : ctx->minimized) {
+        cudaFreeAsync(m.record, ctx->stream);
+        if (m.hostRecord) cudaFreeAsync(m.hostRecord, ctx->stream);
+    }
     if (ctx->recordPool) { cudaStreamSynchronize(ctx->stream); cudaMemPoolDestroy(ctx->recordPool); }
+    if (ctx->hostPool) { cudaStreamSynchronize(ctx->stream); cudaMemPoolDestroy(ctx->hostPool); }
     cudaFree(ctx->arena);
     if (ctx->stageRing) cudaFree(ctx->stageRing);
     if (ctx->dRemapX) cudaFree(ctx->dRemapX);

@@ -141,12 +141,14 @@ extern "C" int lsdgpu_frame_release(lsdgpu_ctx* ctx, int frame_id)
             if (ctx->minimized[i].id == frame_id) {
                 LSD_CHECK(ctx, cudaSetDevice(ctx->device));
                 LSD_CHECK(ctx, cudaFreeAsync(ctx->minimized[i].record, ctx->stream));
+                if (ctx->minimized[i].hostRecord) LSD_CHECK(ctx, cudaFreeAsync(ctx->minimized[i].hostRecord, ctx->stream));
                 ctx->minimized.erase(ctx->minimized.begin() + i);
-                // the pool keeps freed records for later minimizes (see lsdgpu_frame_minimize); a released frame's memory goes back
-                // to the device, down to what the records still alive need
-                size_t live = 0;
-                for (const auto& m : ctx->minimized) live += m.recordBytes;
+                // the pools keep freed records for later minimizes and offloads (see lsdgpu_frame_minimize); a released frame's
+                // memory goes back to the device and the host, down to what the records still alive need
+                size_t live = 0, liveHost = 0;
+                for (const auto& m : ctx->minimized) { live += m.recordBytes; liveHost += m.hostRecordBytes; }
                 LSD_CHECK(ctx, cudaMemPoolTrimTo(ctx->recordPool, live));
+                if (ctx->hostPool) LSD_CHECK(ctx, cudaMemPoolTrimTo(ctx->hostPool, liveHost));
                 return 0;
             }
         return lsd_fail(ctx, "unknown frame id");
@@ -160,21 +162,22 @@ extern "C" int lsdgpu_frame_release(lsdgpu_ctx* ctx, int frame_id)
 // frame memory: Frame::minimizeInMemory and FrameMemory::activateFrame + Frame::require (DESIGN.md section 3)
 // ------------------------------------------------------------------------------------------------------
 // The buffers of a frame that a minimized record keeps, in record order: dStats, image / idepth / idepthVar of level 0, the
-// reactivation data, the permaRef.  Buffers the frame does not have are null.
-struct RecordPart { char** ptr; size_t bytes; };
+// reactivation data, the permaRef.  Buffers the frame does not have are null.  `body`: the part moves to the host body when the
+// record is offloaded; the others (the device residue) are what the permaRef batches and the pending depth statistics read.
+struct RecordPart { char** ptr; size_t bytes; bool body; };
 static int recordParts(const lsdgpu_ctx* ctx, FrameSlot& s, RecordPart* p)
 {
     const size_t n0 = (size_t)ctx->w * ctx->h;
     int k = 0;
-    p[k++] = { (char**)&s.dStats, 3 * sizeof(double) };
-    p[k++] = { (char**)&s.image[0], n0 * 4 };
-    p[k++] = { (char**)&s.idepth[0], s.hasDepth ? n0 * 4 : 0 };
-    p[k++] = { (char**)&s.idepthVar[0], s.hasDepth ? n0 * 4 : 0 };
-    p[k++] = { (char**)&s.reactIdepth, s.reactValid ? n0 * 4 : 0 };
-    p[k++] = { (char**)&s.reactVar, s.reactValid ? n0 * 4 : 0 };
-    p[k++] = { (char**)&s.reactValidity, s.reactValid ? n0 : 0 };
-    p[k++] = { (char**)&s.permaPC, (size_t)s.permaNumPts * 16 };
-    p[k++] = { (char**)&s.permaVar, (size_t)s.permaNumPts * 4 };
+    p[k++] = { (char**)&s.dStats, 3 * sizeof(double), false };
+    p[k++] = { (char**)&s.image[0], n0 * 4, true };
+    p[k++] = { (char**)&s.idepth[0], s.hasDepth ? n0 * 4 : 0, true };
+    p[k++] = { (char**)&s.idepthVar[0], s.hasDepth ? n0 * 4 : 0, true };
+    p[k++] = { (char**)&s.reactIdepth, s.reactValid ? n0 * 4 : 0, true };
+    p[k++] = { (char**)&s.reactVar, s.reactValid ? n0 * 4 : 0, true };
+    p[k++] = { (char**)&s.reactValidity, s.reactValid ? n0 : 0, true };
+    p[k++] = { (char**)&s.permaPC, (size_t)s.permaNumPts * 16, false };
+    p[k++] = { (char**)&s.permaVar, (size_t)s.permaNumPts * 4, false };
     return k;
 }
 cudaError_t ensureRecordPool(lsdgpu_ctx* ctx)
@@ -288,12 +291,105 @@ extern "C" int lsdgpu_frame_activate(lsdgpu_ctx* ctx, int frame_id)
     LAUNCH(ctx);
     LSD_CHECK(ctx, cudaGetLastError());
     LSD_CHECK(ctx, cudaFreeAsync(m->record, ctx->stream));
+    if (m->hostRecord) LSD_CHECK(ctx, cudaFreeAsync(m->hostRecord, ctx->stream));
     a.record = nullptr; a.recordBytes = 0;
+    a.hostRecord = nullptr; a.hostRecordBytes = 0;
     a.used = true;
     a.idepthPyrValid = false;                                       // ensureIdepthPyramid rebuilds levels 1..4 on first use
     a.reactAllocated = a.reactValid;
     *c = a;
     ctx->minimized.erase(ctx->minimized.begin() + (m - ctx->minimized.data()));
+    return 0;
+}
+
+// The host tier of minimized records: a stream-ordered pool of pinned memory on the host NUMA node next to the device, mapped
+// into the device's address space, so that the kernels that read a record (k_record_copy, k_image_pyramid, the cloud export)
+// read a host body over the bus unchanged.  Created on the first offload, destroyed with the context.
+static cudaError_t ensureHostPool(lsdgpu_ctx* ctx)
+{
+    if (ctx->hostPool) return cudaSuccess;
+    int supported = 0, numa = 0;
+    cudaError_t e = cudaDeviceGetAttribute(&supported, cudaDevAttrHostNumaMemoryPoolsSupported, ctx->device);
+    if (e == cudaSuccess && !supported) e = cudaErrorNotSupported;
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&numa, cudaDevAttrHostNumaId, ctx->device);
+    if (e != cudaSuccess) return e;
+    cudaMemPoolProps pp;
+    memset(&pp, 0, sizeof(pp));
+    pp.allocType = cudaMemAllocationTypePinned;
+    pp.location.type = cudaMemLocationTypeHostNuma; pp.location.id = numa < 0 ? 0 : numa;     // -1: a host without NUMA nodes
+    cudaMemPool_t pool;
+    if ((e = cudaMemPoolCreate(&pool, &pp)) != cudaSuccess) return e;
+    cudaMemAccessDesc ad;
+    memset(&ad, 0, sizeof(ad));
+    ad.location.type = cudaMemLocationTypeDevice; ad.location.id = ctx->device;
+    ad.flags = cudaMemAccessFlagsProtReadWrite;
+    uint64_t keep = UINT64_MAX;                                        // as recordPool: freed bodies stay for the next offload
+    if ((e = cudaMemPoolSetAccess(pool, &ad, 1)) != cudaSuccess ||
+        (e = cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep)) != cudaSuccess) {
+        cudaMemPoolDestroy(pool);
+        return e;
+    }
+    ctx->hostPool = pool;
+    return cudaSuccess;
+}
+
+extern "C" int lsdgpu_frame_offload(lsdgpu_ctx* ctx, int frame_id)
+{ LSD_LOCK(ctx);
+    FrameSlot* m = findMinimized(ctx, frame_id);
+    if (!m) {
+        if (!findSlot(ctx, frame_id)) return lsd_fail(ctx, "unknown frame id");
+        ctx->err = "frame " + std::to_string(frame_id) + " is active: only a minimized frame can be offloaded (lsdgpu_frame_minimize it first)";
+        return -2;
+    }
+    if (m->hostRecord) return 0;
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    FrameSlot o = *m;
+    RecordPart from[REC_MAX_SEGS], to[REC_MAX_SEGS];
+    const int np = recordParts(ctx, *m, from);
+    recordParts(ctx, o, to);
+    size_t bytes[2] = { 0, 0 };                                        // [0] the device residue, [1] the host body
+    for (int k = 0; k < np; k++) bytes[from[k].body] += alignUp(from[k].bytes, 256);
+    char* base[2] = { nullptr, nullptr };
+    cudaError_t e = ensureHostPool(ctx);
+    if (e == cudaSuccess) e = cudaMallocFromPoolAsync((void**)&base[1], bytes[1], ctx->hostPool, ctx->stream);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        ctx->err = "frame_offload: no host memory for frame " + std::to_string(frame_id) + " (" + cudaGetErrorString(e) +
+                   "); it stays minimized in device memory";
+        return -1;
+    }
+    e = cudaMallocFromPoolAsync((void**)&base[0], bytes[0], ctx->recordPool, ctx->stream);
+    if (e != cudaSuccess) { cudaFreeAsync(base[1], ctx->stream); LSD_CHECK(ctx, e); }
+    RecordCopy c;
+    memset(&c, 0, sizeof(c));
+    size_t off[2] = { 0, 0 };
+    for (int k = 0; k < np; k++) {
+        const int b = from[k].body;
+        *to[k].ptr = from[k].bytes ? base[b] + off[b] : nullptr;
+        addCopy(c, *from[k].ptr, *to[k].ptr, from[k].bytes);
+        off[b] += alignUp(from[k].bytes, 256);
+    }
+    const int r = launchRecordCopy(ctx, c);
+    if (r) { cudaFreeAsync(base[0], ctx->stream); cudaFreeAsync(base[1], ctx->stream); return r; }
+    LSD_CHECK(ctx, cudaFreeAsync(m->record, ctx->stream));
+    o.record = base[0]; o.recordBytes = bytes[0];
+    o.hostRecord = base[1]; o.hostRecordBytes = bytes[1];
+    *m = o;
+    return 0;
+}
+
+extern "C" int lsdgpu_frame_memory_usage(lsdgpu_ctx* ctx, int* n_device, size_t* device_bytes, int* n_host, size_t* host_bytes)
+{ LSD_LOCK(ctx);
+    int nd = 0, nh = 0;
+    size_t db = 0, hb = 0;
+    for (const auto& m : ctx->minimized) {
+        (m.hostRecord ? nh : nd)++;
+        db += m.recordBytes; hb += m.hostRecordBytes;
+    }
+    if (n_device) *n_device = nd;
+    if (device_bytes) *device_bytes = db;
+    if (n_host) *n_host = nh;
+    if (host_bytes) *host_bytes = hb;
     return 0;
 }
 
@@ -359,7 +455,9 @@ extern "C" int lsdgpu_frame_download(lsdgpu_ctx* ctx, int frame_id, int what, in
     int r = downloadPlane(ctx, frame_id, what, level, &s, &bytes);
     if (r || (r = downloadSource(ctx, s, what, level, &src))) return r;
     if (!src) { memset(out, 1, bytes); return 0; }
-    LSD_CHECK(ctx, cudaMemcpyAsync(out, src, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    // from an offloaded frame's host body the copy is host to host, which cudaMemcpyAsync need not order behind the stream
+    if (s->hostRecord) LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+    LSD_CHECK(ctx, cudaMemcpyAsync(out, src, bytes, cudaMemcpyDefault, ctx->stream));
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
     return 0;
 }
@@ -377,7 +475,7 @@ extern "C" int lsdgpu_frame_download_device(lsdgpu_ctx* ctx, int frame_id, int w
         return r;
     LSD_CHECK(ctx, afterCallerStream(ctx, stream));
     if ((r = downloadSource(ctx, s, what, level, &src))) return r;
-    if (src) LSD_CHECK(ctx, cudaMemcpyAsync(d_out, src, bytes, cudaMemcpyDeviceToDevice, ctx->stream));
+    if (src) LSD_CHECK(ctx, cudaMemcpyAsync(d_out, src, bytes, cudaMemcpyDefault, ctx->stream));
     else LSD_CHECK(ctx, cudaMemsetAsync(d_out, 1, bytes, ctx->stream));
     LSD_CHECK(ctx, beforeCallerStream(ctx, stream));
     return 0;

@@ -63,6 +63,10 @@ struct FrameSlot {
     int numFramesTrackedOnThis = 0, numMappedOnThis = 0;
     char* record = nullptr;              // minimized frame (lsdgpu_frame_minimize): its record, which the pointers above point into
     size_t recordBytes = 0;
+    // offloaded frame (lsdgpu_frame_offload): the host body (image / idepth / idepthVar of level 0, the reactivation data), which
+    // those pointers point into; `record` is then the device residue (dStats, the permaRef)
+    char* hostRecord = nullptr;
+    size_t hostRecordBytes = 0;
 };
 
 struct PyrPtrs {
@@ -134,9 +138,10 @@ struct lsdgpu_ctx {
     std::vector<FrameSlot> slots;
     // minimized frames (Frame::minimizeInMemory): the frame's metadata, with image / idepth / idepthVar of level 0, the
     // reactivation data, the permaRef and dStats pointing into its record and every other device pointer null.  Records come
-    // in stream order from recordPool (DESIGN.md section 3).
+    // in stream order from recordPool, the host bodies of offloaded ones from hostPool (DESIGN.md section 3).
     std::vector<FrameSlot> minimized;
     cudaMemPool_t recordPool = nullptr;
+    cudaMemPool_t hostPool = nullptr;    // the host bodies of offloaded records: pinned memory on the device's host NUMA node
 
     // depth map
     HypField cur, oth;

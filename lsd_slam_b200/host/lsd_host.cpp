@@ -131,12 +131,17 @@ void FrameMemory::minimizeLeastRecent()
         Frame* f = *it;
         if (f->id() == activeKf || std::find(held_.begin(), held_.end(), f) != held_.end()) continue;
         activeFrames.erase(std::next(it).base());
-        f->minimizeOnDevice();
-        f->isActive = false;
+        minimize(f);
         return;
     }
     throw LsdGpuError("FrameMemory: no frame slot can be freed: every active frame is the active keyframe or in use by this call "
                       "(raise max_frames)");
+}
+void FrameMemory::minimize(Frame* frame)
+{
+    frame->minimizeOnDevice();
+    frame->isActive = false;
+    deviceRecords_.push_front(frame);
 }
 void FrameMemory::makeRoom()
 {
@@ -151,8 +156,9 @@ void FrameMemory::activateFrame(Frame* frame)
         activeFrames.remove(frame);
     } else {
         makeRoom();
-        dev_.check(lsdgpu_frame_activate(dev_.raw(), frame->id()), "FrameMemory::activateFrame");
+        dev_.check(lsdgpu_frame_activate(dev_.raw(), frame->id()), "FrameMemory::activateFrame");     // from either tier
         frame->isActive = true;
+        deviceRecords_.remove(frame);
     }
     activeFrames.push_front(frame);
 }
@@ -162,14 +168,18 @@ void FrameMemory::deactivateFrame(Frame* frame)
     std::lock_guard<std::recursive_mutex> l(mu_);
     if (!frame->isActive) return;
     activeFrames.remove(frame);
-    frame->minimizeOnDevice();
-    frame->isActive = false;
+    minimize(frame);
 }
 void FrameMemory::pruneActiveFrames()
 {
     dev_.followGlobals();
     std::lock_guard<std::recursive_mutex> l(mu_);
     while ((int)activeFrames.size() > maxActive_) minimizeLeastRecent();
+    while (maxDeviceRecords_ >= 0 && (int)deviceRecords_.size() > maxDeviceRecords_) {
+        Frame* f = deviceRecords_.back();
+        dev_.check(lsdgpu_frame_offload(dev_.raw(), f->id()), "FrameMemory::pruneActiveFrames");
+        deviceRecords_.pop_back();
+    }
 }
 
 ActiveFrames::ActiveFrames(FrameMemory& memory, std::initializer_list<Frame*> frames)
@@ -212,6 +222,7 @@ Frame::~Frame()
         FrameMemory& m = dev_.frameMemory();
         std::lock_guard<std::recursive_mutex> l(m.mu_);
         if (isActive) m.activeFrames.remove(this);
+        else m.deviceRecords_.remove(this);
     }
     lsdgpu_frame_release(dev_.raw(), id_);      // may fail for the active keyframe: DepthMap::invalidate() first
     delete pose;

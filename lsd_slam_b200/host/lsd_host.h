@@ -85,23 +85,31 @@ extern bool allowNegativeIdepths, useSubpixelStereo, useAffineLightningEstimatio
 // reference's heap is unbounded; a context has max_frames slots, so activating a frame (or constructing one) with every slot
 // taken first minimizes the least recently activated frame that is neither the depth map's active keyframe nor held by a call
 // in progress (ActiveFrames).  A call that needs more frames than that leaves free throws LsdGpuError.
+// The reference keeps minimized frames in host RAM; here their records stay in device memory unless setMaxDeviceRecords(n) is set:
+// pruneActiveFrames then also offloads the least recently minimized records beyond n to host memory (lsdgpu_frame_offload).
 class FrameMemory {
 public:
     FrameMemory(DeviceContext& dev, int maxActive);
     void activateFrame(Frame* frame);                   // FrameMemory.cpp:129-137 + Frame::require (lsdgpu_frame_activate)
     void deactivateFrame(Frame* frame);                 // FrameMemory.cpp:138-147
-    void pruneActiveFrames();                           // FrameMemory.cpp:149-166: at most maxActive frames stay active
+    // FrameMemory.cpp:149-166: at most maxActive frames stay active, and at most maxDeviceRecords minimized ones in device memory
+    void pruneActiveFrames();
     int maxActiveFrames() const { return maxActive_; }
     void setMaxActiveFrames(int n) { maxActive_ = n; }
+    int maxDeviceRecords() const { return maxDeviceRecords_; }
+    void setMaxDeviceRecords(int n) { maxDeviceRecords_ = n; }     // < 0: unlimited (the default)
 
 private:
     friend class Frame;
     friend class ActiveFrames;
     void makeRoom();                                    // a free slot for one more active frame
     void minimizeLeastRecent();
+    void minimize(Frame* frame);
     DeviceContext& dev_;
     int maxActive_;
+    int maxDeviceRecords_ = -1;
     std::list<Frame*> activeFrames;                     // most recently activated first
+    std::list<Frame*> deviceRecords_;                   // minimized frames whose record is in device memory, most recent first
     std::vector<Frame*> held_;                          // frames of the calls in progress (ActiveFrames)
     std::recursive_mutex mu_;                           // FrameMemory::activeFramesMutex (tracking and mapping threads)
 };

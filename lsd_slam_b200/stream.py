@@ -16,6 +16,8 @@ The stream keeps the ids of its keyframes and their camToWorld, chained from the
 viewer's map of the run.  With ``keep_keyframes=True`` finished keyframes stay resident (the context needs a frame slot for each);
 adding ``max_active_keyframes=k`` keeps only the newest k finished keyframes in frame slots and minimizes the older ones after each
 keyframe change (``Context.minimize``, FrameMemory::pruneActiveFrames, FrameMemory.cpp:149-166), so the map can outgrow max_frames.
+Adding ``max_device_records=m`` then keeps only the newest m minimized records in device memory and offloads the older ones to
+host memory (``Context.offload``), so the map is bounded by host memory, as the reference's minimized frames are.
 
 ``GpuStreamGroup`` steps K such streams (one context each, same GPU) with ONE call per frame
 (``lsdgpu_track_and_map_group``): the trackings of the K frames share one launch, each stream on its own slice of the SMs.
@@ -64,12 +66,15 @@ def qts_to_sim3f(qts) -> np.ndarray:
 
 class GpuStream:
     def __init__(self, ctx: abi.Context, mode: int = 1, kf_every: int = 20, fused_call: bool = True, kf_phase: int = 0,
-                 keep_keyframes: bool = False, max_active_keyframes: int | None = None):
+                 keep_keyframes: bool = False, max_active_keyframes: int | None = None, max_device_records: int | None = None):
         if max_active_keyframes is not None and (not keep_keyframes or max_active_keyframes < 0):
             raise ValueError("max_active_keyframes needs keep_keyframes=True and a count >= 0")
+        if max_device_records is not None and (max_active_keyframes is None or max_device_records < 0):
+            raise ValueError("max_device_records needs max_active_keyframes and a count >= 0")
         self.ctx = ctx
         self.keep_keyframes = keep_keyframes
         self.max_active_keyframes = max_active_keyframes
+        self.max_device_records = max_device_records
         self.keyframe_ids: list[int] = []          # every keyframe of the run, oldest first
         self.keyframe_cam_to_world: list[np.ndarray] = []   # their camToWorld as qts[8], the first keyframe at the origin
         self.kf_phase = kf_phase          # shifts the forced keyframe changes: frame n changes keyframe when (n + kf_phase) % kf_every == 0
@@ -176,8 +181,12 @@ class GpuStream:
             self.prev_ids = []
             if self.max_active_keyframes is not None:
                 finished = self.keyframe_ids[:-1]
-                for i in finished[:max(0, len(finished) - self.max_active_keyframes)]:
+                minimized = finished[:max(0, len(finished) - self.max_active_keyframes)]
+                for i in minimized:
                     ctx.minimize(i)             # a no-op for a keyframe that is minimized already; one the caller re-activated goes again
+                if self.max_device_records is not None:
+                    for i in minimized[:max(0, len(minimized) - self.max_device_records)]:
+                        ctx.offload(i)          # likewise a no-op for a keyframe whose record is in host memory already
         else:
             self.last_pose = pose
             self.prev_ids.append(fid)
