@@ -173,12 +173,9 @@ extern "C" void lsdgpu_destroy(lsdgpu_ctx* ctx)
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     peerCloseAll(ctx);
     cloudRelease(ctx);
-    for (auto& m : ctx->minimized) {
-        cudaFreeAsync(m.record, ctx->stream);
-        if (m.hostRecord) cudaFreeAsync(m.hostRecord, ctx->stream);
-    }
-    if (ctx->recordPool) { cudaStreamSynchronize(ctx->stream); cudaMemPoolDestroy(ctx->recordPool); }
-    if (ctx->hostPool) { cudaStreamSynchronize(ctx->stream); cudaMemPoolDestroy(ctx->hostPool); }
+    for (auto& m : ctx->minimized) freeRecord(ctx, m);
+    for (cudaMemPool_t p : ctx->pool)
+        if (p) { cudaStreamSynchronize(ctx->stream); cudaMemPoolDestroy(p); }
     cudaFree(ctx->arena);
     if (ctx->stageRing) cudaFree(ctx->stageRing);
     if (ctx->dRemapX) cudaFree(ctx->dRemapX);

@@ -736,7 +736,7 @@ extern "C" int lsdgpu_frame_download_reactivation_data(lsdgpu_ctx* ctx, int kf_i
     if (!kf->reactValid) return lsd_fail(ctx, "keyframe has no reactivation data");
     const size_t n = (size_t)ctx->w * ctx->h;
     // from an offloaded keyframe's host body the copies are host to host, which cudaMemcpyAsync need not order behind the stream
-    if (kf->hostRecord) LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+    if (kf->record[TIER_HOST]) LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
     if (idepth_reAct) LSD_CHECK(ctx, cudaMemcpyAsync(idepth_reAct, kf->reactIdepth, n * 4, cudaMemcpyDefault, ctx->stream));
     if (idepthVar_reAct) LSD_CHECK(ctx, cudaMemcpyAsync(idepthVar_reAct, kf->reactVar, n * 4, cudaMemcpyDefault, ctx->stream));
     if (validity_reAct) LSD_CHECK(ctx, cudaMemcpyAsync(validity_reAct, kf->reactValidity, n, cudaMemcpyDefault, ctx->stream));

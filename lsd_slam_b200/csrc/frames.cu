@@ -1,5 +1,5 @@
-// frames.cu -- frame slots of the C ABI (include/lsdgpu.h): upload, the device prefetch ring, release, download, pose / counter
-// setters and getters, depth import, and the input undistorters (UndistorterPTAM, UndistorterOpenCV) in front of the frame construction.
+// frames.cu -- frame slots of the C ABI (include/lsdgpu.h): upload, the device prefetch ring, download, pose / counter setters and
+// getters, depth import, the input undistorters in front of the frame construction, and the kernel launches of records.cu.
 #include <algorithm>
 #include <cfloat>
 #include <climits>
@@ -110,8 +110,8 @@ extern "C" int lsdgpu_stage_put_device(lsdgpu_ctx* ctx, int index, const uint8_t
     return 0;
 }
 
-// dsrc: the u8 image (PYR_U8) or the raw image (PYR_PTAM, PYR_OPENCV), `pitch` bytes per row
-static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int pitch, int src)
+// k_image_pyramid<src> from `dsrc` (`pitch` bytes per row), then k_gradients, over the buffers of slot `s`
+static int buildImagePyramid(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int pitch, int src)
 {
     const int w = ctx->w, h = ctx->h;
     PyrPtrs pp;
@@ -120,6 +120,7 @@ static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* 
     else if (src == PYR_OPENCV)
         k_image_pyramid<PYR_OPENCV><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h, nullptr, nullptr, ctx->rawW,
                                                                                    nullptr, ctx->dCvMap1, ctx->dCvMap2, ctx->rawH);
+    else if (src == PYR_F32) k_image_pyramid<PYR_F32><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h);
     else k_image_pyramid<PYR_U8><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h);
     LAUNCH(ctx);
     GradPtrs gp;
@@ -129,267 +130,37 @@ static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* 
     LSD_CHECK(ctx, launchPDL(k_gradients, dim3(divUp(w, GR_TW) * divUp(h, GR_TH), LSD_LEVELS), dim3(256), 0, ctx->stream, gp));      // + maxGradients of level 0
     LAUNCH(ctx);
     LSD_CHECK(ctx, cudaGetLastError());
-    s->hasDepth = false; s->idepthPyrValid = false; s->hasGoodMask = false;
     return 0;
 }
 
-extern "C" int lsdgpu_frame_release(lsdgpu_ctx* ctx, int frame_id)
-{ LSD_LOCK(ctx);
-    FrameSlot* s = findSlot(ctx, frame_id);
-    if (!s) {
-        for (size_t i = 0; i < ctx->minimized.size(); i++)
-            if (ctx->minimized[i].id == frame_id) {
-                LSD_CHECK(ctx, cudaSetDevice(ctx->device));
-                LSD_CHECK(ctx, cudaFreeAsync(ctx->minimized[i].record, ctx->stream));
-                if (ctx->minimized[i].hostRecord) LSD_CHECK(ctx, cudaFreeAsync(ctx->minimized[i].hostRecord, ctx->stream));
-                ctx->minimized.erase(ctx->minimized.begin() + i);
-                // the pools keep freed records for later minimizes and offloads (see lsdgpu_frame_minimize); a released frame's
-                // memory goes back to the device and the host, down to what the records still alive need
-                size_t live = 0, liveHost = 0;
-                for (const auto& m : ctx->minimized) { live += m.recordBytes; liveHost += m.hostRecordBytes; }
-                LSD_CHECK(ctx, cudaMemPoolTrimTo(ctx->recordPool, live));
-                if (ctx->hostPool) LSD_CHECK(ctx, cudaMemPoolTrimTo(ctx->hostPool, liveHost));
-                return 0;
-            }
-        return lsd_fail(ctx, "unknown frame id");
+// dsrc: the u8 image (PYR_U8) or the raw image (PYR_PTAM, PYR_OPENCV), `pitch` bytes per row
+static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int pitch, int src)
+{
+    const int r = buildImagePyramid(ctx, s, dsrc, pitch, src);
+    if (!r) { s->hasDepth = false; s->idepthPyrValid = false; s->hasGoodMask = false; }
+    return r;
+}
+
+int buildImagePyramidFromRecord(lsdgpu_ctx* ctx, FrameSlot* s, const float* image0)
+{
+    return buildImagePyramid(ctx, s, (const uint8_t*)image0, ctx->w * 4, PYR_F32);
+}
+
+int launchRecordCopy(lsdgpu_ctx* ctx, const RecordPart* from, const RecordPart* to, int n)
+{
+    static_assert(REC_PARTS <= REC_MAX_SEGS, "a record's parts are copied in one launch");
+    RecordCopy c = {};
+    for (int k = 0; k < n; k++) {
+        if (!from[k].bytes) continue;
+        c.src[c.n] = (const uint4*)*from[k].ptr; c.dst[c.n] = (uint4*)*to[k].ptr;
+        c.end[c.n] = (c.n ? c.end[c.n - 1] : 0) + (long long)(alignUp(from[k].bytes, 16) / 16);
+        c.n++;
     }
-    if (ctx->activeKf == frame_id) return lsd_fail(ctx, "frame is the active keyframe of the depth map");
-    s->used = false; s->id = -1;
-    return 0;
-}
-
-// ------------------------------------------------------------------------------------------------------
-// frame memory: Frame::minimizeInMemory and FrameMemory::activateFrame + Frame::require (DESIGN.md section 3)
-// ------------------------------------------------------------------------------------------------------
-// The buffers of a frame that a minimized record keeps, in record order: dStats, image / idepth / idepthVar of level 0, the
-// reactivation data, the permaRef.  Buffers the frame does not have are null.  `body`: the part moves to the host body when the
-// record is offloaded; the others (the device residue) are what the permaRef batches and the pending depth statistics read.
-struct RecordPart { char** ptr; size_t bytes; bool body; };
-static int recordParts(const lsdgpu_ctx* ctx, FrameSlot& s, RecordPart* p)
-{
-    const size_t n0 = (size_t)ctx->w * ctx->h;
-    int k = 0;
-    p[k++] = { (char**)&s.dStats, 3 * sizeof(double), false };
-    p[k++] = { (char**)&s.image[0], n0 * 4, true };
-    p[k++] = { (char**)&s.idepth[0], s.hasDepth ? n0 * 4 : 0, true };
-    p[k++] = { (char**)&s.idepthVar[0], s.hasDepth ? n0 * 4 : 0, true };
-    p[k++] = { (char**)&s.reactIdepth, s.reactValid ? n0 * 4 : 0, true };
-    p[k++] = { (char**)&s.reactVar, s.reactValid ? n0 * 4 : 0, true };
-    p[k++] = { (char**)&s.reactValidity, s.reactValid ? n0 : 0, true };
-    p[k++] = { (char**)&s.permaPC, (size_t)s.permaNumPts * 16, false };
-    p[k++] = { (char**)&s.permaVar, (size_t)s.permaNumPts * 4, false };
-    return k;
-}
-cudaError_t ensureRecordPool(lsdgpu_ctx* ctx)
-{
-    if (ctx->recordPool) return cudaSuccess;
-    cudaMemPoolProps pp;
-    memset(&pp, 0, sizeof(pp));
-    pp.allocType = cudaMemAllocationTypePinned;
-    pp.location.type = cudaMemLocationTypeDevice; pp.location.id = ctx->device;
-    cudaError_t e = cudaMemPoolCreate(&ctx->recordPool, &pp);
-    if (e != cudaSuccess) { ctx->recordPool = nullptr; return e; }
-    // freed blocks stay mapped for the next allocation instead of going back to the device at each synchronisation (which
-    // made every allocation map fresh memory on the stream); the context's destruction returns them
-    uint64_t keep = UINT64_MAX;
-    return cudaMemPoolSetAttribute(ctx->recordPool, cudaMemPoolAttrReleaseThreshold, &keep);
-}
-static void addCopy(RecordCopy& c, const void* src, void* dst, size_t bytes)
-{
-    if (!bytes) return;
-    c.src[c.n] = (const uint4*)src; c.dst[c.n] = (uint4*)dst;
-    c.end[c.n] = (c.n ? c.end[c.n - 1] : 0) + (long long)(alignUp(bytes, 16) / 16);
-    c.n++;
-}
-static int launchRecordCopy(lsdgpu_ctx* ctx, const RecordCopy& c)
-{
     const long long total = c.end[c.n - 1];
     const int grid = (int)std::min<long long>((total + 255) / 256, (long long)ctx->smCount * 8);
     k_record_copy<<<grid, 256, 0, ctx->stream>>>(c);
     LAUNCH(ctx);
     LSD_CHECK(ctx, cudaGetLastError());
-    return 0;
-}
-
-extern "C" int lsdgpu_frame_minimize(lsdgpu_ctx* ctx, int frame_id)
-{ LSD_LOCK(ctx);
-    if (findMinimized(ctx, frame_id)) return 0;
-    FrameSlot* s = findSlot(ctx, frame_id);
-    if (!s) return lsd_fail(ctx, "unknown frame id");
-    if (ctx->activeKf == frame_id) return lsd_fail(ctx, "frame is the active keyframe of the depth map");
-    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
-    LSD_CHECK(ctx, ensureRecordPool(ctx));
-    FrameSlot m = *s;
-    RecordPart from[REC_MAX_SEGS], to[REC_MAX_SEGS];
-    const int np = recordParts(ctx, *s, from);
-    recordParts(ctx, m, to);
-    size_t bytes = 0;
-    for (int k = 0; k < np; k++) bytes += alignUp(from[k].bytes, 256);
-    char* rec = nullptr;
-    LSD_CHECK(ctx, cudaMallocFromPoolAsync((void**)&rec, bytes, ctx->recordPool, ctx->stream));
-    RecordCopy c;
-    memset(&c, 0, sizeof(c));
-    size_t off = 0;
-    for (int k = 0; k < np; k++) {
-        *to[k].ptr = from[k].bytes ? rec + off : nullptr;
-        addCopy(c, *from[k].ptr, *to[k].ptr, from[k].bytes);
-        off += alignUp(from[k].bytes, 256);
-    }
-    const int r = launchRecordCopy(ctx, c);
-    if (r) { cudaFreeAsync(rec, ctx->stream); return r; }
-    for (int l = 0; l < LSD_LEVELS; l++) {
-        m.grad[l] = nullptr;
-        if (l) m.image[l] = m.idepth[l] = m.idepthVar[l] = nullptr;
-    }
-    m.maxgrad = nullptr; m.goodMask = nullptr;
-    m.record = rec; m.recordBytes = bytes;
-    m.idepthPyrValid = false;
-    m.hasGoodMask = false;                                          // clear_refPixelWasGood, Frame.cpp:388
-    ctx->minimized.push_back(m);
-    s->used = false; s->id = -1;
-    return 0;
-}
-
-extern "C" int lsdgpu_frame_activate(lsdgpu_ctx* ctx, int frame_id)
-{ LSD_LOCK(ctx);
-    if (findSlot(ctx, frame_id)) return 0;
-    FrameSlot* m = findMinimized(ctx, frame_id);
-    if (!m) return lsd_fail(ctx, "unknown frame id");
-    FrameSlot* c = nullptr;
-    for (auto& f : ctx->slots)
-        if (!f.used) { c = &f; break; }
-    if (!c) {
-        ctx->err = "no free frame slot to activate frame " + std::to_string(frame_id) + " (minimize or release frames, or raise max_frames); it stays minimized";
-        return -2;
-    }
-    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
-    FrameSlot a = *m;
-    RecordPart from[REC_MAX_SEGS], to[REC_MAX_SEGS];
-    const int np = recordParts(ctx, *m, from);
-    for (int l = 0; l < LSD_LEVELS; l++) {                         // the slot's buffers
-        a.image[l] = c->image[l]; a.grad[l] = c->grad[l]; a.idepth[l] = c->idepth[l]; a.idepthVar[l] = c->idepthVar[l];
-    }
-    a.maxgrad = c->maxgrad; a.goodMask = c->goodMask; a.dStats = c->dStats;
-    a.permaPC = c->permaPC; a.permaVar = c->permaVar;
-    a.reactIdepth = c->reactIdepth; a.reactVar = c->reactVar; a.reactValidity = c->reactValidity;
-    recordParts(ctx, a, to);
-    RecordCopy cp;
-    memset(&cp, 0, sizeof(cp));
-    for (int k = 0; k < np; k++)
-        if (from[k].ptr != (char**)&m->image[0]) addCopy(cp, *from[k].ptr, *to[k].ptr, from[k].bytes);   // level 0 of the image: below
-    int r = launchRecordCopy(ctx, cp);
-    if (r) return r;
-    PyrPtrs pp;
-    for (int l = 0; l < LSD_LEVELS; l++) pp.l[l] = a.image[l];
-    k_image_pyramid<PYR_F32><<<dim3(ctx->w / 16, ctx->h / 16), 256, 0, ctx->stream>>>((const uint8_t*)m->image[0], ctx->w * 4, pp, ctx->w,
-                                                                                      ctx->h);
-    LAUNCH(ctx);
-    GradPtrs gp;
-    for (int l = 0; l < LSD_LEVELS; l++) { gp.img[l] = a.image[l]; gp.grad[l] = a.grad[l]; gp.w[l] = ctx->w >> l; gp.h[l] = ctx->h >> l; }
-    gp.maxgrad0 = a.maxgrad;
-    LSD_CHECK(ctx, launchPDL(k_gradients, dim3(divUp(ctx->w, GR_TW) * divUp(ctx->h, GR_TH), LSD_LEVELS), dim3(256), 0, ctx->stream, gp));
-    LAUNCH(ctx);
-    LSD_CHECK(ctx, cudaGetLastError());
-    LSD_CHECK(ctx, cudaFreeAsync(m->record, ctx->stream));
-    if (m->hostRecord) LSD_CHECK(ctx, cudaFreeAsync(m->hostRecord, ctx->stream));
-    a.record = nullptr; a.recordBytes = 0;
-    a.hostRecord = nullptr; a.hostRecordBytes = 0;
-    a.used = true;
-    a.idepthPyrValid = false;                                       // ensureIdepthPyramid rebuilds levels 1..4 on first use
-    a.reactAllocated = a.reactValid;
-    *c = a;
-    ctx->minimized.erase(ctx->minimized.begin() + (m - ctx->minimized.data()));
-    return 0;
-}
-
-// The host tier of minimized records: a stream-ordered pool of pinned memory on the host NUMA node next to the device, mapped
-// into the device's address space, so that the kernels that read a record (k_record_copy, k_image_pyramid, the cloud export)
-// read a host body over the bus unchanged.  Created on the first offload, destroyed with the context.
-static cudaError_t ensureHostPool(lsdgpu_ctx* ctx)
-{
-    if (ctx->hostPool) return cudaSuccess;
-    int supported = 0, numa = 0;
-    cudaError_t e = cudaDeviceGetAttribute(&supported, cudaDevAttrHostNumaMemoryPoolsSupported, ctx->device);
-    if (e == cudaSuccess && !supported) e = cudaErrorNotSupported;
-    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&numa, cudaDevAttrHostNumaId, ctx->device);
-    if (e != cudaSuccess) return e;
-    cudaMemPoolProps pp;
-    memset(&pp, 0, sizeof(pp));
-    pp.allocType = cudaMemAllocationTypePinned;
-    pp.location.type = cudaMemLocationTypeHostNuma; pp.location.id = numa < 0 ? 0 : numa;     // -1: a host without NUMA nodes
-    cudaMemPool_t pool;
-    if ((e = cudaMemPoolCreate(&pool, &pp)) != cudaSuccess) return e;
-    cudaMemAccessDesc ad;
-    memset(&ad, 0, sizeof(ad));
-    ad.location.type = cudaMemLocationTypeDevice; ad.location.id = ctx->device;
-    ad.flags = cudaMemAccessFlagsProtReadWrite;
-    uint64_t keep = UINT64_MAX;                                        // as recordPool: freed bodies stay for the next offload
-    if ((e = cudaMemPoolSetAccess(pool, &ad, 1)) != cudaSuccess ||
-        (e = cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep)) != cudaSuccess) {
-        cudaMemPoolDestroy(pool);
-        return e;
-    }
-    ctx->hostPool = pool;
-    return cudaSuccess;
-}
-
-extern "C" int lsdgpu_frame_offload(lsdgpu_ctx* ctx, int frame_id)
-{ LSD_LOCK(ctx);
-    FrameSlot* m = findMinimized(ctx, frame_id);
-    if (!m) {
-        if (!findSlot(ctx, frame_id)) return lsd_fail(ctx, "unknown frame id");
-        ctx->err = "frame " + std::to_string(frame_id) + " is active: only a minimized frame can be offloaded (lsdgpu_frame_minimize it first)";
-        return -2;
-    }
-    if (m->hostRecord) return 0;
-    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
-    FrameSlot o = *m;
-    RecordPart from[REC_MAX_SEGS], to[REC_MAX_SEGS];
-    const int np = recordParts(ctx, *m, from);
-    recordParts(ctx, o, to);
-    size_t bytes[2] = { 0, 0 };                                        // [0] the device residue, [1] the host body
-    for (int k = 0; k < np; k++) bytes[from[k].body] += alignUp(from[k].bytes, 256);
-    char* base[2] = { nullptr, nullptr };
-    cudaError_t e = ensureHostPool(ctx);
-    if (e == cudaSuccess) e = cudaMallocFromPoolAsync((void**)&base[1], bytes[1], ctx->hostPool, ctx->stream);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        ctx->err = "frame_offload: no host memory for frame " + std::to_string(frame_id) + " (" + cudaGetErrorString(e) +
-                   "); it stays minimized in device memory";
-        return -1;
-    }
-    e = cudaMallocFromPoolAsync((void**)&base[0], bytes[0], ctx->recordPool, ctx->stream);
-    if (e != cudaSuccess) { cudaFreeAsync(base[1], ctx->stream); LSD_CHECK(ctx, e); }
-    RecordCopy c;
-    memset(&c, 0, sizeof(c));
-    size_t off[2] = { 0, 0 };
-    for (int k = 0; k < np; k++) {
-        const int b = from[k].body;
-        *to[k].ptr = from[k].bytes ? base[b] + off[b] : nullptr;
-        addCopy(c, *from[k].ptr, *to[k].ptr, from[k].bytes);
-        off[b] += alignUp(from[k].bytes, 256);
-    }
-    const int r = launchRecordCopy(ctx, c);
-    if (r) { cudaFreeAsync(base[0], ctx->stream); cudaFreeAsync(base[1], ctx->stream); return r; }
-    LSD_CHECK(ctx, cudaFreeAsync(m->record, ctx->stream));
-    o.record = base[0]; o.recordBytes = bytes[0];
-    o.hostRecord = base[1]; o.hostRecordBytes = bytes[1];
-    *m = o;
-    return 0;
-}
-
-extern "C" int lsdgpu_frame_memory_usage(lsdgpu_ctx* ctx, int* n_device, size_t* device_bytes, int* n_host, size_t* host_bytes)
-{ LSD_LOCK(ctx);
-    int nd = 0, nh = 0;
-    size_t db = 0, hb = 0;
-    for (const auto& m : ctx->minimized) {
-        (m.hostRecord ? nh : nd)++;
-        db += m.recordBytes; hb += m.hostRecordBytes;
-    }
-    if (n_device) *n_device = nd;
-    if (device_bytes) *device_bytes = db;
-    if (n_host) *n_host = nh;
-    if (host_bytes) *host_bytes = hb;
     return 0;
 }
 
@@ -412,7 +183,7 @@ static int downloadPlane(lsdgpu_ctx* ctx, int frame_id, int what, int level, Fra
     FrameSlot* s = findFrame(ctx, frame_id);
     if (!s) return lsd_fail(ctx, "unknown frame id");
     if (level < 0 || level >= LSD_LEVELS) return lsd_fail(ctx, "bad level");
-    if (s->record && !(level == 0 && (what == LSDGPU_BUF_IMAGE || what == LSDGPU_BUF_IDEPTH || what == LSDGPU_BUF_IDEPTH_VAR))) {
+    if ((s->record[TIER_DEVICE] || s->record[TIER_HOST]) && !(level == 0 && (what == LSDGPU_BUF_IMAGE || what == LSDGPU_BUF_IDEPTH || what == LSDGPU_BUF_IDEPTH_VAR))) {
         ctx->err = "frame " + std::to_string(frame_id) + " is minimized: only image, idepth and idepthVar of level 0 are kept (lsdgpu_frame_activate it first)";
         return -2;
     }
@@ -456,7 +227,7 @@ extern "C" int lsdgpu_frame_download(lsdgpu_ctx* ctx, int frame_id, int what, in
     if (r || (r = downloadSource(ctx, s, what, level, &src))) return r;
     if (!src) { memset(out, 1, bytes); return 0; }
     // from an offloaded frame's host body the copy is host to host, which cudaMemcpyAsync need not order behind the stream
-    if (s->hostRecord) LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+    if (s->record[TIER_HOST]) LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
     LSD_CHECK(ctx, cudaMemcpyAsync(out, src, bytes, cudaMemcpyDefault, ctx->stream));
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
     return 0;

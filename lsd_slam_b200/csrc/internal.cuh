@@ -34,6 +34,8 @@ struct LevelCam {
     float K[9], KInv[9];
 };
 
+enum { TIER_DEVICE = 0, TIER_HOST = 1, TIERS = 2 };     // the memory of a minimized frame's record: device, or host (records.cu)
+
 struct FrameSlot {
     int id = -1;
     bool used = false;
@@ -61,13 +63,14 @@ struct FrameSlot {
     int parentId = -1;
     float initialTrackedResidual = 0.f;
     int numFramesTrackedOnThis = 0, numMappedOnThis = 0;
-    char* record = nullptr;              // minimized frame (lsdgpu_frame_minimize): its record, which the pointers above point into
-    size_t recordBytes = 0;
-    // offloaded frame (lsdgpu_frame_offload): the host body (image / idepth / idepthVar of level 0, the reactivation data), which
-    // those pointers point into; `record` is then the device residue (dStats, the permaRef)
-    char* hostRecord = nullptr;
-    size_t hostRecordBytes = 0;
+    // minimized frame: its record's block per tier, which the pointers above point into.  An offloaded record (lsdgpu_frame_offload)
+    // keeps the residue (dStats, the permaRef) in the device block and the body (level 0, the reactivation data) in the host block.
+    char* record[TIERS] = { nullptr, nullptr };
+    size_t recordBytes[TIERS] = { 0, 0 };
 };
+// a buffer of a frame that its minimized record keeps (recordParts, records.cu): the frame's pointer to it, its size, its tier
+struct RecordPart { char** ptr; size_t bytes; int tier; };
+#define REC_PARTS 9
 
 struct PyrPtrs {
     float* l[LSD_LEVELS];
@@ -137,11 +140,10 @@ struct lsdgpu_ctx {
     size_t arenaBytes = 0;
     std::vector<FrameSlot> slots;
     // minimized frames (Frame::minimizeInMemory): the frame's metadata, with image / idepth / idepthVar of level 0, the
-    // reactivation data, the permaRef and dStats pointing into its record and every other device pointer null.  Records come
-    // in stream order from recordPool, the host bodies of offloaded ones from hostPool (DESIGN.md section 3).
+    // reactivation data, the permaRef and dStats pointing into its record and every other device pointer null.  Records come in
+    // stream order from the pool of their tier; the host tier is pinned memory on the device's host NUMA node (DESIGN.md section 3).
     std::vector<FrameSlot> minimized;
-    cudaMemPool_t recordPool = nullptr;
-    cudaMemPool_t hostPool = nullptr;    // the host bodies of offloaded records: pinned memory on the device's host NUMA node
+    cudaMemPool_t pool[TIERS] = { nullptr, nullptr };
 
     // depth map
     HypField cur, oth;
@@ -380,7 +382,12 @@ static inline size_t alignUp(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 // ---- host helpers shared by the units of the library (each defined once, in the unit named) ---------------------------
 int ensureIdepthPyramid(lsdgpu_ctx* ctx, FrameSlot* s);     // frames.cu: levels 1..4 of a keyframe's idepth / idepthVar
-cudaError_t ensureRecordPool(lsdgpu_ctx* ctx);              // frames.cu: the context's stream-ordered memory pool (recordPool)
+// frames.cu, which compiles frame.cuh's kernels, launches them for records.cu: one k_record_copy of the parts from[k] -> to[k]
+// that have bytes, and Frame::require's image pyramid and gradients of slot `s` from the fp32 level 0 of a record
+int launchRecordCopy(lsdgpu_ctx* ctx, const RecordPart* from, const RecordPart* to, int n);
+int buildImagePyramidFromRecord(lsdgpu_ctx* ctx, FrameSlot* s, const float* image0);
+cudaError_t ensureRecordPool(lsdgpu_ctx* ctx);              // records.cu: the context's stream-ordered pool of device memory
+cudaError_t freeRecord(lsdgpu_ctx* ctx, const FrameSlot& m); // records.cu: returns a minimized frame's blocks to their pools
 cudaError_t trackPersistentSetup(lsdgpu_ctx* ctx);          // tracking.cu: launch shape of the persistent tracker
 void cloudRelease(lsdgpu_ctx* ctx);                         // output.cu: frees the point-cloud reservation
 

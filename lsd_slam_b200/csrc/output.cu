@@ -366,7 +366,7 @@ extern "C" int lsdgpu_map_export_pointcloud_device(lsdgpu_ctx* ctx, int n, const
     LSD_CHECK(ctx, ensureRecordPool(ctx));
     LSD_CHECK(ctx, afterCallerStream(ctx, stream));
     char* blk = nullptr;
-    LSD_CHECK(ctx, cudaMallocFromPoolAsync((void**)&blk, kfBytes + tabBytes + stateBytes, ctx->recordPool, ctx->stream));
+    LSD_CHECK(ctx, cudaMallocFromPoolAsync((void**)&blk, kfBytes + tabBytes + stateBytes, ctx->pool[TIER_DEVICE], ctx->stream));
     char* st = blk + kfBytes + tabBytes;
     CloudParams P;
     P.kfs = (const CloudKf*)blk;

@@ -44,7 +44,7 @@ def slot_bytes(w, h):
 
 
 def record_bytes(w, h, n_perma):
-    """a minimized keyframe with depth, reactivation data and a permaRef (csrc/frames.cu recordParts)"""
+    """a minimized keyframe with depth, reactivation data and a permaRef (csrc/records.cu recordParts)"""
     n0 = w * h
     return a256(24) + 3 * a256(n0 * 4) + 2 * a256(n0 * 4) + a256(n0) + a256(n_perma * 16) + a256(n_perma * 4)
 

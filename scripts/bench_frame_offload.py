@@ -37,7 +37,7 @@ from bench_frame_memory import KF_EVERY, _render_image, a256, run_stream  # noqa
 
 
 def body_bytes(w, h):
-    """the host body of a keyframe with depth and reactivation data (csrc/frames.cu recordParts)"""
+    """the host body of a keyframe with depth and reactivation data (csrc/records.cu recordParts)"""
     n0 = w * h
     return 5 * a256(n0 * 4) + a256(n0)
 

@@ -14,6 +14,9 @@
 //                             useSubpixelStereo useAffineLightningEstimation
 //     --reactivate K KF       before frame K: finishCurrentKeyframe, then setFromExistingKF(keyframe KF) (loadNewCurrentKeyframe)
 //     --threads               the constraint calls on a second thread fed from a queue of finished keyframes
+//     --device-records N      FrameMemory::setMaxDeviceRecords(N): pruneActiveFrames offloads the minimized records beyond N to
+//                             host memory.  stdout also gets "MEMORY n_device device_bytes n_host host_bytes"
+//                             (lsdgpu_frame_memory_usage) before setFromExistingKF and before the final DepthMap::invalidate.
 //
 // FRAMES: int32 w, h, n; float K[9]; float depth of frame 0 [w*h]; n images uint8 [w*h].  MAIN.bin and CONSTRAINTS.bin are raw
 // records (native byte order, see put* below); stdout gets the activity of the constraint calls' reference keyframes, the
@@ -228,7 +231,8 @@ int main(int argc, char** argv)
     if (argc < 4) { std::fprintf(stderr, "usage: see the head of host_slam_mode.cpp\n"); return 2; }
     const Input in = readInput(argv[1]);
     int kfEvery = 5, maxFrames = 16, prune = -1, globalsAt = -1, reactAt = -1, reactKf = -1;
-    bool threads = false;
+    bool threads = false, deviceRecordsSet = false;
+    int deviceRecords = -1;
     float gf[3] = { 0, 0, 0 };
     int gb[3] = { 0, 0, 0 };
     for (int i = 4; i < argc; i++) {
@@ -237,6 +241,7 @@ int main(int argc, char** argv)
         else if (a == "--max-frames") maxFrames = std::atoi(argv[++i]);
         else if (a == "--prune") prune = std::atoi(argv[++i]);
         else if (a == "--threads") threads = true;
+        else if (a == "--device-records") { deviceRecords = std::atoi(argv[++i]); deviceRecordsSet = true; }
         else if (a == "--reactivate") { reactAt = std::atoi(argv[i + 1]); reactKf = std::atoi(argv[i + 2]); i += 2; }
         else if (a == "--globals") {
             globalsAt = std::atoi(argv[++i]);
@@ -251,6 +256,14 @@ int main(int argc, char** argv)
     try {
         DeviceContext dev(0, in.w, in.h, in.K, maxFrames);
         if (prune >= 0) dev.frameMemory().setMaxActiveFrames(prune);
+        if (deviceRecordsSet) dev.frameMemory().setMaxDeviceRecords(deviceRecords);
+        auto reportMemory = [&] {
+            if (!deviceRecordsSet) return;
+            int nd = 0, nh = 0;
+            size_t db = 0, hb = 0;
+            dev.check(lsdgpu_frame_memory_usage(dev.raw(), &nd, &db, &nh, &hb), "lsdgpu_frame_memory_usage");
+            std::printf("MEMORY %d %zu %d %zu\n", nd, db, nh, hb);
+        };
         SE3Tracker tracker(dev, in.w, in.h, in.K);
         for (int lvl = 4; lvl < LSDGPU_LEVELS; lvl++) tracker.settings.maxItsPerLvl[lvl] = 0;     // SlamSystem.cpp:80-81
         DepthMap map(dev, in.w, in.h, in.K);
@@ -292,6 +305,7 @@ int main(int argc, char** argv)
                 finishCurrentKeyframe();
                 Frame* kf = keyframes.at(reactKf).get();
                 std::printf("REACTIVATE %d %d\n", kf->id(), kf->isActive);
+                reportMemory();
                 map.setFromExistingKF(kf);
                 current = kf;
                 putI(out, REC_REACTIVATE); putI(out, old->id()); putI(out, kf->id()); putI(out, old->permaRefNumPts);
@@ -340,6 +354,7 @@ int main(int argc, char** argv)
             printGlobals("fresh", g);
         }
         lastOwned.reset();
+        reportMemory();
         map.invalidate();
     } catch (const std::exception& e) {
         std::fprintf(stderr, "error: %s\n", e.what());

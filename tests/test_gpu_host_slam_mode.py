@@ -1,6 +1,6 @@
 """SlamSystem's SLAM mode through the C++ adapter (lsd_slam_b200/host/lsd_host.h): Frame::setPermaRef, SE3Tracker::checkPermaRefOverlap /
-trackFrameOnPermaref, DepthMap::setFromExistingKF(Frame*) and the reference's run-time globals, driven by
-tests/native/host_slam_mode.cpp in SlamSystem's order and compared bit for bit with the same calls made through abi.py.  Those ABI
+trackFrameOnPermaref, DepthMap::setFromExistingKF(Frame*), FrameMemory::setMaxDeviceRecords and the reference's run-time globals,
+driven by tests/native/host_slam_mode.cpp in SlamSystem's order and compared bit for bit with the same calls made through abi.py.  Those ABI
 calls are held to the reference's recorded values by test_gpu_sim3_motions.py / test_gpu_perma.py / test_gpu_globals.py."""
 import os
 import struct
@@ -319,6 +319,40 @@ def test_slam_mode_constraint_thread_on_one_context(runs):
     assert [t for t, _ in seq.cons_records].count(OVERLAP) == 3
     assert_same(thr.main, seq.main, "tracking and mapping")
     assert_same(thr.cons, seq.cons, "constraint calls")
+
+
+def _memory(run):
+    """the MEMORY lines of a --device-records run: (n_device, device_bytes, n_host, host_bytes) before the re-activation, if any,
+    then at the end"""
+    return [tuple(int(v) for v in ln[1:]) for ln in run.lines if ln[0] == "MEMORY"]
+
+
+@pytest.mark.gpu
+def test_setFromExistingKF_on_an_offloaded_keyframe(driver, tmp_path, seq_small, frames_small):
+    """FrameMemory::setMaxDeviceRecords(0) with two active frames: keyframe 5 is re-activated from host memory by
+    setFromExistingKF(Frame*) and tracked and mapped on; the permaRef and Sim3 calls read offloaded keyframes"""
+    react = ["--reactivate", str(REACTIVATE[0]), str(REACTIVATE[1])]
+    run = Run(driver, tmp_path, seq_small, frames_small, *react, "--prune", "2", "--device-records", "0")
+    assert ["REACTIVATE", str(REACTIVATE[1]), "0"] in run.lines
+    before, end = _memory(run)
+    assert before[0] == 0 and before[2] >= 1, before      # keyframe 5 is minimized, so its record is in host memory
+    assert end[0] == 0 and end[2] >= 2, end
+    m = AbiMirror(seq_small, frames_small, run, react=REACTIVATE)
+    assert_same(run.main, m.main, "tracking and mapping")
+    assert_same(run.cons, m.cons, "constraint calls")
+
+
+@pytest.mark.gpu
+def test_constraint_thread_with_offloaded_keyframes(driver, tmp_path, seq_small, frames_small):
+    """the constraint calls on a second thread while the main thread prunes and offloads.  Three active frames: the two frames a
+    constraint call holds and the active keyframe, so that pruning always finds a frame to minimize; which one it picks depends on
+    the threads' timing, and none of the outputs does."""
+    run = Run(driver, tmp_path, seq_small, frames_small, "--threads", "--prune", "3", "--device-records", "0")
+    (end,) = _memory(run)
+    assert end[0] == 0 and end[2] >= 1, end
+    m = AbiMirror(seq_small, frames_small, run)
+    assert_same(run.main, m.main, "tracking and mapping")
+    assert_same(run.cons, m.cons, "constraint calls")
 
 
 @pytest.mark.gpu
