@@ -422,12 +422,15 @@ extern "C" int lsdgpu_undistorter_ptam_prepare(const float ic[5], int iw, int ih
             const float c_tl = sqrtf(rl * rl + rt * rt), c_tr = sqrtf(rr * rr + rt * rt);
             const float c_bl = sqrtf(rl * rl + rb * rb), c_br = sqrtf(rr * rr + rb * rb);
             const float u_tl = undistRadius(c_tl), u_tr = undistRadius(c_tr), u_bl = undistRadius(c_bl), u_br = undistRadius(c_br);
-            const float hor = fmaxf(c_br, c_tr) + fmaxf(c_bl, c_tl), vert = fmaxf(c_tr, c_tl) + fmaxf(c_bl, c_br);
-            const float uhor = fmaxf(u_br, u_tr) + fmaxf(u_bl, u_tl), uvert = fmaxf(u_tr, u_tl) + fmaxf(u_bl, u_br);
+            // std::max(a, b) is `a < b ? b : a` (not fmaxf): a NaN first argument wins, a NaN second one loses.  With cx or
+            // cy == 0 a corner radius is 0 and u / c is 0/0; the reference's ocy (or ocx) is then NaN and every entry -1.
+            const auto stdMax = [](float a, float b) { return a < b ? b : a; };
+            const float hor = stdMax(c_br, c_tr) + stdMax(c_bl, c_tl), vert = stdMax(c_tr, c_tl) + stdMax(c_bl, c_br);
+            const float uhor = stdMax(u_br, u_tr) + stdMax(u_bl, u_tl), uvert = stdMax(u_tr, u_tl) + stdMax(u_bl, u_br);
             ofy = fy * ((vert) / (uvert)) * sy;
-            ocy = fmaxf(u_tl / c_tl, u_tr / c_tr) * ofy * cy / fy;
+            ocy = stdMax(u_tl / c_tl, u_tr / c_tr) * ofy * cy / fy;
             ofx = fx * ((hor) / (uhor)) * sx;
-            ocx = fmaxf(u_bl / c_bl, u_tl / c_tl) * ofx * cx / fx;
+            ocx = stdMax(u_bl / c_bl, u_tl / c_tl) * ofx * cx / fx;
         }
     } else {
         ofx = ocIn[0] * ow; ofy = ocIn[1] * oh;

@@ -13,8 +13,9 @@
  * Sim3Tracker.cpp, Frame.cpp, TrackingReference.cpp ... unmodified from /root/reference against stand-in headers
  * (oracle/ref_shim/: an Eigen 3.2 subset, Boost -> std, OpenCV debug stubs) into oracle/_ref/liblsd_ref.so, exported under the
  * same lsdo_* API by oracle/ref_driver.cpp; tests/test_ref_pin.py holds this restatement to it BIT FOR BIT on every function of
- * the path, and tests/golden/reference_320x240.npz are outputs of that library.  Still unpinned: UndistorterPTAM
- * (util/Undistorter.cpp needs OpenCV's remap machinery and is not part of the _ref build) -- see lsd_oracle_undistort.inc.
+ * the path, and tests/golden/reference_320x240.npz are outputs of that library.  UndistorterPTAM is pinned the same way:
+ * util/Undistorter.cpp is part of the _ref build, and tests/test_ref_pin_undistort.py holds lsd_oracle_undistort.inc and the
+ * library's table builder to it over a calibration sweep (tests/golden/ref_pin_undistort.npz).
  *
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl
  * reference legs may load this library.  The product (lsd_slam_b200/) never does.

@@ -181,6 +181,12 @@ def lib(fast=False):
     sig("lsdo_sim3_track", C.c_int, vp, vp, dp, C.c_int, C.c_int, C.POINTER(TrackSettings), C.POINTER(Sim3Result))
     sig("lsdo_undistorter_ptam_prepare", C.c_int, fp, C.c_int, C.c_int, fp, C.c_int, C.c_int, fp, fp, fp)
     sig("lsdo_undistort", None, fp, fp, C.c_int, C.c_int, C.c_int, u8p, u8p)
+    sig("lsdo_ref_undistorter_open", vp, C.c_char_p)
+    sig("lsdo_ref_undistorter_close", None, vp)
+    sig("lsdo_ref_undistorter_info", None, vp, ip, fp)
+    sig("lsdo_ref_undistorter_tables", C.c_int, vp, fp, fp)
+    sig("lsdo_ref_undistorter_undistort", C.c_int, vp, u8p, C.c_int, C.c_int, u8p, C.c_int)
+    sig("lsdo_ref_undistorter_for_file", C.c_int, C.c_char_p)
     sig("lsdo_frame_setPermaRef", C.c_int, vp, fp, fp)
     sig("lsdo_checkPermaRefOverlap", C.c_float, C.c_int, C.c_int, fp, fp, C.c_int, dp)
     sig("lsdo_trackFrameOnPermaref", C.c_int, C.c_int, C.c_int, fp, fp, C.c_int, vp, dp, C.POINTER(TrackResult))
@@ -407,7 +413,8 @@ class PermaRef:
 
 class UndistorterPTAM:
     """util/Undistorter.cpp:91-411 with the calibration file's four lines already parsed.  out_calib: "crop", "full" or
-    (fx, fy, cx, cy, 0) relative to the output size."""
+    (fx, fy, cx, cy, 0) relative to the output size.  Under a reference flavour ("ref", "ref_legacy_math", ...) the reference's
+    own class computes the tables from the same lines (oracle/ref_driver.cpp)."""
 
     def __init__(self, in_calib, in_size, out_calib, out_size, fast: bool = False):
         self.L = lib(fast)
@@ -435,6 +442,54 @@ class UndistorterPTAM:
         u8p = C.POINTER(C.c_uint8)
         self.L.lsdo_undistort(_fp(self.remapX), _fp(self.remapY), self.in_w, self.out_w, self.out_h, img.ctypes.data_as(u8p), out.ctypes.data_as(u8p))
         return out
+
+
+class RefUndistorterFile:
+    """lsd_slam::UndistorterPTAM(configFileName) of the reference itself (util/Undistorter.cpp:91-345), constructed from a
+    calibration file in zero-filled storage by oracle/_ref (flavour "ref", "ref_legacy_math" or "ref_sse").  valid, the sizes,
+    K as main_on_images.cpp:164-167 reads getK(), the tables (None when the reference built none) and undistort()."""
+
+    def __init__(self, path: str, flavour: str = "ref"):
+        self.L = lib(flavour)
+        self.ptr = self.L.lsdo_ref_undistorter_open(os.fsencode(path))
+        info = np.zeros(5, np.int32)
+        K = np.zeros(9, np.float32)
+        self.L.lsdo_ref_undistorter_info(self.ptr, info.ctypes.data_as(C.POINTER(C.c_int)), _fp(K))
+        self.valid = bool(info[0])
+        self.in_w, self.in_h, self.out_w, self.out_h = (int(v) for v in info[1:])
+        self.K = K.reshape(3, 3)
+        self.remapX = np.zeros((max(self.out_h, 0), max(self.out_w, 0)), np.float32)
+        self.remapY = np.zeros_like(self.remapX)
+        if not self.L.lsdo_ref_undistorter_tables(self.ptr, _fp(self.remapX), _fp(self.remapY)):
+            self.remapX = self.remapY = None
+
+    def undistort(self, image_u8: np.ndarray) -> np.ndarray:
+        img = np.ascontiguousarray(image_u8, np.uint8)
+        cap = max(img.size, self.out_w * self.out_h)
+        out = np.zeros(cap, np.uint8)
+        u8p = C.POINTER(C.c_uint8)
+        shape = self.L.lsdo_ref_undistorter_undistort(self.ptr, img.ctypes.data_as(u8p), img.shape[1], img.shape[0],
+                                                      out.ctypes.data_as(u8p), cap)
+        assert shape >= 0
+        return out[:(shape >> 16) * (shape & 0xFFFF)].reshape(shape >> 16, shape & 0xFFFF)
+
+    def close(self):
+        if self.ptr:
+            self.L.lsdo_ref_undistorter_close(self.ptr)
+            self.ptr = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def ref_undistorter_for_file(path: str, flavour: str = "ref") -> int:
+    """Undistorter::getUndistorterForFile (util/Undistorter.cpp:38-88) of the reference: 0 for its null result, 1 for an
+    UndistorterPTAM.  Never pass a file with 8 numbers on its first line: that constructs UndistorterOpenCV, which oracle/_ref
+    cannot run."""
+    return int(lib(flavour).lsdo_ref_undistorter_for_file(os.fsencode(path)))
 
 
 def se3_track(kf: Frame, frame: Frame, init_frameToRef_qt, settings: TrackSettings | None = None) -> TrackResult:

@@ -6,10 +6,12 @@ TEST INFRASTRUCTURE.  Compiles, UNMODIFIED and straight from /root/reference (no
     lsd_slam_core/src/Tracking/SE3Tracker.cpp, Sim3Tracker.cpp, TrackingReference.cpp      (+ LGSX.h)
     lsd_slam_core/src/DataStructures/Frame.cpp, FrameMemory.cpp, FramePoseStruct.cpp
     lsd_slam_core/src/util/settings.cpp, SophusUtil.cpp                                   (+ globalFuncs.h, IndexThreadReduce.h)
+    lsd_slam_core/src/util/Undistorter.cpp                                                (UndistorterPTAM; UndistorterOpenCV
+                                                                                           compiles but is never constructed)
     lsd_slam_core/thirdparty/Sophus/sophus/{so3,se3,rxso3,sim3}.hpp                       (vendored, header only)
 
 against the stand-in headers in oracle/ref_shim/ (a fixed-size Eigen 3.2 subset, Boost.Thread -> std::, OpenCV debug
-images, empty KeyFrameGraph / g2o declarations) plus oracle/ref_driver.cpp, which exports the reference's classes under
+images and K storage, empty KeyFrameGraph / g2o declarations, OpenCV calib3d entry points that abort if reached) plus oracle/ref_driver.cpp, which exports the reference's classes under
 the C names of oracle/lsd_oracle.h.  The reference's own build system (rosbuild + cmake + Eigen3 + SuiteSparse + X11 +
 dynamic_reconfigure, lsd_slam_core/CMakeLists.txt:3-33) cannot run in this image; this is the short recipe instead.
 
@@ -38,7 +40,7 @@ SOURCES = [
     "src/DepthEstimation/DepthMap.cpp", "src/DepthEstimation/DepthMapPixelHypothesis.cpp",
     "src/Tracking/SE3Tracker.cpp", "src/Tracking/Sim3Tracker.cpp", "src/Tracking/TrackingReference.cpp",
     "src/DataStructures/Frame.cpp", "src/DataStructures/FrameMemory.cpp", "src/DataStructures/FramePoseStruct.cpp",
-    "src/util/settings.cpp", "src/util/SophusUtil.cpp",
+    "src/util/settings.cpp", "src/util/SophusUtil.cpp", "src/util/Undistorter.cpp",
 ]
 SOPHUS_TESTS = ["so3", "se3", "sim3", "rxso3"]
 
@@ -48,7 +50,8 @@ FLAVOURS = {
     # Release build type (CMakeLists.txt:11) => NDEBUG => enablePrintDebugInfo == false (util/settings.h:44-48)
     "liblsd_ref.so": ["-O2", "-ffp-contract=off", "-fno-fast-math", "-msse2"],
     "liblsd_ref_sse.so": ["-O3", "-DENABLE_SSE", "-march=x86-64-v3", "-msse4.1", "-msse3", "-msse2", "-msse"],
-    # the scalar build as a g++ < 6 toolchain resolves the reference's unqualified sqrt() calls (see ref_shim/opencv2)
+    # the scalar build as a g++ < 6 toolchain resolves the reference's unqualified sqrt() / tan() / atan() calls (see
+    # ref_shim/opencv2)
     "liblsd_ref_legacy_math.so": ["-O2", "-ffp-contract=off", "-fno-fast-math", "-msse2", "-DLSD_REF_SHIM_LEGACY_MATH"],
 }
 
@@ -111,7 +114,7 @@ def build(force: bool = False, verbose: bool = False) -> bool:
             print(f"[ref_build] Sophus test_{t} passed")
     info = {"reference": REF, "sources": SOURCES, "flags": {k: COMMON[:5] + v for k, v in FLAVOURS.items()},
             "gxx": subprocess.run(["g++", "--version"], capture_output=True, text=True).stdout.splitlines()[0],
-            "shim": "oracle/ref_shim (Eigen 3.2 fixed-size subset, Boost.Thread -> std, OpenCV debug images)",
+            "shim": "oracle/ref_shim (Eigen 3.2 fixed-size subset, Boost.Thread -> std, OpenCV debug images and Undistorter stand-ins)",
             "sophus_tests": SOPHUS_TESTS}
     with open(os.path.join(OUT, "BUILD_INFO.json"), "w") as f:
         json.dump(info, f, indent=1)

@@ -7,6 +7,7 @@
 //   lsd_slam::SE3Tracker       Tracking/SE3Tracker.{h,cpp}, LGSX.h
 //   lsd_slam::DepthMap         DepthEstimation/DepthMap.{h,cpp}, DepthMapPixelHypothesis.{h,cpp}
 //   lsd_slam::Sim3Tracker      Tracking/Sim3Tracker.{h,cpp}
+//   lsd_slam::UndistorterPTAM  util/Undistorter.{h,cpp} (and Undistorter::getUndistorterForFile's dispatch)
 //   Sophus                     thirdparty/Sophus/sophus/{so3,se3,rxso3,sim3}.hpp (vendored, unmodified)
 // against the stand-in headers of oracle/ref_shim/ (Eigen 3.2 subset, Boost.Thread -> std, OpenCV debug images).
 // The exported names and structs are those of oracle/lsd_oracle.h, so oracle/pyoracle.py drives this library and the
@@ -38,7 +39,9 @@
 #include <chrono>
 #include <limits>
 #include <stdexcept>
+#include <new>
 #include <sys/time.h>
+#include <unistd.h>
 
 #include "Eigen/Core"                       // shim (no private members of its own that matter)
 #include "boost/thread.hpp"
@@ -56,6 +59,7 @@
 #include "Tracking/SE3Tracker.h"
 #include "Tracking/Sim3Tracker.h"
 #include "IOWrapper/ImageDisplay.h"
+#include "util/Undistorter.h"
 #undef private
 #undef protected
 
@@ -567,6 +571,133 @@ void lsdo_ref_prepareForStereoWith(lsdo_frame* frame, lsdo_frame* kf, const doub
     out[k++] = f->distSquared;
     out[k++] = (float)f->referenceID;
     out[k++] = (float)f->referenceLevel;
+}
+
+// ---- UndistorterPTAM (util/Undistorter.cpp:38-411) ----
+// The reference constructs the class from a calibration file only.  The object lives in zero-filled storage: for "none" the
+// constructor leaves outputCalibration unset (Undistorter.cpp:140-143) and reads it at :270-273, and zero is what the library's
+// adapter uses there (lsd_host.cpp), so this makes that case defined and the same on both sides.
+struct lsdo_ref_undistorter {
+    alignas(UndistorterPTAM) unsigned char storage[sizeof(UndistorterPTAM)];
+    UndistorterPTAM* u;
+};
+
+lsdo_ref_undistorter* lsdo_ref_undistorter_open(const char* path)
+{
+    lsdo_ref_undistorter* o = new lsdo_ref_undistorter;
+    std::memset(o->storage, 0, sizeof(o->storage));
+    o->u = new (o->storage) UndistorterPTAM(path);
+    return o;
+}
+void lsdo_ref_undistorter_close(lsdo_ref_undistorter* o)
+{
+    o->u->~UndistorterPTAM();
+    delete o;
+}
+// info = valid, in_w, in_h, out_w, out_h; K as main_on_images.cpp:164-167 reads getK() (float of (0,0), (1,1), (2,0), (2,1))
+void lsdo_ref_undistorter_info(const lsdo_ref_undistorter* o, int info[5], float K[9])
+{
+    const UndistorterPTAM* u = o->u;
+    info[0] = u->isValid() ? 1 : 0;
+    info[1] = u->getInputWidth(); info[2] = u->getInputHeight();
+    info[3] = u->getOutputWidth(); info[4] = u->getOutputHeight();
+    std::memset(K, 0, 9 * sizeof(float));
+    K[0] = (float)u->getK().at<double>(0, 0);
+    K[4] = (float)u->getK().at<double>(1, 1);
+    K[2] = (float)u->getK().at<double>(2, 0);
+    K[5] = (float)u->getK().at<double>(2, 1);
+    K[8] = 1;
+}
+// remapX / remapY (out_w * out_h floats each); 0 when the reference built none (an invalid file)
+int lsdo_ref_undistorter_tables(const lsdo_ref_undistorter* o, float* remapX, float* remapY)
+{
+    const UndistorterPTAM* u = o->u;
+    if (!u->remapX || !u->remapY) return 0;
+    const size_t n = (size_t)u->out_width * u->out_height;
+    std::memcpy(remapX, u->remapX, n * sizeof(float));
+    std::memcpy(remapY, u->remapY, n * sizeof(float));
+    return 1;
+}
+// undistort() of an in_h x in_w image into out (capacity `cap` bytes); returns rows * 65536 + cols of the result, which is the
+// input itself when the reference passes it through (Undistorter.cpp:357-375)
+int lsdo_ref_undistorter_undistort(const lsdo_ref_undistorter* o, const uint8_t* image, int in_w, int in_h, uint8_t* out, int cap)
+{
+    cv::Mat img(in_h, in_w, CV_8U, const_cast<uint8_t*>(image));
+    cv::Mat res;
+    o->u->undistort(img, res);
+    if ((long long)res.rows * res.cols > cap) return -1;
+    std::memcpy(out, res.data, (size_t)res.rows * res.cols);
+    return res.rows * 65536 + res.cols;
+}
+// Undistorter::getUndistorterForFile (:38-88): 0 for its null result, 1 for an UndistorterPTAM.  A file whose first line holds
+// 8 numbers constructs UndistorterOpenCV, whose OpenCV calls this library does not have: callers must not pass one.
+int lsdo_ref_undistorter_for_file(const char* path)
+{
+    Undistorter* u = Undistorter::getUndistorterForFile(path);
+    if (!u) return 0;
+    const int kind = dynamic_cast<UndistorterPTAM*>(u) ? 1 : 2;
+    delete u;
+    return kind;
+}
+
+// The C oracle's parsed-line API (oracle/lsd_oracle_undistort.inc) over the reference's class: the four lines are written to a
+// temporary file with %.9g, which sscanf("%f") reads back to the same floats, and the file goes through the constructor above.
+int lsdo_undistorter_ptam_prepare(const float inputCalibration[5], int in_width, int in_height, const float outputCalibrationIn[5],
+                                  int out_width, int out_height, float* remapX, float* remapY, float K_out[9])
+{
+    if (in_width <= 0 || in_height <= 0 || out_width <= 0 || out_height <= 0) return -1;
+    const char* tmpdir = std::getenv("TMPDIR");
+    const std::string tpl = std::string(tmpdir && *tmpdir ? tmpdir : "/tmp") + "/lsdo_undistorter_XXXXXX";
+    std::vector<char> name(tpl.begin(), tpl.end());
+    name.push_back(0);
+    const int fd = mkstemp(name.data());
+    if (fd < 0) return -1;
+    FILE* f = fdopen(fd, "w");
+    const float* ic = inputCalibration;
+    const float* oc = outputCalibrationIn;
+    std::fprintf(f, "%.9g %.9g %.9g %.9g %.9g\n%d %d\n", ic[0], ic[1], ic[2], ic[3], ic[4], in_width, in_height);
+    if (oc[0] == -1) std::fprintf(f, "crop\n");
+    else if (oc[0] == -2) std::fprintf(f, "full\n");
+    else std::fprintf(f, "%.9g %.9g %.9g %.9g %.9g\n", oc[0], oc[1], oc[2], oc[3], oc[4]);
+    std::fprintf(f, "%d %d\n", out_width, out_height);
+    std::fclose(f);
+    lsdo_ref_undistorter* o = lsdo_ref_undistorter_open(name.data());
+    unlink(name.data());
+    int info[5];
+    float K[9];
+    lsdo_ref_undistorter_info(o, info, K);
+    int status = -1;
+    if (info[0]) {
+        if (K_out) std::memcpy(K_out, K, sizeof(K));
+        if (remapX && remapY) lsdo_ref_undistorter_tables(o, remapX, remapY);
+        status = (in_height == out_height && in_width == out_width && ic[4] == 0) ? 1 : 0;
+    }
+    lsdo_ref_undistorter_close(o);
+    return status;
+}
+
+// UndistorterPTAM::undistort (:380-410) with the caller's tables.  The object is built from no file (not valid, no tables) and
+// then given the tables and sizes; undistort() addresses the input through in_width alone (:402) and compares the image's rows
+// with in_height only to refuse a wrong size, so in_height is set to the rows of the wrapper it is handed.  The distortion is
+// set non-zero so that the pass-through of :370-375 is not taken (callers handle that case themselves, as pyoracle does).
+void lsdo_undistort(const float* remapX, const float* remapY, int in_width, int out_width, int out_height,
+                    const uint8_t* image, uint8_t* data)
+{
+    lsdo_ref_undistorter* o = lsdo_ref_undistorter_open("");
+    UndistorterPTAM* u = o->u;
+    const int rows = 1;
+    u->valid = true;
+    u->in_width = in_width; u->in_height = rows;
+    u->out_width = out_width; u->out_height = out_height;
+    u->inputCalibration[4] = 1;
+    u->remapX = const_cast<float*>(remapX);
+    u->remapY = const_cast<float*>(remapY);
+    cv::Mat img(rows, in_width, CV_8U, const_cast<uint8_t*>(image));
+    cv::Mat res;
+    u->undistort(img, res);
+    std::memcpy(data, res.data, (size_t)out_width * out_height);
+    u->remapX = u->remapY = nullptr;              // the caller's arrays: not the reference's to free
+    lsdo_ref_undistorter_close(o);
 }
 
 }  // extern "C"

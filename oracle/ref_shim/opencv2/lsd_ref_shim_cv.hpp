@@ -2,7 +2,9 @@
 // The reference's hot-path sources use OpenCV only for debug images (cv::Mat members of DepthMap / SE3Tracker that are
 // written under the plot* / debug flags of util/settings.cpp, all false by default) and for display.  This header gives
 // those names a small self-contained implementation so that the reference files compile unmodified into oracle/_ref/;
-// drawing and file output are no-ops.  Nothing here takes part in any number the oracle/_ref library returns.
+// drawing and file output are no-ops.  Nothing here takes part in any number the oracle/_ref library returns, except the
+// storage of util/Undistorter.cpp's UndistorterPTAM: the CV_64F K matrices it fills through at<double>() and the CV_8U image
+// its undistort() writes through OutputArray, both plain element storage here.
 #ifndef LSD_REF_SHIM_CV
 #define LSD_REF_SHIM_CV
 #include <algorithm>
@@ -22,7 +24,8 @@
 // (DepthMap.cpp:229, 336, 1517, 1597) are float operations.  With the g++ 4.6 / 4.8 of the reference's own era
 // (Ubuntu 12.04 / 14.04, README.md) the same calls resolve to `double sqrt(double)`; only DepthMap.cpp:229
 // (`GRADIENT_SAMPLE_DIST / sqrt(eplLengthSquared)`, then evaluated in double) changes value, by <= 1 ulp.
-// -DLSD_REF_SHIM_LEGACY_MATH builds that variant (tests/test_ref_pin.py measures its distance).
+// -DLSD_REF_SHIM_LEGACY_MATH builds that variant (tests/test_ref_pin.py measures its distance).  The same switch turns the
+// unqualified tan / atan / sqrt of util/Undistorter.cpp into double operations (tests/test_ref_pin_undistort.py measures that).
 #ifndef LSD_REF_SHIM_LEGACY_MATH
 #include <math.h>
 #endif
@@ -84,6 +87,21 @@ public:
     Mat(int r, int c, int type) { create(r, c, type); }
     Mat(int r, int c, int type, void* ext) : rows(r), cols(c), data(static_cast<unsigned char*>(ext)), type_(type), esz_(elem(type)) {}
     Mat(Size s, int type) { create(s.height, s.width, type); }
+    Mat(int r, int c, int type, const Scalar& v)
+    {
+        create(r, c, type);
+        for (int i = 0; i < r * c * channels(); ++i) setElem(i, v.val[0]);
+    }
+    static Mat zeros(int r, int c, int type) { return Mat(r, c, type); }
+    bool isContinuous() const { return true; }
+    // single-channel transpose (util/Undistorter.cpp:556-557)
+    Mat t() const
+    {
+        Mat m(cols, rows, type_);
+        for (int y = 0; y < rows; ++y)
+            for (int x = 0; x < cols; ++x) std::memcpy(m.data + (static_cast<size_t>(x) * rows + y) * esz_, data + (static_cast<size_t>(y) * cols + x) * esz_, esz_);
+        return m;
+    }
     void create(int r, int c, int type)
     {
         rows = r; cols = c; type_ = type; esz_ = elem(type);
@@ -104,6 +122,15 @@ public:
     // value conversion of debug images: geometry only (contents of debug plots are not part of any returned number)
     void convertTo(Mat& dst, int type, double = 1.0, double = 0.0) const { if (&dst != this) dst.create(rows, cols, type); }
 private:
+    void setElem(int i, double v)
+    {
+        switch (type_ & 7) {
+        case CV_8U: data[i] = static_cast<unsigned char>(v); break;
+        case CV_32F: reinterpret_cast<float*>(data)[i] = static_cast<float>(v); break;
+        case CV_64F: reinterpret_cast<double*>(data)[i] = v; break;
+        default: std::abort();
+        }
+    }
     static int elem(int type) { static const int dsz[8] = {1, 1, 2, 2, 4, 4, 8, 2}; return dsz[type & 7] * ((type >> 3) + 1); }
     int type_, esz_;
     std::shared_ptr<std::vector<unsigned char> > own_;
@@ -130,5 +157,24 @@ inline int waitKey(int = 0) { return -1; }
 inline void namedWindow(const std::string&, int = 0) {}
 inline void destroyAllWindows() {}
 inline void resize(const Mat& s, Mat& d, Size sz, double = 0, double = 0, int = 1) { d.create(sz.height, sz.width, s.type()); }
+
+// the output-argument proxy of Undistorter::undistort (util/Undistorter.h:39): getMatRef() and create() of the wrapped Mat
+class _OutputArray {
+public:
+    _OutputArray(Mat& m) : m_(&m) {}
+    Mat& getMatRef() const { return *m_; }
+    void create(int r, int c, int type) const { m_->create(r, c, type); }
+private:
+    Mat* m_;
+};
+typedef const _OutputArray& OutputArray;
+
+// UndistorterOpenCV::undistort (Undistorter.cpp:564-567) is compiled but never run from oracle/_ref: reaching it is a bug
+enum { INTER_LINEAR = 1 };
+inline void remap(const Mat&, OutputArray, const Mat&, const Mat&, int, int = 0, const Scalar& = Scalar())
+{
+    std::fprintf(stderr, "oracle/ref_shim: cv::remap is not implemented (UndistorterOpenCV is not part of oracle/_ref)\n");
+    std::abort();
+}
 }  // namespace cv
 #endif

@@ -6,8 +6,9 @@
                             reproduce them bit for bit (tests/test_oracle_kats.py) and the CUDA path is compared with them on the
                             GPU (tests/test_gpu_golden.py).  Needs /root/reference (present in the build container only).
   oracle_8f_320x240.npz     Sim3 entries from the reference-compiled library as above; keyframeMsg packing, re-activation data and
-                            UndistorterPTAM from the C oracle (their reference sources need ROS message headers / OpenCV remap and
-                            are not part of oracle/_ref).
+                            UndistorterPTAM from the C oracle (the packing's reference sources need ROS message headers; the
+                            UndistorterPTAM entries are pinned to the reference's own Undistorter.cpp separately, by
+                            ref_pin_undistort.npz: python -m tests.golden.make_golden_ref_pin_undistort).
   ref_pin_320x240.npz       the reference-compiled side of every comparison of tests/test_ref_pin.py (digests of the bit-exact
                             observations, values of the others).
   reference_line_counts.json  line count of every source file of the reference, by path relative to its root: what
