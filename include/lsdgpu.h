@@ -276,6 +276,37 @@ int lsdgpu_set_undistorter_opencv(lsdgpu_ctx* ctx, int in_width, int in_height, 
 /* UndistorterPTAM::undistort, util/Undistorter.cpp:355-411, or UndistorterOpenCV::undistort (:564-567, cv::remap INTER_LINEAR
  * with a constant 0 border), whichever is installed: raw (in_width*in_height) -> out (w*h), 8 bit */
 int lsdgpu_undistort_u8(lsdgpu_ctx* ctx, const uint8_t* raw, uint8_t* out);
+/* ---- input staging: the camera's pixel format (cv_bridge::toCvCopy(img, MONO8), ROSImageStreamThread.cpp:117, and
+ * LiveSLAMWrapper::newImageCallback's cvtColor(img, grayImg, CV_RGB2GRAY), LiveSLAMWrapper.cpp:116-121) fused in front of the
+ * undistorter.  Found by symbol lookup (dlsym), like lsdgpu_track_and_map_group; LSDGPU_ABI_VERSION is unchanged.
+ * The formats are named after the ROS image encodings.  Every raw pixel is converted to 8-bit gray as OpenCV 4.13's cv::cvtColor
+ * does, bit for bit, before the undistorter reads it:
+ *   RGB8 / RGBA8   COLOR_RGB2GRAY  (R * 9798 + G * 19235 + B * 3735 + 16384) >> 15  (alpha ignored)
+ *   BGR8 / BGRA8   COLOR_BGR2GRAY  the same with R and B swapped
+ *   YUV422         COLOR_YUV2GRAY_UYVY  byte 1 of each 2-byte pixel     YUV422_YUY2  COLOR_YUV2GRAY_YUY2  byte 0 */
+enum {
+    LSDGPU_PIX_MONO8 = 0,               /* 1 byte per pixel (the default) */
+    LSDGPU_PIX_RGB8 = 1,                /* 3 */
+    LSDGPU_PIX_BGR8 = 2,                /* 3 */
+    LSDGPU_PIX_RGBA8 = 3,               /* 4 */
+    LSDGPU_PIX_BGRA8 = 4,               /* 4 */
+    LSDGPU_PIX_YUV422 = 5,              /* 2, U Y0 V Y1 (UYVY) */
+    LSDGPU_PIX_YUV422_YUY2 = 6          /* 2, Y0 U Y1 V */
+};
+/* The pixel format of the installed undistorter's raw images (in_width x in_height pixels, in_width * bytes_per_pixel bytes per
+ * row on the host).  Needs an undistorter (lsdgpu_set_undistorter, the pass-through one included, or lsdgpu_set_undistorter_opencv);
+ * the format persists when another undistorter is installed.  It applies to lsdgpu_undistort_u8, lsdgpu_frame_upload_distorted_u8,
+ * lsdgpu_frame_upload_distorted_device_u8 (whose pitch must then be >= in_width * bytes_per_pixel) and lsdgpu_stage_put_raw*.
+ * Rejected, changing nothing: an unknown format, no undistorter, a 4:2:2 format with an odd in_width (installing an undistorter of
+ * odd in_width while a 4:2:2 format is set is rejected too).  MONO8 gives exactly the behaviour without this call. */
+int lsdgpu_set_input_format(lsdgpu_ctx* ctx, int format);
+/* Camera image in, prefetch-ring entry out: converts raw (HOST, in the input format, of the installed undistorter's input size),
+ * undistorts it and writes the w x h gray result into ring entry `index` -- what lsdgpu_stage_put would store after a host
+ * cvtColor + undistort.  Waits for the device, as lsdgpu_stage_put does. */
+int lsdgpu_stage_put_raw(lsdgpu_ctx* ctx, int index, const uint8_t* raw);
+/* The same from a DEVICE raw image with row pitch pitch_bytes >= in_width * bytes_per_pixel, ordered on the caller's stream and
+ * without waiting for the device, as the *_device entry points below: every argument is checked before anything changes. */
+int lsdgpu_stage_put_raw_device(lsdgpu_ctx* ctx, int index, const uint8_t* d_raw, size_t pitch_bytes, void* stream);
 /* undistort + Frame::Frame(id, w, h, K, ts, const uchar*) + buildImage/buildGradients/buildMaxGradients of all levels:
  * the raw image is copied to the device once and the remap feeds the pyramid kernel directly
  * (main_on_images.cpp:238-244: undistorter->undistort(imageDist, image); system->trackFrame(image.data, ...)) */

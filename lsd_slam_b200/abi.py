@@ -229,6 +229,9 @@ SYMBOLS = [
     ("lsdgpu_frame_upload_device_u8", C.c_int, [_vp, C.c_int, _vp, C.c_size_t, _vp]),
     ("lsdgpu_frame_upload_distorted_device_u8", C.c_int, [_vp, C.c_int, _vp, C.c_size_t, _vp]),
     ("lsdgpu_stage_put_device", C.c_int, [_vp, C.c_int, _vp, C.c_size_t, _vp]),
+    ("lsdgpu_set_input_format", C.c_int, [_vp, C.c_int]),
+    ("lsdgpu_stage_put_raw", C.c_int, [_vp, C.c_int, C.POINTER(C.c_uint8)]),
+    ("lsdgpu_stage_put_raw_device", C.c_int, [_vp, C.c_int, _vp, C.c_size_t, _vp]),
     ("lsdgpu_frame_download_device", C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_size_t, _vp]),
     ("lsdgpu_map_export_pointcloud_device", C.c_int, [_vp, C.c_int, _ip, _fp, C.c_int, C.c_void_p, C.c_int, _vp, C.c_int64,
                                                       C.POINTER(C.c_int64), C.POINTER(C.c_int32), _vp]),
@@ -360,6 +363,12 @@ def hyp_fields(t) -> dict:
     return out
 
 
+# the camera's raw pixel formats (LSDGPU_PIX_*), by ROS image encoding: (format, bytes per pixel).  Context.set_input_format selects
+# one; the device converts each raw pixel as OpenCV 4.13's cv::cvtColor(.., COLOR_RGB2GRAY / BGR2GRAY / YUV2GRAY_UYVY / _YUY2) does.
+INPUT_FORMATS = {"mono8": (0, 1), "rgb8": (1, 3), "bgr8": (2, 3), "rgba8": (3, 4), "bgra8": (4, 4), "yuv422": (5, 2),
+                 "yuv422_yuy2": (6, 2)}
+
+
 class UndistorterPTAM:
     """Mirror of lsd_slam::UndistorterPTAM (util/Undistorter.h:96-160) with the calibration file's lines already parsed.
     out_calib: "crop", "full" or (fx, fy, cx, cy, 0).  Host-only; `install(ctx)` puts the tables on the device."""
@@ -443,6 +452,8 @@ def default_track_settings(main_tracker: bool = True) -> TrackSettings:
 
 class Context:
     """One device context = the device state of one SlamSystem (frames + one tracker + one depth map)."""
+
+    input_format = "mono8"                    # ROS encoding of the installed undistorter's raw images (set_input_format)
 
     def __init__(self, w: int, h: int, K: np.ndarray, device: int = 0, max_frames: int = 8, **globals_kw):
         self.L = load()
@@ -663,23 +674,73 @@ class Context:
         self._ck(self.L.lsdgpu_frame_get_depth_stats(self.ptr, fid, None, None, C.byref(f)))
         return bool(f.value)
 
+    def set_input_format(self, encoding: str):
+        """the ROS image encoding of the installed undistorter's raw images (lsdgpu_set_input_format): "mono8" (the default),
+        "rgb8", "bgr8", "rgba8", "bgra8", "yuv422" (UYVY) or "yuv422_yuy2".  undistort, upload_distorted and stage_put_raw then take
+        (h, w, 3 | 4 | 2) images and convert them to gray as cv_bridge / cv::cvtColor does (ROSImageStreamThread.cpp:117)"""
+        if encoding not in INPUT_FORMATS:
+            raise ValueError(f"set_input_format: unknown encoding {encoding!r}, not one of {sorted(INPUT_FORMATS)}")
+        self._ck(self.L.lsdgpu_set_input_format(self.ptr, INPUT_FORMATS[encoding][0]))
+        self.input_format = encoding
+
+    def _raw_shape(self, what: str) -> tuple:
+        """the array shape of one raw image in the input format: (h, w) for mono8, (h, w, bytes per pixel) otherwise"""
+        if self.raw_size is None:
+            raise ValueError(f"{what}: no undistorter installed")
+        (w, h), bpp = self.raw_size, INPUT_FORMATS[self.input_format][1]
+        return (h, w) if bpp == 1 else (h, w, bpp)
+
+    def _host_raw(self, raw, what: str) -> np.ndarray:
+        raw = np.ascontiguousarray(raw, np.uint8)
+        shape = self._raw_shape(what)
+        if raw.shape != shape:
+            raise ValueError(f"{what}: a {self.input_format} image needs shape {shape}, not {raw.shape}")
+        return raw
+
+    def _device_raw(self, t, what: str):
+        """a CUDA uint8 tensor of the raw shape whose pixels are contiguous within each row -> (pointer, row pitch in bytes, stream)"""
+        _tensor_dtype(t, "uint8", what)
+        shape = self._raw_shape(what)
+        if tuple(t.shape) != shape:
+            raise ValueError(f"{what}: a {self.input_format} tensor needs shape {shape}, not {tuple(t.shape)}")
+        row = shape[1] * (shape[2] if len(shape) == 3 else 1)
+        if t.stride(1) != (shape[2] if len(shape) == 3 else 1) or (len(shape) == 3 and t.stride(2) != 1) or t.stride(0) < row:
+            raise ValueError(f"{what}: needs contiguous rows (stride(0) >= {row} bytes), not strides {t.stride()}")
+        return t.data_ptr(), t.stride(0), _cuda_stream(t, self.device, what)
+
+    def stage_put_raw(self, index: int, raw):
+        """camera image in, prefetch-ring entry out: converts (input format), undistorts and writes the gray result into ring entry
+        `index` (lsdgpu_stage_put_raw); a CUDA tensor is read on the device, ordered on its current stream, without waiting for the
+        device (lsdgpu_stage_put_raw_device)"""
+        if _is_tensor(raw):
+            ptr, pitch, stream = self._device_raw(raw, "stage_put_raw")
+            self._ck(self.L.lsdgpu_stage_put_raw_device(self.ptr, index, ptr, pitch, stream))
+            return
+        img = self._host_raw(raw, "stage_put_raw")
+        self._ck(self.L.lsdgpu_stage_put_raw(self.ptr, index, img.ctypes.data_as(C.POINTER(C.c_uint8))))
+
     def undistort(self, raw_u8: np.ndarray) -> np.ndarray:
-        """UndistorterPTAM::undistort (Undistorter.cpp:355-411) or UndistorterOpenCV::undistort (:564-567), whichever is installed"""
-        raw = np.ascontiguousarray(raw_u8, np.uint8)
+        """UndistorterPTAM::undistort (Undistorter.cpp:355-411) or UndistorterOpenCV::undistort (:564-567), whichever is installed,
+        of a raw image in the input format (converted to gray first)"""
+        raw = np.ascontiguousarray(raw_u8, np.uint8) if self.input_format == "mono8" else self._host_raw(raw_u8, "undistort")
         out = np.zeros((self.h, self.w), np.uint8)
         self._ck(self.L.lsdgpu_undistort_u8(self.ptr, raw.ctypes.data_as(C.POINTER(C.c_uint8)), out.ctypes.data_as(C.POINTER(C.c_uint8))))
         return out
 
     def upload_distorted(self, fid: int, raw_u8):
         """undistort (either model) + Frame construction fused (one H2D copy of the raw image, remap feeds the pyramid kernel).
-        raw_u8 may be a CUDA tensor as `upload` takes it, of the undistorter's input size (lsdgpu_frame_upload_distorted_device_u8)"""
+        raw_u8 may be a CUDA tensor as `upload` takes it, of the undistorter's input size (lsdgpu_frame_upload_distorted_device_u8).
+        In another input format than mono8 (set_input_format) the image is (h, w, bytes per pixel), converted to gray on the device."""
         if _is_tensor(raw_u8):
             if self.raw_size is None:
                 raise ValueError("upload_distorted: no undistorter installed")
-            ptr, pitch, stream = _device_image(raw_u8, self.device, *self.raw_size, "upload_distorted")
+            if self.input_format == "mono8":
+                ptr, pitch, stream = _device_image(raw_u8, self.device, *self.raw_size, "upload_distorted")
+            else:
+                ptr, pitch, stream = self._device_raw(raw_u8, "upload_distorted")
             self._ck(self.L.lsdgpu_frame_upload_distorted_device_u8(self.ptr, fid, ptr, pitch, stream))
             return
-        raw = np.ascontiguousarray(raw_u8, np.uint8)
+        raw = np.ascontiguousarray(raw_u8, np.uint8) if self.input_format == "mono8" else self._host_raw(raw_u8, "upload_distorted")
         self._ck(self.L.lsdgpu_frame_upload_distorted_u8(self.ptr, fid, raw.ctypes.data_as(C.POINTER(C.c_uint8))))
 
     def pack_pointcloud(self, kf_id: int, level: int = 0, out=None):

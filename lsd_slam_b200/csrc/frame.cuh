@@ -23,6 +23,27 @@
 // UndistorterOpenCV's fixed-point remap (remapPixelOpenCV, maps map1 / map2, raw image in_w x in_h).
 // `pitch` is the row stride of the source image in bytes: its width for the library's own staging copies, any value >= the
 // width for a caller's device image (lsdgpu_frame_upload_device_u8 and its siblings; it may be odd, so loads are bytewise).
+// The camera's raw pixel formats (LSDGPU_PIX_*, include/lsdgpu.h): bytes per pixel, and the 8-bit gray value of the pixel whose
+// first byte is p, as cv_bridge::toCvCopy(img, MONO8) (IOWrapper/ROS/ROSImageStreamThread.cpp:117) and LiveSLAMWrapper's
+// cvtColor(img, grayImg, CV_RGB2GRAY) (LiveSLAMWrapper.cpp:116-121) compute it with OpenCV 4.13: COLOR_RGB2GRAY is
+// (R * 9798 + G * 19235 + B * 3735 + 2^14) >> 15 for every colour (BGR swaps R and B, the 4-channel formats ignore alpha),
+// COLOR_YUV2GRAY_UYVY / _YUY2 take the luma byte of each 2-byte pixel.  Integer arithmetic, bytewise loads (the pitch may be odd).
+__host__ __device__ constexpr int pixBytes(int fmt)
+{
+    return fmt == LSDGPU_PIX_RGB8 || fmt == LSDGPU_PIX_BGR8 ? 3 : fmt == LSDGPU_PIX_RGBA8 || fmt == LSDGPU_PIX_BGRA8 ? 4
+         : fmt == LSDGPU_PIX_YUV422 || fmt == LSDGPU_PIX_YUV422_YUY2 ? 2 : 1;
+}
+template <int FMT>
+__device__ __forceinline__ int grayOf(const uint8_t* __restrict__ p)
+{
+    if (FMT == LSDGPU_PIX_RGB8 || FMT == LSDGPU_PIX_RGBA8) return (__ldg(p) * 9798 + __ldg(p + 1) * 19235 + __ldg(p + 2) * 3735 + (1 << 14)) >> 15;
+    if (FMT == LSDGPU_PIX_BGR8 || FMT == LSDGPU_PIX_BGRA8) return (__ldg(p + 2) * 9798 + __ldg(p + 1) * 19235 + __ldg(p) * 3735 + (1 << 14)) >> 15;
+    if (FMT == LSDGPU_PIX_YUV422) return __ldg(p + 1);
+    return __ldg(p);                                       // MONO8, YUV422_YUY2
+}
+// FMT = the raw image's pixel format: each of the four taps reads the converted value of its source pixel (conversion before the
+// undistorter, as ROSImageStreamThread::vidCb orders them).  `pitch` is in bytes.
+template <int FMT = LSDGPU_PIX_MONO8>
 __device__ __forceinline__ unsigned char undistortPixel(const uint8_t* __restrict__ raw, int pitch, float xx, float yy)
 {
     if (xx < 0) return 0;
@@ -30,33 +51,43 @@ __device__ __forceinline__ unsigned char undistortPixel(const uint8_t* __restric
     xx -= xxi;
     yy -= yyi;
     const float xxyy = xx * yy;
-    const uint8_t* src = raw + xxi + yyi * pitch;
-    const float v = xxyy * src[1 + pitch] + (yy - xxyy) * src[pitch] + (xx - xxyy) * src[1] + (1 - xx - yy + xxyy) * src[0];
+    if (FMT == LSDGPU_PIX_MONO8) {
+        const uint8_t* src = raw + xxi + yyi * pitch;
+        const float v = xxyy * src[1 + pitch] + (yy - xxyy) * src[pitch] + (xx - xxyy) * src[1] + (1 - xx - yy + xxyy) * src[0];
+        return (unsigned char)v;
+    }
+    constexpr int B = pixBytes(FMT);
+    const uint8_t* src = raw + xxi * B + yyi * pitch;
+    const float v = xxyy * grayOf<FMT>(src + B + pitch) + (yy - xxyy) * grayOf<FMT>(src + pitch) + (xx - xxyy) * grayOf<FMT>(src + B)
+                  + (1 - xx - yy + xxyy) * grayOf<FMT>(src);
     return (unsigned char)v;
 }
 // UndistorterOpenCV::undistort (util/Undistorter.cpp:564-567) = cv::remap(image, result, map1, map2, INTER_LINEAR) with the default
 // BORDER_CONSTANT border (value 0) on u8: map1 = the integer source position (sx, sy), map2 = its 5-bit fractions (fy << 5 | fx).
 // The 2x2 weights are OpenCV's 15-bit fixed-point bilinear table, (32 - fx) * (32 - fy) * 32 ... (exact, they sum to 32768); a
 // tap outside the in_w x in_h image contributes 0; the sum is rounded as OpenCV's fixed-point cast, (sum + 2^14) >> 15.  Every
-// tap is bounds-checked, so any pair of maps is safe to install.
+// tap is bounds-checked, so any pair of maps is safe to install.  FMT as for undistortPixel.
+template <int FMT = LSDGPU_PIX_MONO8>
 __device__ __forceinline__ unsigned char remapPixelOpenCV(const uint8_t* __restrict__ raw, int in_w, int in_h, int pitch, short2 m1,
                                                           unsigned int m2)
 {
+    constexpr int B = pixBytes(FMT);
     const int sx = m1.x, sy = m1.y;
     const int fx = m2 & 31, fy = (m2 >> 5) & 31;          // cv::remap reads map2 & (INTER_TAB_SIZE2 - 1)
     const bool x0 = sx >= 0 && sx < in_w, x1 = sx + 1 >= 0 && sx + 1 < in_w;
     const bool y0 = sy >= 0 && sy < in_h, y1 = sy + 1 >= 0 && sy + 1 < in_h;
-    const uint8_t* s = raw + (ptrdiff_t)sy * pitch + sx;
-    const int p00 = (x0 && y0) ? __ldg(s) : 0, p01 = (x1 && y0) ? __ldg(s + 1) : 0;
-    const int p10 = (x0 && y1) ? __ldg(s + pitch) : 0, p11 = (x1 && y1) ? __ldg(s + pitch + 1) : 0;
+    const uint8_t* s = raw + (ptrdiff_t)sy * pitch + (ptrdiff_t)sx * B;
+    const int p00 = (x0 && y0) ? grayOf<FMT>(s) : 0, p01 = (x1 && y0) ? grayOf<FMT>(s + B) : 0;
+    const int p10 = (x0 && y1) ? grayOf<FMT>(s + pitch) : 0, p11 = (x1 && y1) ? grayOf<FMT>(s + pitch + B) : 0;
     const int v = p00 * ((32 - fx) * (32 - fy) * 32) + p01 * (fx * (32 - fy) * 32) + p10 * ((32 - fx) * fy * 32) + p11 * (fx * fy * 32);
     return (unsigned char)((v + (1 << 14)) >> 15);
 }
 // source of level 0 of k_image_pyramid: the u8 image itself, or a raw image through UndistorterPTAM's / UndistorterOpenCV's tables,
 // or (PYR_F32) the fp32 level 0 kept in a minimized frame's record (Frame::require after minimizeInMemory, Frame.cpp:319-338)
 enum { PYR_U8 = 0, PYR_PTAM = 1, PYR_OPENCV = 2, PYR_F32 = 3 };
-// src_pitch = the row stride in bytes of src (PYR_U8, PYR_PTAM, PYR_OPENCV); PYR_F32 reads w floats per row.
-template <int SRC>
+// src_pitch = the row stride in bytes of src (PYR_U8, PYR_PTAM, PYR_OPENCV); PYR_F32 reads w floats per row.  FMT = the pixel
+// format of src (PYR_U8 with another format than MONO8 is the pass-through undistorter fed a colour or 4:2:2 camera image).
+template <int SRC, int FMT = LSDGPU_PIX_MONO8>
 __global__ void __launch_bounds__(256) k_image_pyramid(const uint8_t* __restrict__ src, int src_pitch, PyrPtrs p, int w, int h,
                                                        const float* __restrict__ remapX = nullptr, const float* __restrict__ remapY = nullptr,
                                                        int in_w = 0, uint8_t* __restrict__ undist = nullptr,
@@ -71,12 +102,14 @@ __global__ void __launch_bounds__(256) k_image_pyramid(const uint8_t* __restrict
     if (SRC == PYR_F32)
         v = reinterpret_cast<const float*>(src)[y * w + x];
     else if (SRC != PYR_U8) {
-        const unsigned char u = SRC == PYR_PTAM ? undistortPixel(src, src_pitch, __ldg(remapX + y * w + x), __ldg(remapY + y * w + x))
-                                                : remapPixelOpenCV(src, in_w, in_h, src_pitch, map1[y * w + x], __ldg(map2 + y * w + x));
+        const unsigned char u = SRC == PYR_PTAM ? undistortPixel<FMT>(src, src_pitch, __ldg(remapX + y * w + x), __ldg(remapY + y * w + x))
+                                                : remapPixelOpenCV<FMT>(src, in_w, in_h, src_pitch, map1[y * w + x], __ldg(map2 + y * w + x));
         if (undist) undist[y * w + x] = u;
         v = (float)u;
-    } else
+    } else if (FMT == LSDGPU_PIX_MONO8)
         v = (float)src[y * src_pitch + x];
+    else
+        v = (float)grayOf<FMT>(src + y * src_pitch + x * pixBytes(FMT));
     p.l[0][y * w + x] = v;
     s0[ty][tx] = v;
     __syncthreads();
@@ -263,20 +296,31 @@ __global__ void __launch_bounds__(256) k_idepth_pyramid(PyrPtrs id, PyrPtrs var,
     }
 }
 
-// UndistorterPTAM::undistort alone (u8 -> u8), util/Undistorter.cpp:380-410
-__global__ void __launch_bounds__(256) k_undistort(const uint8_t* __restrict__ raw, int in_w, const float* __restrict__ remapX,
+// UndistorterPTAM::undistort alone (u8 -> u8), util/Undistorter.cpp:380-410; `pitch` = the raw image's row stride in bytes
+template <int FMT = LSDGPU_PIX_MONO8>
+__global__ void __launch_bounds__(256) k_undistort(const uint8_t* __restrict__ raw, int pitch, const float* __restrict__ remapX,
                                                    const float* __restrict__ remapY, int n, uint8_t* __restrict__ out)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = undistortPixel(raw, in_w, __ldg(remapX + i), __ldg(remapY + i));
+    if (i < n) out[i] = undistortPixel<FMT>(raw, pitch, __ldg(remapX + i), __ldg(remapY + i));
 }
 
-// UndistorterOpenCV::undistort alone (u8 -> u8), util/Undistorter.cpp:564-567
+// UndistorterOpenCV::undistort alone (u8 -> u8), util/Undistorter.cpp:564-567; the raw image's rows are in_w pixels apart
+template <int FMT = LSDGPU_PIX_MONO8>
 __global__ void __launch_bounds__(256) k_undistort_opencv(const uint8_t* __restrict__ raw, int in_w, int in_h, const short2* __restrict__ map1,
                                                           const uint16_t* __restrict__ map2, int n, uint8_t* __restrict__ out)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = remapPixelOpenCV(raw, in_w, in_h, in_w, map1[i], __ldg(map2 + i));
+    if (i < n) out[i] = remapPixelOpenCV<FMT>(raw, in_w, in_h, in_w * pixBytes(FMT), map1[i], __ldg(map2 + i));
+}
+
+// the pass-through undistorter (Undistorter.cpp:370-375) fed a colour or 4:2:2 image: cvtColor alone, w x h pixels, `pitch` bytes
+// per raw row
+template <int FMT>
+__global__ void __launch_bounds__(256) k_to_gray(const uint8_t* __restrict__ raw, int pitch, int w, int n, uint8_t* __restrict__ out)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = (uint8_t)grayOf<FMT>(raw + (i / w) * pitch + (i % w) * pixBytes(FMT));
 }
 
 // The copies of lsdgpu_frame_minimize (slot -> record) and lsdgpu_frame_activate (record -> slot): up to REC_MAX_SEGS buffers of

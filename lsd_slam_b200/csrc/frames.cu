@@ -4,6 +4,7 @@
 #include <cfloat>
 #include <climits>
 #include <cmath>
+#include <type_traits>
 
 #include "internal.cuh"
 #include "frame.cuh"
@@ -32,7 +33,23 @@ static FrameSlot* acquireSlot(lsdgpu_ctx* ctx, int id)
     return nullptr;
 }
 
-static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int pitch, int src = PYR_U8);
+static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int pitch, int src = PYR_U8,
+                                  int fmt = LSDGPU_PIX_MONO8);
+
+// f(std::integral_constant<int, FMT>()) for the pixel format fmt (LSDGPU_PIX_*): picks the kernels' FMT instantiation
+template <typename F>
+static void withFormat(int fmt, F&& f)
+{
+    switch (fmt) {
+    case LSDGPU_PIX_RGB8: f(std::integral_constant<int, LSDGPU_PIX_RGB8>()); break;
+    case LSDGPU_PIX_BGR8: f(std::integral_constant<int, LSDGPU_PIX_BGR8>()); break;
+    case LSDGPU_PIX_RGBA8: f(std::integral_constant<int, LSDGPU_PIX_RGBA8>()); break;
+    case LSDGPU_PIX_BGRA8: f(std::integral_constant<int, LSDGPU_PIX_BGRA8>()); break;
+    case LSDGPU_PIX_YUV422: f(std::integral_constant<int, LSDGPU_PIX_YUV422>()); break;
+    case LSDGPU_PIX_YUV422_YUY2: f(std::integral_constant<int, LSDGPU_PIX_YUV422_YUY2>()); break;
+    default: f(std::integral_constant<int, LSDGPU_PIX_MONO8>()); break;
+    }
+}
 
 extern "C" int lsdgpu_frame_upload_u8(lsdgpu_ctx* ctx, int frame_id, const uint8_t* gray)
 { LSD_LOCK(ctx);
@@ -110,18 +127,24 @@ extern "C" int lsdgpu_stage_put_device(lsdgpu_ctx* ctx, int index, const uint8_t
     return 0;
 }
 
-// k_image_pyramid<src> from `dsrc` (`pitch` bytes per row), then k_gradients, over the buffers of slot `s`
-static int buildImagePyramid(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int pitch, int src)
+// k_image_pyramid<src, fmt> from `dsrc` (`pitch` bytes per row, pixels of format fmt), then k_gradients, over the buffers of slot `s`
+static int buildImagePyramid(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int pitch, int src, int fmt = LSDGPU_PIX_MONO8)
 {
     const int w = ctx->w, h = ctx->h;
     PyrPtrs pp;
     for (int l = 0; l < LSD_LEVELS; l++) pp.l[l] = s->image[l];
-    if (src == PYR_PTAM) k_image_pyramid<PYR_PTAM><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h, ctx->dRemapX, ctx->dRemapY, ctx->rawW, nullptr);
-    else if (src == PYR_OPENCV)
-        k_image_pyramid<PYR_OPENCV><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h, nullptr, nullptr, ctx->rawW,
-                                                                                   nullptr, ctx->dCvMap1, ctx->dCvMap2, ctx->rawH);
-    else if (src == PYR_F32) k_image_pyramid<PYR_F32><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h);
-    else k_image_pyramid<PYR_U8><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h);
+    if (src == PYR_F32) k_image_pyramid<PYR_F32><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h);
+    else
+        withFormat(fmt, [&](auto f) {
+            constexpr int F = decltype(f)::value;
+            if (src == PYR_PTAM)
+                k_image_pyramid<PYR_PTAM, F><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h, ctx->dRemapX, ctx->dRemapY,
+                                                                                           ctx->rawW, nullptr);
+            else if (src == PYR_OPENCV)
+                k_image_pyramid<PYR_OPENCV, F><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h, nullptr, nullptr, ctx->rawW,
+                                                                                             nullptr, ctx->dCvMap1, ctx->dCvMap2, ctx->rawH);
+            else k_image_pyramid<PYR_U8, F><<<dim3(w / 16, h / 16), 256, 0, ctx->stream>>>(dsrc, pitch, pp, w, h);
+        });
     LAUNCH(ctx);
     GradPtrs gp;
     for (int l = 0; l < LSD_LEVELS; l++) { gp.img[l] = s->image[l]; gp.grad[l] = s->grad[l]; gp.w[l] = w >> l; gp.h[l] = h >> l; }
@@ -133,10 +156,10 @@ static int buildImagePyramid(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc,
     return 0;
 }
 
-// dsrc: the u8 image (PYR_U8) or the raw image (PYR_PTAM, PYR_OPENCV), `pitch` bytes per row
-static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int pitch, int src)
+// dsrc: the u8 image (PYR_U8) or the raw image (PYR_PTAM, PYR_OPENCV), `pitch` bytes per row, pixels of format fmt
+static int buildFrameFromDeviceU8(lsdgpu_ctx* ctx, FrameSlot* s, const uint8_t* dsrc, int pitch, int src, int fmt)
 {
-    const int r = buildImagePyramid(ctx, s, dsrc, pitch, src);
+    const int r = buildImagePyramid(ctx, s, dsrc, pitch, src, fmt);
     if (!r) { s->hasDepth = false; s->idepthPyrValid = false; s->hasGoodMask = false; }
     return r;
 }
@@ -489,11 +512,28 @@ static void releaseUndistorter(lsdgpu_ctx* ctx)
     ctx->undistorterSet = false;
 }
 
+// 0 if raw images of in_width pixels can have format fmt: the 4:2:2 formats pair the pixels of a row
+static int checkFormatWidth(lsdgpu_ctx* ctx, int fmt, int in_width)
+{
+    if ((fmt == LSDGPU_PIX_YUV422 || fmt == LSDGPU_PIX_YUV422_YUY2) && in_width % 2) {
+        char msg[160];
+        snprintf(msg, sizeof(msg), "a 4:2:2 input format needs an even input width, not %d", in_width);
+        return lsd_fail(ctx, msg);
+    }
+    return 0;
+}
+// bytes of one raw image of the installed undistorter in the input format (the host staging's size and a host image's)
+static size_t rawBytes(const lsdgpu_ctx* ctx)
+{
+    return (size_t)ctx->rawW * ctx->rawH * pixBytes(ctx->inputFormat);
+}
+
 extern "C" int lsdgpu_set_undistorter(lsdgpu_ctx* ctx, int in_width, int in_height, const float* remapX, const float* remapY)
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     if (in_width <= 0 || in_height <= 0) return lsd_fail(ctx, "bad input size");
-    const size_t n = (size_t)ctx->w * ctx->h, nr = (size_t)in_width * in_height;
+    if (int r = checkFormatWidth(ctx, ctx->inputFormat, in_width)) return r;
+    const size_t n = (size_t)ctx->w * ctx->h, nr = (size_t)in_width * in_height * pixBytes(ctx->inputFormat);
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
     releaseUndistorter(ctx);
     if (!remapX || !remapY) {
@@ -516,7 +556,7 @@ extern "C" int lsdgpu_set_undistorter(lsdgpu_ctx* ctx, int in_width, int in_heig
 static int uploadRaw(lsdgpu_ctx* ctx, const uint8_t* raw)
 {
     if (!ctx->undistorterSet) return lsd_fail(ctx, "no undistorter installed (lsdgpu_set_undistorter)");
-    const size_t nr = (size_t)ctx->rawW * ctx->rawH;
+    const size_t nr = rawBytes(ctx);
     cudaPointerAttributes pa;
     const bool pinned = cudaPointerGetAttributes(&pa, raw) == cudaSuccess && pa.type == cudaMemoryTypeHost;
     if (!pinned) {
@@ -528,26 +568,89 @@ static int uploadRaw(lsdgpu_ctx* ctx, const uint8_t* raw)
     return 0;
 }
 
+// cvtColor (the input format) + the installed undistorter from the raw image in ctx->dRaw to the w x h gray image `out` (device)
+static int undistortStaged(lsdgpu_ctx* ctx, uint8_t* out)
+{
+    const int n = ctx->w * ctx->h, fmt = ctx->inputFormat, pitch = ctx->rawW * pixBytes(fmt);
+    if (!ctx->dRemapX && !ctx->dCvMap1 && fmt == LSDGPU_PIX_MONO8) {  // result = image, Undistorter.cpp:370-375
+        LSD_CHECK(ctx, cudaMemcpyAsync(out, ctx->dRaw, n, cudaMemcpyDeviceToDevice, ctx->stream));
+        return 0;
+    }
+    withFormat(fmt, [&](auto f) {
+        constexpr int F = decltype(f)::value;
+        if (ctx->dCvMap1)
+            k_undistort_opencv<F><<<divUp(n, 256), 256, 0, ctx->stream>>>(ctx->dRaw, ctx->rawW, ctx->rawH, ctx->dCvMap1, ctx->dCvMap2, n, out);
+        else if (ctx->dRemapX)
+            k_undistort<F><<<divUp(n, 256), 256, 0, ctx->stream>>>(ctx->dRaw, pitch, ctx->dRemapX, ctx->dRemapY, n, out);
+        else
+            k_to_gray<F><<<divUp(n, 256), 256, 0, ctx->stream>>>(ctx->dRaw, pitch, ctx->w, n, out);
+    });
+    LAUNCH(ctx);
+    LSD_CHECK(ctx, cudaGetLastError());
+    return 0;
+}
+
 extern "C" int lsdgpu_undistort_u8(lsdgpu_ctx* ctx, const uint8_t* raw, uint8_t* out)
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     int r = uploadRaw(ctx, raw);
     if (r) return r;
     const int n = ctx->w * ctx->h;
-    if (!ctx->dRemapX && !ctx->dCvMap1) {                             // result = image, Undistorter.cpp:370-375
+    if (!ctx->dRemapX && !ctx->dCvMap1 && ctx->inputFormat == LSDGPU_PIX_MONO8) {   // result = image, Undistorter.cpp:370-375
         LSD_CHECK(ctx, cudaMemcpyAsync(out, ctx->dRaw, n, cudaMemcpyDeviceToHost, ctx->stream));
     } else {
         uint8_t* dOut = ctx->dStageU8[ctx->stageIdx];
         LSD_CHECK(ctx, cudaEventSynchronize(ctx->stageDone[ctx->stageIdx]));
-        if (ctx->dCvMap1)
-            k_undistort_opencv<<<divUp(n, 256), 256, 0, ctx->stream>>>(ctx->dRaw, ctx->rawW, ctx->rawH, ctx->dCvMap1, ctx->dCvMap2, n, dOut);
-        else
-            k_undistort<<<divUp(n, 256), 256, 0, ctx->stream>>>(ctx->dRaw, ctx->rawW, ctx->dRemapX, ctx->dRemapY, n, dOut);
-        LAUNCH(ctx);
-        LSD_CHECK(ctx, cudaGetLastError());
+        if ((r = undistortStaged(ctx, dOut))) return r;
         LSD_CHECK(ctx, cudaMemcpyAsync(out, dOut, n, cudaMemcpyDeviceToHost, ctx->stream));
     }
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+extern "C" int lsdgpu_set_input_format(lsdgpu_ctx* ctx, int format)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    if (format < LSDGPU_PIX_MONO8 || format > LSDGPU_PIX_YUV422_YUY2) return lsd_fail(ctx, "unknown input format");
+    if (!ctx->undistorterSet) return lsd_fail(ctx, "no undistorter installed (lsdgpu_set_undistorter)");
+    if (int r = checkFormatWidth(ctx, format, ctx->rawW)) return r;
+    if (format == ctx->inputFormat) return 0;
+    const size_t nr = (size_t)ctx->rawW * ctx->rawH * pixBytes(format);
+    LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));                // the staging of the old format may still be in use
+    cudaFree(ctx->dRaw); ctx->dRaw = nullptr;
+    cudaFreeHost(ctx->hRaw); ctx->hRaw = nullptr;
+    ctx->undistorterSet = false;                                       // until the staging of the new format exists
+    LSD_CHECK(ctx, cudaMalloc((void**)&ctx->dRaw, nr));
+    LSD_CHECK(ctx, cudaHostAlloc((void**)&ctx->hRaw, nr, cudaHostAllocDefault));
+    ctx->inputFormat = format;
+    ctx->undistorterSet = true;
+    return 0;
+}
+
+extern "C" int lsdgpu_stage_put_raw(lsdgpu_ctx* ctx, int index, const uint8_t* raw)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    if (index < 0 || index >= ctx->stageEntries) return lsd_fail(ctx, "bad ring index");
+    int r = uploadRaw(ctx, raw);
+    if (r || (r = undistortStaged(ctx, ctx->stageRing + (size_t)index * ctx->w * ctx->h))) return r;
+    LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+extern "C" int lsdgpu_stage_put_raw_device(lsdgpu_ctx* ctx, int index, const uint8_t* d_raw, size_t pitch, void* stream)
+{ LSD_LOCK(ctx);
+    LSD_CHECK(ctx, cudaSetDevice(ctx->device));
+    if (index < 0 || index >= ctx->stageEntries) return lsd_fail(ctx, "bad ring index");
+    if (!ctx->undistorterSet) return lsd_fail(ctx, "no undistorter installed (lsdgpu_set_undistorter)");
+    const int row = ctx->rawW * pixBytes(ctx->inputFormat);
+    int r = checkDeviceImage(ctx, "stage_put_raw_device", d_raw, pitch, row, ctx->rawH);
+    if (r) return r;
+    LSD_CHECK(ctx, afterCallerStream(ctx, stream));
+    // into the raw staging first (one device-to-device copy, stream-ordered like the host uploads into it), so that both routes
+    // run the same kernels on the same tightly packed image
+    LSD_CHECK(ctx, cudaMemcpy2DAsync(ctx->dRaw, row, d_raw, pitch, row, ctx->rawH, cudaMemcpyDeviceToDevice, ctx->stream));
+    if ((r = undistortStaged(ctx, ctx->stageRing + (size_t)index * ctx->w * ctx->h))) return r;
+    LSD_CHECK(ctx, beforeCallerStream(ctx, stream));
     return 0;
 }
 
@@ -558,19 +661,21 @@ extern "C" int lsdgpu_frame_upload_distorted_u8(lsdgpu_ctx* ctx, int frame_id, c
     if (!s) return failMissing(ctx, frame_id, "no free frame slot (release frames or raise max_frames)");
     int r = uploadRaw(ctx, raw);
     if (r) return r;
-    return buildFrameFromDeviceU8(ctx, s, ctx->dRaw, ctx->rawW, ctx->dCvMap1 ? PYR_OPENCV : ctx->dRemapX ? PYR_PTAM : PYR_U8);
+    return buildFrameFromDeviceU8(ctx, s, ctx->dRaw, ctx->rawW * pixBytes(ctx->inputFormat), ctx->dCvMap1 ? PYR_OPENCV : ctx->dRemapX ? PYR_PTAM : PYR_U8,
+                                  ctx->inputFormat);
 }
 
 extern "C" int lsdgpu_frame_upload_distorted_device_u8(lsdgpu_ctx* ctx, int frame_id, const uint8_t* d_raw, size_t pitch, void* stream)
 { LSD_LOCK(ctx);
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     if (!ctx->undistorterSet) return lsd_fail(ctx, "no undistorter installed (lsdgpu_set_undistorter)");
-    int r = checkDeviceImage(ctx, "frame_upload_distorted_device_u8", d_raw, pitch, ctx->rawW, ctx->rawH);
+    int r = checkDeviceImage(ctx, "frame_upload_distorted_device_u8", d_raw, pitch, ctx->rawW * pixBytes(ctx->inputFormat), ctx->rawH);
     if (r) return r;
     FrameSlot* s = acquireSlot(ctx, frame_id);
     if (!s) return failMissing(ctx, frame_id, "no free frame slot (release frames or raise max_frames)");
     LSD_CHECK(ctx, afterCallerStream(ctx, stream));
-    if ((r = buildFrameFromDeviceU8(ctx, s, d_raw, (int)pitch, ctx->dCvMap1 ? PYR_OPENCV : ctx->dRemapX ? PYR_PTAM : PYR_U8))) return r;
+    if ((r = buildFrameFromDeviceU8(ctx, s, d_raw, (int)pitch, ctx->dCvMap1 ? PYR_OPENCV : ctx->dRemapX ? PYR_PTAM : PYR_U8, ctx->inputFormat)))
+        return r;
     LSD_CHECK(ctx, beforeCallerStream(ctx, stream));
     return 0;
 }
@@ -695,7 +800,8 @@ extern "C" int lsdgpu_set_undistorter_opencv(lsdgpu_ctx* ctx, int in_width, int 
     LSD_CHECK(ctx, cudaSetDevice(ctx->device));
     if (in_width <= 0 || in_height <= 0) return lsd_fail(ctx, "bad input size");
     if (!map1 || !map2) return lsd_fail(ctx, "UndistorterOpenCV needs both maps");
-    const size_t n = (size_t)ctx->w * ctx->h, nr = (size_t)in_width * in_height;
+    if (int r = checkFormatWidth(ctx, ctx->inputFormat, in_width)) return r;
+    const size_t n = (size_t)ctx->w * ctx->h, nr = (size_t)in_width * in_height * pixBytes(ctx->inputFormat);
     LSD_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
     releaseUndistorter(ctx);
     LSD_CHECK(ctx, cudaMalloc((void**)&ctx->dCvMap1, n * sizeof(short2)));

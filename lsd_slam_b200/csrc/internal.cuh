@@ -182,6 +182,7 @@ struct lsdgpu_ctx {
     uint8_t* hRaw = nullptr;
     int rawW = 0, rawH = 0;
     bool undistorterSet = false;
+    int inputFormat = LSDGPU_PIX_MONO8;  // pixel format of the raw images (lsdgpu_set_input_format); kept across undistorter installs
     uint32_t* dPacked = nullptr;         // keyframeMsg.pointcloud staging: w*h InputPointDense records (device)
     int trackGrid = 132;                 // launch shape of the persistent tracker (set by trackPersistentSetup): one CTA per SM
     unsigned int* trkSync = nullptr;     // barrier counters + cross-GPU exchange slots of the persistent tracker (TP_SYNC_WORDS)

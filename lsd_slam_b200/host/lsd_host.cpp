@@ -108,6 +108,7 @@ void DeviceContext::check(int rc, const char* where) const
 {
     if (rc != 0) throw LsdGpuError(std::string(where) + ": " + lsdgpu_last_error(ctx_));
 }
+void DeviceContext::setInputFormat(int format) { check(lsdgpu_set_input_format(ctx_, format), "DeviceContext::setInputFormat"); }
 void DeviceContext::followGlobals()
 {
     lsdgpu_globals want, have;

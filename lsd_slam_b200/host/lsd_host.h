@@ -148,6 +148,12 @@ public:
     int maxFrames() const { return maxFrames_; }
     // bound of pruneActiveFrames: maxLoopClosureCandidates + 20 (util/settings.cpp:97)
     FrameMemory& frameMemory() { return *memory_; }
+    // the pixel format (LSDGPU_PIX_*) of the installed undistorter's raw images: Frame(.., image, /*distorted=*/true) and
+    // Undistorter::undistort then take colour or 4:2:2 camera images and convert them on the device as cv::cvtColor does
+    // (LiveSLAMWrapper.cpp:116-121: newImageCallback's cvtColor(img, grayImg, CV_RGB2GRAY) becomes
+    // dev.setInputFormat(img.channels() == 1 ? LSDGPU_PIX_MONO8 : img.channels() == 3 ? LSDGPU_PIX_RGB8 : LSDGPU_PIX_RGBA8)).
+    // Needs an installed undistorter; lsdgpu_set_input_format.
+    void setInputFormat(int format);
 
 private:
     lsdgpu_ctx* ctx_ = nullptr;
